@@ -14,8 +14,10 @@ stereo/mono partial mixes are summed with one NCCL reduce per step (SURVEY.md §
 import argparse
 import json
 import os
+import shutil
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -23,13 +25,21 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 for p in (ROOT, os.path.join(ROOT, "tests")):
     if p not in sys.path:
         sys.path.insert(0, p)
+_SCRATCH = []
+
+
+def scratch():
+    """This run's temporary directory (removed when the run ends)."""
+    if not _SCRATCH:
+        _SCRATCH.append(tempfile.mkdtemp(prefix="fdsp_bench_"))
+    return _SCRATCH[0]
 
 SR = 48000.0
 def _baseline_metric():
     try:
         return json.load(open(os.path.join(ROOT, "BASELINE.json")))["metric"]
     except Exception:
-        return "Msamples/sec (f32) rendered across N voices at 1/2/4/8 B200 vs host-CPU ref"
+        return "Msamples/sec (f32) rendered across N voices at 1/2/4/8 H100 vs host-CPU ref"
 
 
 METRIC = _baseline_metric()   # the metric string of BASELINE.json, verbatim
@@ -47,11 +57,14 @@ def parse():
     ap.add_argument("--seconds", type=float, default=1.0, help="audio seconds rendered per step")
     ap.add_argument("--per-voice", action="store_true", help="also materialise per-voice outputs in HBM (value only)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"], help="weak: --voices per GPU (default); strong: the config's voices split over the GPUs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32): mix.npy [channels][samples] and, with --per-voice, "
+                         "voices.npy = a fixed seeded sample of the per-voice rows with their row indices in voice_rows.npy (float64)")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -109,10 +122,10 @@ def host_cores():
 
 def native_oracle():
     """The timed CPU arm runs the oracle built for THIS host (-march=native, as BASELINE.md §3 states); the parity tests keep the
-    portable x86-64-v3 build. Built once per box next to the portable one; falls back to it if the compiler is missing."""
-    so = os.path.join(ROOT, "oracle", "_build", "libfundsp_oracle_native.so")
+    portable x86-64-v3 build. Built per run in a temporary directory; falls back to the portable build if the compiler is missing."""
+    so = os.path.join(scratch(), "libfundsp_oracle_native.so")
     try:
-        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "native"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL, timeout=600)
+        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "native", "NATIVE=" + so], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL, timeout=600)
         if os.path.exists(so):
             os.environ["FDSP_ORACLE_SO"] = so
             return "g++ -O3 -march=native -ffp-contract=off"
@@ -184,7 +197,7 @@ def job_config(a, world, channels):
     return {"workload": workload_name(a.workload, V0), "voices_per_gpu": per, "voices_total": total, "sample_rate": SR, "block": 64, "seconds_per_step": a.seconds,
             "output": "mix-down to %d channel(s)%s" % (channels, " + per-voice rows in HBM" if a.per_voice else ""),
             "parallelism": "voices sharded x%d, one mix-down per step below the C ABI (NCCL send/recv gather over NVLink + rank-order fold)" % world if world > 1 else "1 GPU",
-            "l2": "flushed between timed steps (512 MB write)"}
+            "l2": "flushed between timed steps (512 MB write)", "state": "reset before the timed steps"}
 
 
 def workload_name(w, V):
@@ -197,6 +210,21 @@ def workload_name(w, V):
     return names[w]
 
 
+def dump_outputs(d, mix, out, max_bytes=64_000_000):
+    """The arrays the timed device path hands its caller: the mix, and a fixed seeded sample of the per-voice rows (at most `max_bytes` in all)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    m = mix.float().cpu().numpy()
+    np.save(os.path.join(d, "mix.npy"), m)
+    if out is not None:
+        rows_fit = max(0, (max_bytes - m.nbytes - 3 * 4096) // (out.shape[1] * 4 + 8))   # (4096: room for each file's .npy header)
+        k = min(out.shape[0], rows_fit)
+        rows = np.sort(np.random.default_rng(0).choice(out.shape[0], size=k, replace=False))
+        np.save(os.path.join(d, "voices.npy"), out[torch.from_numpy(rows).to(out.device)].float().cpu().numpy())
+        np.save(os.path.join(d, "voice_rows.npy"), rows.astype(np.float64))
+
+
 def main():
     a = parse()
     if a.impl == "reference":
@@ -205,6 +233,13 @@ def main():
     import numpy as np
     import torch
 
+    # NVRTC units compiled at run time go to a private copy of the on-disk JIT cache, not into the tree
+    if not os.environ.get("FDSP_JIT_CACHE"):
+        cache = os.path.join(scratch(), "jit_cache")
+        src = os.path.join(ROOT, "fundsp_b200", "jit_cache")
+        if os.path.isdir(src):
+            shutil.copytree(src, cache)
+        os.environ["FDSP_JIT_CACHE"] = cache
     from fundsp_b200 import workloads
     from fundsp_b200.bank import GpuBank
 
@@ -239,7 +274,7 @@ def main():
     mix = torch.zeros((c, n), device="cuda", dtype=torch.float32)
     out = torch.empty((V * c, n), device="cuda", dtype=torch.float32) if a.per_voice else None
     gin = torch.from_numpy(gate).cuda() if gate is not None else None
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     host_mix = torch.empty((c, n), dtype=torch.float32).pin_memory()
     host_in = torch.from_numpy(gate).pin_memory() if gate is not None else None
 
@@ -301,8 +336,13 @@ def main():
     for _ in range(int(extra.item())):
         device_step()
         e2e_step()
+    # the timed steps render the first K steps of audio from the reset state: the same arguments give the same outputs on every run,
+    # whatever the number of warm-up steps
+    bank.reset()
     launches0 = bank.launch_count()
     ms_step, ms_kernel, wall = timed(device_step, a.steps)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, mix, out)
     ms_dom = timed.dominant_ms      # the dominant kernel alone (CUDA events on the stream it is launched on, inside the bank)
     if not ms_dom > 0.0:            # FDSP_NO_DOM=1 (the A/B switch of those event records): fall back on the whole device region
         ms_dom = ms_kernel
@@ -338,7 +378,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))   # fallback: the H100 SXM data-sheet HBM3 bandwidth
     cls = bank.classes()
     state_b = sum(k["voices"] * (2 * k["state_words"] + k["param_words"]) * 4 for k in cls)
     nlaunch_chunks = (n + 16383) // 16384
@@ -352,34 +392,18 @@ def main():
         roof_extra = {"dry_stage": "the stage-pipelined voice program (Moog ladder in its own warp) runs beside it on the other stream and is the longer of the two: "
                                    "kernel_ms_all_per_step - kernel_ms_per_step is what it adds"}
     if a.workload == "conv":
-        # the tensor-core tiles: issued = 3 (3xTF32) x 2 x V(padded to 128) x n(padded to 128 per 16384-chunk) x (128 + P, padded to 32) flops
-        kernel_name, bound, unit = "fdsp::conv_tc_kernel<4>", "tensor", "TFLOP/s"
+        # the tensor-core tiles: issued = 3 (3xTF32) x 2 x V(padded to 128) x n(padded to 64 per 16384-chunk) x (64 + P, padded to 32) flops
+        kernel_name, bound, unit = "fdsp::conv_tc_kernel", "tensor", "TFLOP/s"
         K = 1000
-        J = (128 + ((K - 1 + 3) // 4 * 4) + 31) // 32 * 32
-        npad = sum(((min(16384, n - t0) + 127) // 128) * 128 for t0 in range(0, n, 16384))
+        J = (64 + ((K - 1 + 3) // 4 * 4) + 31) // 32 * 32
+        npad = sum(((min(16384, n - t0) + 63) // 64) * 64 for t0 in range(0, n, 16384))
         flops = 3 * 2.0 * ((V + 127) // 128 * 128) * npad * J
-        peak = float(peaks.get("bf16_tflops", 1720.0)) / 2.0
+        peak = float(peaks.get("bf16_tflops", 989.0)) / 2.0   # fallback: the H100 SXM data-sheet dense BF16 rate
         achieved = flops / (ms_dom * 1e-3) / 1e12
         roof_extra = {"useful_tflops": 2.0 * V * n * K / (ms_dom * 1e-3) / 1e12, "issued_flops_per_step": flops,
-                      "peak_note": "TF32 dense = half of the measured BF16 dense rate of MEASURED_PEAKS.json (bf16_tflops / 2)"}
+                      "peak_note": "TF32 dense = half the dense BF16 rate (MEASURED_PEAKS.json bf16_tflops, else the H100 SXM data sheet's 989)"}
     else:
         achieved = bytes_step / (ms_dom * 1e-3) / 1e9
-    traffic = None
-    issue = None
-    try:
-        prof = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        t = prof.get(a.workload + ("+voices" if a.per_voice else ""))
-        # ncu dram bytes of one 16384-sample launch of the dominant kernel, scaled to the step
-        traffic = t["dram_bytes_per_launch"] * n / t["samples_per_launch"] if t else None
-        if t and t.get("warp_inst_per_launch") and V == HEADLINE[a.workload] and bound == "hbm":
-            # what actually bounds a voice program: warp-instructions issued (ncu count of one 16384-sample launch, scaled to the
-            # step) against 148 SMs x 4 schedulers x 1 instruction per clock at the SM clock sampled during the timed region
-            winst = t["warp_inst_per_launch"] * n / t["samples_per_launch"]
-            mhz = float(clocks.get("sm_mhz") or 1965.0)
-            issue = {"warp_inst_per_step": winst, "achieved_ginst_s": winst / (ms_dom * 1e-3) / 1e9, "peak_ginst_s": 592 * mhz * 1e6 / 1e9,
-                     "frac": winst / (ms_dom * 1e-3) / (592 * mhz * 1e6), "source": "profiles/r02_traffic.json (smsp__inst_executed.sum of one launch)"}
-    except Exception:
-        pass
     # ---- CPU baseline on this box's host cores (bounded sample of the same workload)
     # (timed at N=1 only; multi-GPU runs carry the object with value null — the reference arm `--impl reference` covers every N)
     cores, core_info = host_cores()
@@ -404,14 +428,14 @@ def main():
                 "call": "fdsp_bank_render(host buffers)" if world == 1 else "fdsp_bank_render_reduced(host buffers; D2H of the reduced mix on the root)", "ms_per_step": ms_e2e,
                 "process_granularity": {"value": proc_val, "unit": "Msamples/s", "us_per_call": t_p / pb * 1e6, "call": "fdsp_bank_process(64) per block, host buffers"}},
         "gpu_launches": launches,
-        "roofline": {"bound": bound, "achieved": achieved, "peak": peak, "unit": unit, "frac": achieved / peak, "traffic": traffic,
+        "roofline": {"bound": bound, "achieved": achieved, "peak": peak, "unit": unit, "frac": achieved / peak,
                      "kernel": kernel_name, "kernel_ms_per_step": ms_dom, "kernel_ms_all_per_step": ms_kernel, "algorithmic_bytes_per_step": int(bytes_step), **roof_extra,
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 GB/s (of fallback)", "issue": issue,
-                     "note": "IIR voice programs are issue/latency bound, not HBM bound (DESIGN.md §Roofline); see profiles/ for issue-slot utilisation"},
+                     "peak_source": "MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet",
+                     "note": "IIR voice programs are issue/latency bound, not HBM bound (DESIGN.md §Roofline)"},
         "cpu_baseline": {"value": cpu_val, "unit": "Msamples/s", "cores": cores, "kind": "port", "single_core": per_core, "core_info": core_info,
                          "sample": (f"{Vc} voices x {ns} samples, oracle (C++ restatement of the reference block path; {build}), {cores} threads" if world == 1
                                     else "not timed at N > 1 (see the N=1 line and the --impl reference arm)")},
-        "clocks": clocks,
+        "gpu": torch.cuda.get_device_name(local), "clocks": clocks,
         "wall_s_timed_region": wall,
     }
     print(json.dumps(line))
@@ -420,4 +444,9 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    sys.dont_write_bytecode = True   # the tree may be read-only: nothing is written there (compiled or cached files go to scratch())
+    try:
+        main()
+    finally:
+        for d in _SCRATCH:
+            shutil.rmtree(d, ignore_errors=True)

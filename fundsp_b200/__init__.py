@@ -1,7 +1,7 @@
-"""fundsp_b200 — B200-native block-processing engine for FunDSP's voice-bank hot path.
+"""fundsp_b200 — H100-native block-processing engine for FunDSP's voice-bank hot path.
 
 `prelude` mirrors the reference's opcode vocabulary, `graph.An` its operators; `GpuBank` evaluates V voice
-instances on the GPU through the C ABI in include/fundsp_b200.h (libfundsp_b200.so, hand-written sm_100a CUDA).
+instances on the GPU through the C ABI in include/fundsp_b200.h (libfundsp_b200.so, hand-written sm_90a CUDA).
 """
 from . import prelude  # noqa: F401
 from .graph import An, ArityError  # noqa: F401

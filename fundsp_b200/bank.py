@@ -1,4 +1,4 @@
-"""GpuBank: V voice instances of FunDSP graphs evaluated in lockstep on one B200.
+"""GpuBank: V voice instances of FunDSP graphs evaluated in lockstep on one H100.
 
 To the host it is one `AudioUnit` (reference src/audiounit.rs:21-95) with `inputs()` shared bus inputs
 and either 2-ish mixed outputs (`mix=True`) or `V * channels` per-voice outputs: `process` is

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI (include/fundsp_b200.h) exported by fundsp_b200/libfundsp_b200.so.
 
-The library is hand-written CUDA for sm_100a plus its host runtime; there is no CPU fallback: if the
+The library is hand-written CUDA for sm_90a plus its host runtime; there is no CPU fallback: if the
 shared object is missing or no CUDA device is usable the product path raises `FdspError`.
 """
 from __future__ import annotations

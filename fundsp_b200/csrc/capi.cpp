@@ -42,7 +42,7 @@ int status(const std::string& e, int untagged = FDSP_ERR_CUDA) {
 
 #define API extern "C" __attribute__((visibility("default")))
 
-API const char* fdsp_version(void) { return "fundsp_b200 0.1.0 (sm_100a; mirrors fundsp 0.23.0 hot path)"; }
+API const char* fdsp_version(void) { return "fundsp_b200 0.1.0 (sm_90a; mirrors fundsp 0.23.0 hot path)"; }
 API const char* fdsp_last_error(void) { return g_err.c_str(); }
 API int fdsp_device_count(void) { int n = 0; return cudaGetDeviceCount(&n) == cudaSuccess ? n : 0; }
 

@@ -27,12 +27,12 @@ struct WaveTableDev {
 FDSP_HDC constexpr int mix_tile_samples(int outs) { return outs <= 1 ? 64 : (outs == 2 ? 32 : (outs <= 4 ? 16 : 8)); }
 FDSP_HDC constexpr size_t mix_tile_floats(int outs, int nt) { return (size_t)outs * (size_t)mix_tile_samples(outs) * (size_t)(nt + 1); }
 
-// CTA shape of a class of V voices with NT threads per CTA: enough CTAs to cover the voices, rounded up to whole waves of the
-// 148 SMs once every CTA can still have a full warp, and the voices spread evenly over them (a bank is bound by per-SM
+// CTA shape of a class of V voices with NT threads per CTA on a device of `sms` SMs: enough CTAs to cover the voices, rounded up to
+// whole waves of the SMs once every CTA can still have a full warp, and the voices spread evenly over them (a bank is bound by per-SM
 // pipes and per-warp latency, so idle SMs are the first thing to use up).
-inline uint32_t bank_grid(uint32_t V, uint32_t nt, uint32_t* vpc) {
+inline uint32_t bank_grid(uint32_t V, uint32_t nt, uint32_t sms, uint32_t* vpc) {
   uint32_t grid = (V + nt - 1) / nt;
-  if (V >= 148u * 32u) grid = (grid + 147u) / 148u * 148u;
+  if (V >= sms * 32u) grid = (grid + sms - 1u) / sms * sms;
   if (grid == 0) grid = 1;
   *vpc = (V + grid - 1) / grid;
   return (V + *vpc - 1) / *vpc;

@@ -1,7 +1,6 @@
 // Resident form of the voice-bank kernel for the `AudioUnit::process` call pattern (reference src/audiounit.rs:45, driven one 64-sample
 // block at a time by Wave::render src/wave.rs:452-462 or an audio callback): instead of one launch per block — parameters and state
-// reloaded, 161 KB of wavetables restaged, a launch and a stream synchronisation on the critical path (round 1: 31 us per block of the
-// 16384-voice headline bank) — ONE launch stays resident with every voice's state in registers and serves blocks on a doorbell:
+// reloaded, 161 KB of wavetables restaged, a launch and a stream synchronisation on the critical path — ONE launch stays resident with every voice's state in registers and serves blocks on a doorbell:
 //
 //   host: writes the block's inputs and size into a mapped, pinned control page, then the request's sequence number (the doorbell);
 //         spins on `done` in the same page; copies the mix out.
@@ -169,8 +168,8 @@ __global__ void __launch_bounds__(NT, FDSP_MIN_CTAS) bank_kernel_rt(const BankAr
     if (s_last) {
       __threadfence();
       // CTA-order left fold of the partials (= mix_reduce_kernel, bit for bit). The loads of 8 CTAs are issued together, the adds stay in
-      // order. (A version that staged the partials in shared memory first measured SLOWER — 44.5 vs 23.4 us per block at 148 CTAs: one CTA
-      // cannot keep enough loads in flight to win back the extra pass.)
+      // order. (A version that staged the partials in shared memory first was slower: one CTA cannot keep enough loads in flight to win
+      // back the extra pass.)
       for (uint32_t e = tid; e < (uint32_t)OUT * (uint32_t)nb; e += NT) {
         const uint32_t ch = e / (uint32_t)nb, t = e - ch * (uint32_t)nb;
         const float* p0 = a.partial + (size_t)ch * 64 + t;

@@ -2,7 +2,7 @@
 // the CTA and hand 16-sample slots over through shared memory (mbarrier full / empty pairs per warp and slot).
 //
 // Why: a voice is a serial recurrence and a small bank has far fewer voice-warps than the GPU has warp schedulers (config 4:
-// 1024 voices = 32 warps on 592 schedulers), so the plain kernel (bank_kernel.cuh) runs at the dependency latency of the WHOLE
+// 1024 voices = 32 warps on 528 schedulers of an H100), so the plain kernel (bank_kernel.cuh) runs at the dependency latency of the WHOLE
 // program — oscillator, ladder filter, envelope and pan back to back in one thread (round 1: 258 instructions per sample at
 // 0.3 IPC). Only the Moog ladder (src/moog.rs:81-100, tanh in the loop) is a true per-sample recurrence; everything in front
 // of it and behind it is time-parallel work that merely has to be READY. Cutting the program at the heavy leaf gives the

@@ -16,9 +16,8 @@
 //     17 warp-instructions per block, lanes cover (line, 16-byte chunk) pairs), three blocks in flight per warp;
 //   * the 64 new samples per line are produced in place in the same shared-memory rows and go back with 16-byte stores.
 //   (A first round-2 version moved every line's slice with its own `cp.async.bulk` — 64..96 TMA operations of 256 bytes per block
-//   and warp. It was bit-exact and no faster than round 1: 2.1 ms per 16384 samples, because the TMA unit serves about one
-//   operation per ~46 cycles per SM regardless of size, and 7 warps x 96 operations x 46 cycles is the whole block time. Bulk
-//   copies pay from about 1 KB up; a delay line hands out 256 contiguous bytes per block.)
+//   and warp. It was bit-exact and no faster than round 1, because the TMA unit serves bulk operations at a fixed cost each regardless
+//   of size. Bulk copies pay from about 1 KB up; a delay line hands out 256 contiguous bytes per block.)
 // Ring storage (private to this kernel; the host only sizes, clears and copies it): voice-major [voice][line][ring], each
 // line's ring padded to a multiple of 64 floats (`fdn_ring_phys`) so that block-aligned slices are 16-byte aligned and a
 // block of new samples never straddles the end. The state word of a line holds its WRITE position w; the sample written at w is read

@@ -1,4 +1,4 @@
-// fundsp_b200 device math substrate (sm_100a). Hand-written for the voice-bank kernels.
+// fundsp_b200 device math substrate (sm_90a). Hand-written for the voice-bank kernels.
 //
 // Numeric contract (DESIGN.md §"Arithmetic"): every f32 operation is an individually rounded IEEE
 // operation in the order the reference writes it (the reference is Rust: no a*b+c contraction), so this

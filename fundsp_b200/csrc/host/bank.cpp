@@ -773,27 +773,33 @@ std::string Bank::reset() {  // AudioUnit::reset: back to the construction-time 
 // (process()-sized) read the tables through L1/L2 instead
 static size_t table_bytes_of(const VoiceClass& c, uint32_t len) {
   const int wk = c.k ? c.k->wave_kind : -1;
-  static const uint32_t tb_min = [] { const char* e = getenv("FDSP_TB_MIN"); return e ? (uint32_t)atoi(e) : 32u; }();  // measured: at 64 samples the TMA-staged tables already win (35.0 vs 38.9 us per process call)
+  static const uint32_t tb_min = [] { const char* e = getenv("FDSP_TB_MIN"); return e ? (uint32_t)atoi(e) : 32u; }();  // at 64 samples the TMA-staged tables already win
   return (wk >= 0 && len >= tb_min) ? device_wavetable(wk).data.size() * sizeof(float) : 0;
+}
+// SMs of a device (the CTA shapes below are sized by it)
+static uint32_t sm_count(int device) {
+  static uint32_t n[64] = {};
+  if (device < 0 || device >= 64) device = 0;
+  if (!n[device]) { int v = 0; n[device] = cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && v > 0 ? (uint32_t)v : 1u; }
+  return n[device];
 }
 // Stage-pipelined kernels (dsp/bank_kernel_st.cuh): programs with a heavy serial leaf (Moog ...) run their stages in different warps.
 // Used for launches long enough to fill the pipeline and for classes too small to give every warp scheduler a voice-warp of its own
-// (V <= 148 SMs x 32: measured on B200, the 1024-voice config-4 dry program 6.93 -> 4.60 ms per 16384 samples staged, the 16384-voice
-// saw >> moog >> pan class of config 5 6.35 -> 10.75 ms: with a warp per scheduler already, stages only add hand-off work).
+// (V <= SMs x 32: with a warp per scheduler already, stages only add hand-off work).
 // FDSP_STAGED=0 switches them off (A/B), FDSP_STAGED_MAXV moves the class-size bound.
-static bool use_staged(const Program* k, uint32_t V, uint32_t len) {
+static bool use_staged(const Program* k, uint32_t V, uint32_t len, uint32_t sms) {
   const char* e = getenv("FDSP_STAGED");            // read per call: the tests toggle it inside one process
   const char* m = getenv("FDSP_STAGED_MAXV");
   const int on = e ? atoi(e) : 1;
-  const uint32_t maxv = m ? (uint32_t)atoi(m) : 148u * 32u;
+  const uint32_t maxv = m ? (uint32_t)atoi(m) : sms * 32u;
   return on != 0 && k && k->stages >= 2 && len >= 256u && V <= maxv;
 }
 // CTA shape of a stage-pipelined class: 32 voices per CTA while that still leaves SMs free, else 128 with the voices spread evenly
 // (FDSP_STAGED_W=128 forces the wide shape: lets the tests reach it with few voices)
-static uint32_t staged_grid(uint32_t V, uint32_t* vpc) {
+static uint32_t staged_grid(uint32_t V, uint32_t sms, uint32_t* vpc) {
   const char* w = getenv("FDSP_STAGED_W");
-  if (V <= 148u * 32u && !(w && atoi(w) == 128)) { *vpc = 32u; return (V + 31u) / 32u; }
-  return bank_grid(V, 128u, vpc);
+  if (V <= sms * 32u && !(w && atoi(w) == 128)) { *vpc = 32u; return (V + 31u) / 32u; }
+  return bank_grid(V, 128u, sms, vpc);
 }
 
 // ---- resident process() kernel
@@ -828,8 +834,8 @@ std::string Bank::rt_process(uint32_t size, const float* in, float* out, bool* s
   VoiceClass& c = classes[0];
   if (c.fdn || c.conv || !c.k || !c.k->has_rt) return "";
   uint32_t vpc = (uint32_t)c.k->threads;
-  const uint32_t grid = bank_grid(c.V(), (uint32_t)c.k->threads, &vpc);
-  if (grid > 148u) return "";                       // every CTA must be resident at once
+  const uint32_t grid = bank_grid(c.V(), (uint32_t)c.k->threads, sm_count(device), &vpc);
+  if (grid > sm_count(device)) return "";           // every CTA must be resident at once
   if (++process_streak < 3u && !rt_running) return "";   // a bank that is driven block by block: the third process() call in a row starts the kernel
   if (!rt_running) { std::string re = rt_stop(); if (!re.empty()) return re; }   // (another bank of this device may own the resident slot)
   if (!rt_ctl) {
@@ -971,8 +977,8 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
     bool concurrent = classes.size() > 1 && !pipelined && len > 64 && !getenv("FDSP_NO_CONCURRENT");
     for (auto& c : classes) concurrent = concurrent && !c.fdn;
     if (concurrent) CU(cudaEventRecord(e_begin, stream));
-    // (Launching the class with the longest dependency chain first, on a high-priority stream, was measured on B200 and is WORSE for config 5:
-    // 26.4 ms per step against 22.9 in class order — its CTAs hold ~195 KB of shared memory, so every light class then waits for all of it.
+    // (Launching the class with the longest dependency chain first, on a high-priority stream, is worse for config 5 than class order:
+    // its CTAs hold ~195 KB of shared memory, so every light class then waits for all of it.
     // FDSP_HEAVY_FIRST=1 keeps that order for experiments; FDSP_CARVEOUT=<percent> makes every class kernel ask for the same carve-out.)
     std::vector<size_t> order(classes.size());
     for (size_t q = 0; q < order.size(); q++) order[q] = q;
@@ -980,7 +986,7 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
       std::stable_sort(order.begin(), order.end(), [&](size_t x, size_t y) { return (classes[x].k && classes[x].k->stages > 1) > (classes[y].k && classes[y].k->stages > 1); });
     struct CarveGuard { int saved; CarveGuard() : saved(launch_carveout()) {} ~CarveGuard() { launch_carveout() = saved; } } carve_guard;
     // Concurrent classes ask for ONE carve-out, the maximum: the class that stages the wavetables (~195 KB per CTA) needs it anyway, and kernels
-    // that prefer different L1 / shared-memory splits do not share an SM. Measured on B200, config 5 (bench step, 3 chunks): 22.87 -> 18.72 ms.
+    // that prefer different L1 / shared-memory splits do not share an SM.
     if (concurrent) { const char* cv = getenv("FDSP_CARVEOUT"); launch_carveout() = cv ? atoi(cv) : 100; }
     for (size_t oi = 0; oi < order.size(); oi++) {
       auto& c = classes[order[oi]];
@@ -991,20 +997,21 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
         ks = c.cstream;
         CU(cudaStreamWaitEvent(ks, e_begin, 0));
       }
-      const bool staged = use_staged(c.k.get(), V, len);
+      const uint32_t nsm = sm_count(device);
+      const bool staged = use_staged(c.k.get(), V, len, nsm);
       int fdn_warps = 1;   // voices (= warps) per CTA of the FDN kernel
       if (c.fdn) {
         const int cap = fdn_max_warps();
         // pipelined: leave SMs free for the CTAs of the dry stage of the next chunk (their shared-memory tables cannot share an SM
         // with an FDN CTA), otherwise the two stages serialise on SM residency
-        uint32_t sms = 148;
-        if (pipelined && c.k) { uint32_t dv = 0; const uint32_t dry_ctas = staged ? staged_grid(V, &dv) : (V + (uint32_t)c.k->threads - 1) / (uint32_t)c.k->threads; sms = dry_ctas < 74 ? 148 - dry_ctas : 74; }
+        uint32_t sms = nsm;
+        if (pipelined && c.k) { uint32_t dv = 0; const uint32_t dry_ctas = staged ? staged_grid(V, nsm, &dv) : (V + (uint32_t)c.k->threads - 1) / (uint32_t)c.k->threads; sms = dry_ctas < nsm / 2 ? nsm - dry_ctas : nsm / 2; }
         fdn_warps = (int)((V + sms - 1) / sms); if (fdn_warps > cap) fdn_warps = cap; if (fdn_warps < 1) fdn_warps = 1;
       }
       // voice programs: whole waves of CTAs with the voices spread evenly; the dry stage of a two-stage class stays compact
       // (few CTAs) so that it leaves the other SMs to the FDN kernel it is pipelined with
       uint32_t vpc = c.k ? (uint32_t)c.k->threads : 0u;
-      const uint32_t vgrid = !c.k ? 0u : (staged ? staged_grid(V, &vpc) : (c.fdn || getenv("FDSP_NO_SPREAD") ? (V + vpc - 1) / vpc : bank_grid(V, (uint32_t)c.k->threads, &vpc)));
+      const uint32_t vgrid = !c.k ? 0u : (staged ? staged_grid(V, nsm, &vpc) : (c.fdn || getenv("FDSP_NO_SPREAD") ? (V + vpc - 1) / vpc : bank_grid(V, (uint32_t)c.k->threads, nsm, &vpc)));
       auto launch_voice = [&](const BankArgs& args, int md, cudaStream_t st) { return staged ? c.k->launch_staged(args, md, table_bytes_of(c, len), st) : c.k->launch(args, md, table_bytes_of(c, len), st); };
       const uint32_t grid = c.fdn ? V : vgrid;   // rows of the partial-mix buffer: one per CTA of a voice program, one per VOICE of the FDN kernel (its warps never meet)
       if (c.conv) {
@@ -1124,7 +1131,8 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
         CU(cudaStreamWaitEvent(stream, c.e_done, 0));
         if (want_m) {
           uint32_t vpc = (uint32_t)c.k->threads;
-          const uint32_t grid = use_staged(c.k.get(), c.V(), len) ? staged_grid(c.V(), &vpc) : (getenv("FDSP_NO_SPREAD") ? (c.V() + vpc - 1) / vpc : bank_grid(c.V(), (uint32_t)c.k->threads, &vpc));
+          const uint32_t nsm = sm_count(device);
+          const uint32_t grid = use_staged(c.k.get(), c.V(), len, nsm) ? staged_grid(c.V(), nsm, &vpc) : (getenv("FDSP_NO_SPREAD") ? (c.V() + vpc - 1) / vpc : bank_grid(c.V(), (uint32_t)c.k->threads, nsm, &vpc));
           CU(launch_mix_reduce(c.d_partial, grid, (uint32_t)nout, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, first ? 0 : 1, stream));
           launches++;
         }

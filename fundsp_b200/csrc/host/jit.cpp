@@ -84,7 +84,7 @@ Api& api() {
 // ---- on-disk cache of compiled units. Key: FNV-1a of (NVRTC version, options, embedded headers, unit source, kernel expression), so
 // an entry can only be hit by the identical compilation. Directory: $FDSP_JIT_CACHE, else jit_cache/ next to this library (it travels
 // with the in-tree build; tools/warm_jit_cache.py fills it on a machine without a GPU). FDSP_JIT_CACHE=off disables it.
-static const char* kJitOpts[] = {"--gpu-architecture=sm_100a", "-std=c++17", "--fmad=false", "-lineinfo", "-default-device"};
+static const char* kJitOpts[] = {"--gpu-architecture=sm_90a", "-std=c++17", "--fmad=false", "-lineinfo", "-default-device"};
 static uint64_t fnv(uint64_t h, const void* p, size_t n) { const unsigned char* b = (const unsigned char*)p; for (size_t i = 0; i < n; i++) { h ^= b[i]; h *= 1099511628211ull; } return h; }
 static std::string cache_dir() {
   static const std::string dir = [] {

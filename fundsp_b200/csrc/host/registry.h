@@ -61,12 +61,12 @@ size_t tree_mix_scratch_floats(uint32_t V, uint32_t outs, uint32_t n);
 // warp-per-voice reverb_stereo kernel (inst/inst_fdn.cu)
 cudaError_t launch_fdn(const FdnArgs& a, int warps, cudaStream_t stream);
 int fdn_max_warps();
-// tensor-core convolve path (inst/inst_conv.cu, dsp/conv_tc_kernel.cuh): Y = X * Toeplitz(h) as 3xTF32 tcgen05 GEMM tiles
+// tensor-core convolve path (inst/inst_conv.cu, dsp/conv_tc_kernel.cuh): Y = X * Toeplitz(h) as 3xTF32 wgmma GEMM tiles
 struct ConvTcMaps { alignas(64) unsigned char m[4][128]; };   // four CUtensorMap objects: X, Xlo, T, Tlo
 cudaError_t conv_tc_make_maps(float* x, float* xl, uint32_t V, uint32_t row_stride, float* th, float* tl, uint32_t J, ConvTcMaps* out);
 cudaError_t launch_conv_tc(const ConvTcMaps& maps, float* y, uint32_t y_stride, uint32_t y_offset, const uint32_t* row_map, uint32_t V, uint32_t n, uint32_t K, uint32_t H,
                            cudaStream_t stream);
-cudaError_t launch_conv_split(const float* x, float* xl, uint32_t V, uint32_t row_stride, uint32_t col0, uint32_t n, cudaStream_t stream);
+cudaError_t launch_conv_split(float* x, float* xl, uint32_t V, uint32_t row_stride, uint32_t col0, uint32_t n, cudaStream_t stream);
 cudaError_t launch_conv_history(float* x, float* xl, uint32_t V, uint32_t row_stride, uint32_t H, uint32_t n, cudaStream_t stream);
 cudaError_t launch_conv_toeplitz(const float* h, uint32_t K, float* th, float* tl, uint32_t J, cudaStream_t stream);
 uint32_t conv_tc_toeplitz_cols(uint32_t K);

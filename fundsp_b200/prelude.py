@@ -1,7 +1,7 @@
 """Opcode vocabulary: the hot-path subset of the reference's `prelude32` (src/prelude.rs, F = f32).
 
 Every function returns an `An` expression and cites the reference constructor it mirrors
-(file:line relative to /root/reference).  Names, argument order and argument meaning follow the
+(file:line relative to the reference crate (SamiPerttu/fundsp v0.23.0)).  Names, argument order and argument meaning follow the
 reference; `pass` is spelled `pass_` (Python keyword).  Anything that needs a Rust closure
 (`envelope(|t| ..)`, `map`, `shape_fn`) cannot cross a C ABI and is intentionally absent;
 `adsr_live` is a closed-form opcode (src/adsr.rs:21-70).

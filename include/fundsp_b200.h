@@ -1,4 +1,4 @@
-/* fundsp_b200 — C ABI of the B200-native voice-bank engine (libfundsp_b200.so).
+/* fundsp_b200 — C ABI of the H100-native voice-bank engine (libfundsp_b200.so).
  *
  * Drop-in boundary for the hot path of SamiPerttu/fundsp v0.23.0: the reference has no FFI; the seam is
  * the Rust trait object `AudioUnit` (src/audiounit.rs:21-95). A Rust host keeps `AudioNode`/`AudioUnit`

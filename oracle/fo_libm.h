@@ -1,8 +1,8 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h).
 // Restatement of the scalar f32 libm functions the reference calls through the Rust `libm 0.2.15` crate
 // (src/lib.rs:168-223,444-518,773-798: f32::sin/cos/tan -> libm::sinf/cosf/tanf, f32::tanh -> libm::tanhf).
-// That crate is a port of musl libc's math library (FreeBSD msun lineage); its source is not under
-// /root/reference, so the published algorithms are restated here:
+// That crate is a port of musl libc's math library (FreeBSD msun lineage); its source is not in
+// the reference crate, so the published algorithms are restated here:
 //   sinf/cosf/tanf : k_sinf.c / k_cosf.c / k_tanf.c double-precision kernels + rem_pio2f "medium" reduction
 //   expm1f, tanhf  : s_expm1f.c / s_tanhf.c
 // PARITY UNPINNED at the ulp level against the real crate (no Rust toolchain here); tests pin these against

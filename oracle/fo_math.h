@@ -3,12 +3,12 @@
 // --impl reference legs may use it, and only as the checker / timed CPU baseline.
 //
 // CPU restatement of the scalar math substrate of SamiPerttu/fundsp v0.23.0.
-// Each function cites the reference file:line it follows (paths relative to /root/reference).
+// Each function cites the reference file:line it follows (paths relative to the reference crate (SamiPerttu/fundsp v0.23.0)).
 //
 // PARITY STATUS: integer paths (rnd1, AttoHash, hash32x) are fully in-repo in the reference and
 // are pinned bit-for-bit by the golden vectors in tests/golden/. Transcendentals are NOT pinned at
 // the ulp level: the reference calls the Rust `libm 0.2.15` crate (musl port) for scalars and
-// `wide 1.1.1` for the f32x8 block path; neither source is under /root/reference and no Rust
+// `wide 1.1.1` for the f32x8 block path; neither source is in the reference crate and no Rust
 // toolchain exists here. Scalars use glibc (<= 1 ulp from musl's, both are < 1 ulp functions);
 // `wide::f32x8::sin` is restated from its published algorithm (Agner Fog VCL sincos, Cephes
 // coefficients) below. "parity unpinned" at ulp level for sin/tan/tanh/exp and wavetable entries.

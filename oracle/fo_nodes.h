@@ -496,7 +496,7 @@ inline float optimal4x44(float a0, float a1, float a2, float a3, float x) {
 }
 
 // ---- src/wavetable.rs:40-242 Wavetable. The inverse FFT (`microfft 0.6.0`, src/fft.rs:51-100, not
-// under /root/reference) is replaced by the exact inverse DFT evaluated in f64:
+// in the reference crate) is replaced by the exact inverse DFT evaluated in f64:
 //   x.im[n] * N = sum_k re_k sin(2 pi k n / N) + im_k cos(2 pi k n / N)   (parity unpinned ~1e-7 of peak)
 struct Wavetable {
   std::vector<std::pair<float, std::vector<float>>> table;

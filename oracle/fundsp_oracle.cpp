@@ -2,7 +2,7 @@
 // that tests/ (ctypes) and bench.py's cpu_baseline leg can drive it. Handles are heap `fo::Node*`;
 // combinators CONSUME their children (like Rust move semantics); use fo_clone to reuse a node.
 //
-// Prelude composites restated here (paths relative to /root/reference):
+// Prelude composites restated here (paths relative to the reference crate (SamiPerttu/fundsp v0.23.0)):
 //   sine_hz  src/prelude.rs:349-351      saw_hz etc. src/prelude.rs:2051-2089
 //   fir3     src/prelude.rs:863-867      reverb_stereo src/prelude.rs:1732-1762
 //   moog_q   src/prelude.rs:559-561      Wave::render src/wave.rs:441-466, Wave::filter :518-565

@@ -1,13 +1,11 @@
 // Bring-up probe of the tensor-core convolver kernel (fundsp_b200/csrc/dsp/conv_tc_kernel.cuh), TEST INFRASTRUCTURE.
-// usage: conv_tc_probe STEP [K] [V] [n]   — runs the kernel built at bring-up level STEP (1 TMEM only, 2 + TMA, 3 + MMA, 4 full) on random
-// rows and, for STEP 4, compares with an f64 convolution. One level per process: a faulting level poisons the CUDA context.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O2 -std=c++17 -I fundsp_b200/csrc tests/cpp/conv_tc_probe.cu fundsp_b200/csrc/inst/inst_conv.cu -o tests/cpp/_probe/conv_tc_probe -lcuda
+// usage: conv_tc_probe [K] [V] [n]   — runs the kernel on random rows and compares with an f64 convolution.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O2 -std=c++17 -I fundsp_b200/csrc tests/cpp/conv_tc_probe.cu fundsp_b200/csrc/inst/inst_conv.cu -o tests/cpp/_probe/conv_tc_probe -lcuda
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
 
-#include "dsp/conv_tc_kernel.cuh"
 #include "host/registry.h"
 
 using namespace fdsp;
@@ -15,20 +13,8 @@ using namespace fdsp::host;
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("FAIL %s: %s\n", #x, cudaGetErrorString(e_)); return 1; } } while (0)
 
-template <int STEP> cudaError_t run(const ConvTcMaps& maps, const ConvTcArgs& a) {
-  const CUtensorMap* m = reinterpret_cast<const CUtensorMap*>(maps.m);
-  cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<STEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, CTC_SMEM);
-  if (e != cudaSuccess) return e;
-  dim3 grid((a.n + CTC_N - 1) / CTC_N, (a.V + CTC_M - 1) / CTC_M);
-  conv_tc_kernel<STEP><<<grid, 192, CTC_SMEM>>>(m[0], m[1], m[2], m[3], a);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return cudaDeviceSynchronize();
-}
-
 int main(int argc, char** argv) {
-  const int step = argc > 1 ? atoi(argv[1]) : 4;
-  const uint32_t K = argc > 2 ? atoi(argv[2]) : 100, V = argc > 3 ? atoi(argv[3]) : 200, n = argc > 4 ? atoi(argv[4]) : 300;
+  const uint32_t K = argc > 1 ? atoi(argv[1]) : 100, V = argc > 2 ? atoi(argv[2]) : 200, n = argc > 3 ? atoi(argv[3]) : 300;
   const uint32_t H = (K - 1 + 31) / 32 * 32 ? (K - 1 + 31) / 32 * 32 : 32, stride = H + 1024, J = conv_tc_toeplitz_cols(K);
   std::vector<float> x((size_t)V * stride, 0.0f), h(K);
   srand(1);
@@ -43,10 +29,10 @@ int main(int argc, char** argv) {
   CK(launch_conv_toeplitz(dh, K, dth, dtl, J, 0)); CK(launch_conv_split(dx, dxl, V, stride, H, n, 0)); CK(cudaDeviceSynchronize());
   ConvTcMaps maps;
   CK(conv_tc_make_maps(dx, dxl, V, stride, dth, dtl, J, &maps));
-  ConvTcArgs a{dy, 1024, 0, drow, V, n, K, H};
-  cudaError_t e = step == 1 ? run<1>(maps, a) : step == 2 ? run<2>(maps, a) : step == 3 ? run<3>(maps, a) : run<4>(maps, a);
-  printf("STEP %d K=%u V=%u n=%u: %s\n", step, K, V, n, cudaGetErrorString(e));
-  if (e != cudaSuccess || step < 4) return e != cudaSuccess;
+  cudaError_t e = launch_conv_tc(maps, dy, 1024, 0, drow, V, n, K, H, 0);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  printf("K=%u V=%u n=%u: %s\n", K, V, n, cudaGetErrorString(e));
+  if (e != cudaSuccess) return 1;
   std::vector<float> y((size_t)V * 1024);
   CK(cudaMemcpy(y.data(), dy, y.size() * 4, cudaMemcpyDeviceToHost));
   double worst = 0, peak = 0;

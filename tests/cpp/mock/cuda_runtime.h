@@ -15,12 +15,14 @@ typedef struct MockStream_* cudaStream_t;
 typedef struct MockEvent_* cudaEvent_t;
 enum cudaMemcpyKind { cudaMemcpyHostToHost = 0, cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3, cudaMemcpyDefault = 4 };
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaHostAllocMapped = 2 };
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount = 16 };
 
 inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "mock CUDA error"; }
 inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
+inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) { *v = 132; return cudaSuccess; }
 inline cudaError_t cudaDeviceGetStreamPriorityRange(int* lo, int* hi) { *lo = 0; *hi = -1; return cudaSuccess; }
 // fresh "device" memory is POISONED (0xFF bytes: NaN as f32, huge as an index), like real cudaMalloc memory it is not zero: a kernel
 // or host path that reads a word nobody wrote shows up as a wrong result instead of passing by luck

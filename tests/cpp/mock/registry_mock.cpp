@@ -136,7 +136,7 @@ int fdn_max_warps() { return 8; }
 // the tensor-core convolver form is never selected on the mock (bank.cpp tc_conv_wanted); the symbols only have to link
 cudaError_t conv_tc_make_maps(float*, float*, uint32_t, uint32_t, float*, float*, uint32_t, ConvTcMaps*) { return cudaErrorInvalidValue; }
 cudaError_t launch_conv_tc(const ConvTcMaps&, float*, uint32_t, uint32_t, const uint32_t*, uint32_t, uint32_t, uint32_t, uint32_t, cudaStream_t) { return cudaErrorInvalidValue; }
-cudaError_t launch_conv_split(const float*, float*, uint32_t, uint32_t, uint32_t, uint32_t, cudaStream_t) { return cudaErrorInvalidValue; }
+cudaError_t launch_conv_split(float*, float*, uint32_t, uint32_t, uint32_t, uint32_t, cudaStream_t) { return cudaErrorInvalidValue; }
 cudaError_t launch_conv_history(float*, float*, uint32_t, uint32_t, uint32_t, uint32_t, cudaStream_t) { return cudaErrorInvalidValue; }
 cudaError_t launch_conv_toeplitz(const float*, uint32_t, float*, float*, uint32_t, cudaStream_t) { return cudaErrorInvalidValue; }
 uint32_t conv_tc_toeplitz_cols(uint32_t) { return 0; }

@@ -171,13 +171,13 @@ def test_convolver_matches_linear_convolution(K):
     parts = np.concatenate([b2.render_samples(m)[0] for m in (64, 7, 1000, 61, n - 64 - 7 - 1000 - 61)], axis=-1)
     if K < 32:
         assert np.array_equal(parts, g)
-    else:   # tensor-core form (K >= 32): how a launch is cut into 128-sample tiles changes the order of the partial sums, not the value
+    else:   # tensor-core form (K >= 32): how a launch is cut into 64-sample tiles changes the order of the partial sums, not the value
         assert float(np.abs(parts - g).max()) <= 2e-6 * peak, float(np.abs(parts - g).max()) / peak
 
 
 @pytest.mark.parametrize("K", [64, 257, 1000, 4096])
 def test_tensor_core_convolver(K, monkeypatch):
-    """`x >> convolve(h)` as Toeplitz GEMM tiles on tensor cores (csrc/dsp/conv_tc_kernel.cuh: tcgen05 / TMEM, TMA operand tiles, 3xTF32):
+    """`x >> convolve(h)` as Toeplitz GEMM tiles on tensor cores (csrc/dsp/conv_tc_kernel.cuh: wgmma, TMA operand tiles, 3xTF32):
     against the f64 linear convolution (what the reference's partitioned FFT computes, src/convolve.rs:9-59) within 1e-5 of the output
     peak, for responses from one tile chunk to 4096 taps; partly filled voice tile, ragged last time tile, a render longer than the
     16384-sample chunk (history columns), state across calls, reset, clone, the voice-order mix, and the direct form as a cross-check."""

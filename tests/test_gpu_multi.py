@@ -1,5 +1,5 @@
 """Multi-GPU parity (SURVEY.md §8e): real GpuBank shards on >= 2 GPUs, mix-down through the C ABI's NCCL group, against the oracle's
-index-order mix. Needs two devices (`gpurun --gpus 2`); skipped with the reason on a one-GPU box."""
+index-order mix. Needs two devices; skipped with the reason on a one-GPU machine."""
 import os
 import socket
 import subprocess
@@ -19,7 +19,7 @@ def _gpus():
 def test_sharded_banks_reduce_to_the_oracle_mix():
     n = _gpus()
     if n < 2:
-        pytest.skip(f"needs 2 GPUs, this box has {n} (run: gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu)")
+        pytest.skip(f"needs 2 GPUs, this machine has {n}")
     world = 2 if n < 4 else 4
     s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", str(world), "--master-addr", "127.0.0.1", "--master-port", str(port),

@@ -76,8 +76,8 @@ def test_sharded_bank_on_the_mock_device(mock_env):
 
 
 def test_gpu_box_scripts_run_on_the_mock_device(mock_env):
-    """The scripts of the first GPU call of a round (tools/gpu_first_call.sh) are dry-run here at toy sizes, so GPU minutes are not
-    spent finding a typo: smoke() and the sequencer timing script."""
+    """Scripts meant for a GPU are dry-run here at toy sizes, so GPU time is not spent finding a typo: smoke() and the sequencer
+    timing script."""
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "prof_sequencer.py"), "--voices", "24", "--samples", "2048"],
                        capture_output=True, text=True, env=mock_env, cwd=ROOT, timeout=900)
     assert r.returncode == 0 and "sequencer bank" in r.stdout and "per push_event" in r.stdout, (r.stdout[-800:], r.stderr[-1500:])

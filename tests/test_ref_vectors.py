@@ -1,8 +1,8 @@
 """Pins the oracle (and the CUDA path) to outputs of the REAL reference crate — when they exist.
 
-`oracle/ref_dump` (a small Rust crate depending on the reference by path) renders the BASELINE configurations and a few single nodes with
-the real fundsp and writes tests/golden/ref/{manifest.json, *.f32}. The build image of this repository has no Rust toolchain, so the
-vectors cannot be produced here: every test below SKIPS with that reason until the directory is populated; on any machine with `cargo`
+`oracle/ref_dump` (a small Rust crate depending on the reference crate, fundsp 0.23.0) renders the BASELINE configurations and a few single nodes with
+the real fundsp and writes tests/golden/ref/{manifest.json, *.f32}. Producing the vectors needs a Rust toolchain; until they are
+committed every test below SKIPS with that reason until the directory is populated; on any machine with `cargo`
 the recipe in tests/golden/ref/README.md turns "parity unpinned" (DESIGN.md §4) into a checked claim. Bar: the north-star's 1e-5
 relative f32 (floor at 1e-2 of the vector's peak); the count of bit-exact samples is printed."""
 import json
@@ -25,7 +25,7 @@ def _manifest():
 
 MAN = _manifest()
 NAMES = [v["name"] for v in MAN["vectors"]] if MAN else ["(none)"]
-need = pytest.mark.skipif(MAN is None, reason="no reference vectors: tests/golden/ref/ is empty (needs cargo + the reference checkout: oracle/ref_dump)")
+need = pytest.mark.skipif(MAN is None, reason="no reference vectors: tests/golden/ref/ is empty (needs cargo and fundsp 0.23.0: oracle/ref_dump)")
 
 
 def _vector(name):

@@ -29,7 +29,7 @@ def compile_sig(sig):
     for mode in (1, 2, 3):
         for tb in ("false", "true"):
             nvrtc.nvrtcAddNameExpression(prog, f"fdsp::bank_kernel<fdsp::JitG, 128, {mode}, {tb}>".encode())
-    opts = [b"--gpu-architecture=sm_100a", b"-std=c++17", b"--fmad=false", b"-lineinfo", b"-default-device"]
+    opts = [b"--gpu-architecture=sm_90a", b"-std=c++17", b"--fmad=false", b"-lineinfo", b"-default-device"]
     (err,) = nvrtc.nvrtcCompileProgram(prog, len(opts), opts)
     _, n = nvrtc.nvrtcGetProgramLogSize(prog)
     log = b" " * n

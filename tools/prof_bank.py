@@ -1,4 +1,4 @@
-"""Profiling driver: one workload, device-resident buffers, a few launches (run under ncu via gpurun)."""
+"""Profiling driver: one workload, device-resident buffers, a few launches (run it under a profiler)."""
 import argparse, sys
 sys.path.insert(0, "."); sys.path.insert(0, "tests")
 import torch

@@ -1,6 +1,6 @@
 #!/bin/bash
 # Times the main workloads against each kernel build variant (fundsp_b200/variants/*.so) and the product library.
-# usage (on the GPU box): tools/variant_bench.sh > gpurun_out/variants.txt
+# usage (on a GPU machine): tools/variant_bench.sh
 for lib in fundsp_b200/libfundsp_b200.so fundsp_b200/variants/*.so; do
   [ -f "$lib" ] || continue
   echo "== $lib"
