@@ -10,13 +10,13 @@
 //   64-block), of which 2 * 128 * 64 * K are the convolution's own.
 //
 // Precision: TF32 keeps 10 mantissa bits, the bar is 1e-5 of the output peak, so the product is taken in the 3xTF32 split
-//     x = xh + xl,  h = hh + hl   (xh = x with the low 13 mantissa bits cleared, xl = x - xh exactly)
-//     x * h  ~  xh*hl + xl*hh + xh*hh        (the dropped xl*hl is <= 2^-20 |x h|)
+//     x ~ xh + xl,  h ~ hh + hl   (tf32(f) = f with the low 13 mantissa bits cleared; xh = tf32(x), xl = tf32(x - xh), same for h)
+//     x * h  ~  xh*hl + xl*hh + xh*hh        (xh + xl and hh + hl are within 2^-20 of x and h; the dropped xl*hl is <= 2^-20 |x h|)
 // as three `wgmma.mma_async ... .tf32` per 8-wide k-step. The split is stored: conv_split_lo_kernel rewrites the X rows as xh in place
-// and writes xl beside them (xh + xl = x exactly), conv_toeplitz_kernel writes hh and hl, so the tensor core reads operands that are
-// already TF32 and the result does not depend on how it would have converted an FP32 operand.
-// Accumulation: the tensor core rounds the FP32 accumulator at every MMA, and a 4096-tap response is 520 k-steps in a row — one
-// accumulator gave 1.3e-5 of the peak at K = 4096 (error growing with K). So the sum is spread over FIVE register accumulators: the
+// and writes xl beside them, conv_toeplitz_kernel writes hh and hl, all four already TF32, so the result does not depend on how the
+// tensor core would have converted an FP32 operand. (xh + xl is exact in FP32: with a one-hot response the output is exactly xh + xl.)
+// Accumulation: the tensor core rounds the FP32 accumulator at every MMA, and a 4096-tap response is 520 k-steps in a row (the error grows
+// with K; DESIGN.md §2 has the errors measured on an H100 from 32 to 48 000 taps). So the sum is spread over FIVE register accumulators: the
 // xh*hh products of k-step k = 0..3 of every chunk in four of them — a quarter of the sequential roundings each; the k-step picks the
 // accumulator statically, so no branch sits between the asynchronous MMAs — and both cross terms, 2^-11 smaller, in the fifth, where
 // their roundings do not count; the epilogue adds the five in FP32.
@@ -37,6 +37,10 @@
 namespace fdsp {
 
 constexpr int CTC_M = 128, CTC_N = 64, CTC_KC = 32, CTC_STAGES = 4;
+// Every CTC_FLUSH contraction chunks (and only if more follow) the consumers wait for their wgmma groups, add the five accumulators into a
+// register sum on the CUDA cores and restart them from zero, so no accumulator takes more than CTC_FLUSH * 4 roundings in a row. 64 chunks:
+// responses up to 1985 taps (K = 1000 is 34 chunks) never flush.
+constexpr int CTC_FLUSH = 64;
 constexpr int CTC_THREADS = 384;                                                          // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int CTC_TILE_A = CTC_M * CTC_KC * 4, CTC_TILE_B = CTC_N * CTC_KC * 4;          // bytes: 16 KB, 8 KB
 constexpr int CTC_STAGE_BYTES = 2 * CTC_TILE_A + 2 * CTC_TILE_B;                          // X, Xlo, T, Tlo
@@ -136,6 +140,9 @@ static __global__ void __launch_bounds__(CTC_THREADS, 1) conv_tc_kernel(const __
   float a0[32], a1[32], a2[32], a3[32], ax[32];
 #pragma unroll
   for (int j = 0; j < 32; j++) { a0[j] = 0.0f; a1[j] = 0.0f; a2[j] = 0.0f; a3[j] = 0.0f; ax[j] = 0.0f; }
+  float sum[32];                                                               // flushed partial sums, added on the CUDA cores (round to nearest)
+#pragma unroll
+  for (int j = 0; j < 32; j++) sum[j] = 0.0f;
   const uint32_t arow = (uint32_t)g * (64u * CTC_KC * 4u);                     // this warpgroup's 64 rows of the X tiles (8 swizzle atoms)
 #pragma unroll 1
   for (int c = 0; c < nchunk; c++) {
@@ -152,6 +159,15 @@ static __global__ void __launch_bounds__(CTC_THREADS, 1) conv_tc_kernel(const __
     ctc_wgmma_wait<1>();                                                       // chunk c - 1 has been read: its stage is free
     __syncwarp();
     if (c > 0 && lane == 0) ctc_mbar_arrive(empty_bar((c - 1) % CTC_STAGES));
+    if ((c + 1) % CTC_FLUSH == 0 && c + 1 < nchunk) {                     // long responses: bound the run of tensor-core accumulator roundings
+      ctc_wgmma_wait<0>();
+      ctc_fence_acc(a0); ctc_fence_acc(a1); ctc_fence_acc(a2); ctc_fence_acc(a3); ctc_fence_acc(ax);
+#pragma unroll
+      for (int j = 0; j < 32; j++) {
+        sum[j] += ((a0[j] + a1[j]) + (a2[j] + a3[j])) + ax[j];
+        a0[j] = 0.0f; a1[j] = 0.0f; a2[j] = 0.0f; a3[j] = 0.0f; ax[j] = 0.0f;
+      }
+    }
   }
   ctc_wgmma_wait<0>();
   ctc_fence_acc(a0); ctc_fence_acc(a1); ctc_fence_acc(a2); ctc_fence_acc(a3); ctc_fence_acc(ax);
@@ -168,8 +184,8 @@ static __global__ void __launch_bounds__(CTC_THREADS, 1) conv_tc_kernel(const __
 #pragma unroll
     for (int i = 0; i < CTC_N / 8; i++) {
       const int j = 4 * i + 2 * half;
-      const float y0 = ((a0[j] + a1[j]) + (a2[j] + a3[j])) + ax[j];            // ((a0 + a1) + (a2 + a3)) + cross
-      const float y1 = ((a0[j + 1] + a1[j + 1]) + (a2[j + 1] + a3[j + 1])) + ax[j + 1];
+      const float y0 = sum[j] + (((a0[j] + a1[j]) + (a2[j] + a3[j])) + ax[j]);  // flushed + (((a0 + a1) + (a2 + a3)) + cross); 0 + y = y
+      const float y1 = sum[j + 1] + (((a0[j + 1] + a1[j + 1]) + (a2[j + 1] + a3[j + 1])) + ax[j + 1]);
       const uint32_t col = (uint32_t)(8 * i + 2 * (lane & 3));
       const uint32_t left = a.n > t0 + col ? a.n - t0 - col : 0u;             // valid samples from this column on
       if (vec_ok && left >= 2u) *reinterpret_cast<float2*>(yrow + col) = make_float2(y0, y1);
@@ -178,33 +194,44 @@ static __global__ void __launch_bounds__(CTC_THREADS, 1) conv_tc_kernel(const __
   }
 }
 
-// xh = x with the low 13 mantissa bits cleared (in place), xl = x - xh, over the new columns of every X row
+__device__ __forceinline__ float ctc_tf32(float f) { return __uint_as_float(__float_as_uint(f) & 0xffffe000u); }   // low 13 mantissa bits cleared
+
+// xh = tf32(x) (in place), xl = tf32(x - xh), over the new columns of every X row. Grid = (voices, time blocks): voices on x, which has
+// no 65 535 limit.
 static __global__ void conv_split_lo_kernel(float* __restrict__ x, float* __restrict__ xl, uint32_t V, uint32_t row_stride, uint32_t col0, uint32_t n) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x, v = blockIdx.y;
+  const uint32_t t = blockIdx.y * blockDim.x + threadIdx.x, v = blockIdx.x;
   if (t >= n || v >= V) return;
   const size_t e = (size_t)v * row_stride + col0 + t;
-  const float f = x[e], hi = __uint_as_float(__float_as_uint(f) & 0xffffe000u);
+  const float f = x[e], hi = ctc_tf32(f);
   x[e] = hi;
-  xl[e] = f - hi;
+  xl[e] = ctc_tf32(f - hi);
 }
 // the last H samples of every row (columns [n, n + H)) move to the front (columns [0, H)): history for the next chunk. One CTA per
-// (row, array); the row's H values go through shared memory because source and destination overlap when n < H.
-static __global__ void conv_history_kernel(float* x, float* xl, uint32_t row_stride, uint32_t H, uint32_t n) {
-  extern __shared__ float hs[];
+// (row, array). Source and destination overlap when n < H, so this is a memmove to lower addresses: tiles of CTC_HIST_TILE columns in
+// ascending order, each read whole into registers before any of it is written. A later tile reads only columns >= n + its start, which
+// no earlier tile wrote, so any H works without shared memory.
+constexpr int CTC_HIST_THREADS = 256, CTC_HIST_PER = 4, CTC_HIST_TILE = CTC_HIST_THREADS * CTC_HIST_PER;
+static __global__ void __launch_bounds__(CTC_HIST_THREADS) conv_history_kernel(float* x, float* xl, uint32_t row_stride, uint32_t H, uint32_t n) {
   float* row = (blockIdx.y ? xl : x) + (size_t)blockIdx.x * row_stride;
-  for (uint32_t i = threadIdx.x; i < H; i += blockDim.x) hs[i] = row[n + i];
-  __syncthreads();
-  for (uint32_t i = threadIdx.x; i < H; i += blockDim.x) row[i] = hs[i];
+  for (uint32_t base = 0; base < H; base += CTC_HIST_TILE) {
+    float r[CTC_HIST_PER];
+#pragma unroll
+    for (int q = 0; q < CTC_HIST_PER; q++) { const uint32_t i = base + q * CTC_HIST_THREADS + threadIdx.x; if (i < H) r[q] = row[n + i]; }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < CTC_HIST_PER; q++) { const uint32_t i = base + q * CTC_HIST_THREADS + threadIdx.x; if (i < H) row[i] = r[q]; }
+    __syncthreads();
+  }
 }
-// T[n][j] = h[P + n - j] inside the band, 0 outside (P = K - 1 rounded up to 4: window column j is input sample t0 - P + j); hi = h with
-// the low 13 mantissa bits cleared, lo = h - hi. Rows n < CTC_N, J columns (multiple of 32).
+// T[n][j] = h[P + n - j] inside the band, 0 outside (P = K - 1 rounded up to 4: window column j is input sample t0 - P + j); hi = tf32(h),
+// lo = tf32(h - hi). Rows n < CTC_N, J columns (multiple of 32).
 static __global__ void conv_toeplitz_kernel(const float* __restrict__ h, uint32_t K, float* th, float* tl, uint32_t J) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x, n = blockIdx.y;
   if (j >= J) return;
   const int k = (int)((K - 1u + 3u) & ~3u) + (int)n - (int)j;
-  const float f = (k >= 0 && k < (int)K) ? h[k] : 0.0f, hi = __uint_as_float(__float_as_uint(f) & 0xffffe000u);
+  const float f = (k >= 0 && k < (int)K) ? h[k] : 0.0f, hi = ctc_tf32(f);
   th[(size_t)n * J + j] = hi;
-  tl[(size_t)n * J + j] = f - hi;
+  tl[(size_t)n * J + j] = ctc_tf32(f - hi);
 }
 
 }  // namespace fdsp

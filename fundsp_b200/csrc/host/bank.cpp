@@ -1017,7 +1017,7 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
       if (c.conv) {
         // stage 1: the program in front of the convolver writes its rows behind the history columns; then x_lo, the Toeplitz GEMM tiles
         // (rows straight into the caller's buffer, or an internal one), the history shift, and the voice-order fold of the rows
-        BankArgs d;
+        BankArgs d{};
         d.params = c.d_params; d.state = c.d_state; d.uniform = c.d_uniform; d.dline = c.d_dline; d.wt = d_wt; d.in = in_dev; d.partial = nullptr;
         d.out = c.d_cx; d.V = V; d.n = len; d.vpc = vpc; d.in_stride = (uint32_t)in_stride; d.in_offset = (uint32_t)t0; d.out_stride = c.conv_stride; d.out_offset = c.conv_H;
         d.row_map = c.d_dryrows; d.sr = (float)sr; d.sd64 = (float)(1.0 / sr); d.sd32 = 1.0f / (float)sr; d.ticket = nullptr; d.mix = nullptr; d.mix_stride = 0; d.mix_offset = 0; d.mix_accumulate = 0;

@@ -40,11 +40,15 @@ cudaError_t conv_tc_make_maps(float* x, float* xl, uint32_t V, uint32_t row_stri
 }
 cudaError_t launch_conv_tc(const ConvTcMaps& maps, float* y, uint32_t y_stride, uint32_t y_offset, const uint32_t* row_map, uint32_t V, uint32_t n, uint32_t K, uint32_t H,
                            cudaStream_t st) {
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CTC_SMEM);
+  // function attributes belong to each device's context: set once per device
+  static bool attr[64] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64 || !attr[dev]) {
+    e = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CTC_SMEM);
     if (e != cudaSuccess) return e;
-    attr = true;
+    if (dev >= 0 && dev < 64) attr[dev] = true;
   }
   const CUtensorMap* m = reinterpret_cast<const CUtensorMap*>(maps.m);
   ConvTcArgs a{y, y_stride, y_offset, row_map, V, n, K, H};
@@ -54,12 +58,12 @@ cudaError_t launch_conv_tc(const ConvTcMaps& maps, float* y, uint32_t y_stride, 
 }
 cudaError_t launch_conv_split(float* x, float* xl, uint32_t V, uint32_t row_stride, uint32_t col0, uint32_t n, cudaStream_t st) {
   if (n == 0 || V == 0) return cudaSuccess;
-  conv_split_lo_kernel<<<dim3((n + 255) / 256, V), 256, 0, st>>>(x, xl, V, row_stride, col0, n);
+  conv_split_lo_kernel<<<dim3(V, (n + 255) / 256), 256, 0, st>>>(x, xl, V, row_stride, col0, n);
   return cudaGetLastError();
 }
 cudaError_t launch_conv_history(float* x, float* xl, uint32_t V, uint32_t row_stride, uint32_t H, uint32_t n, cudaStream_t st) {
-  if (V == 0 || H == 0) return cudaSuccess;
-  conv_history_kernel<<<dim3(V, 2), 256, (size_t)H * sizeof(float), st>>>(x, xl, row_stride, H, n);
+  if (V == 0 || H == 0 || n == 0) return cudaSuccess;
+  conv_history_kernel<<<dim3(V, 2), CTC_HIST_THREADS, 0, st>>>(x, xl, row_stride, H, n);
   return cudaGetLastError();
 }
 cudaError_t launch_conv_toeplitz(const float* h, uint32_t K, float* th, float* tl, uint32_t J, cudaStream_t st) {

@@ -6,11 +6,15 @@
 namespace fdsp { namespace host {
 template <int NST> static cudaError_t launch_fdn_t(FdnArgs a, int warps, cudaStream_t st) {
   const size_t smem = (size_t)warps * fdn_warp_floats(NST) * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(fdn_kernel<NST>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  // function attributes belong to each device's context: set once per device
+  static bool attr[64] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64 || !attr[dev]) {
+    e = cudaFuncSetAttribute(fdn_kernel<NST>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
-    attr = true;
+    if (dev >= 0 && dev < 64) attr[dev] = true;
   }
   if (smem > 227 * 1024) return cudaErrorInvalidValue;
   const unsigned grid = (a.V + (unsigned)warps - 1) / (unsigned)warps;

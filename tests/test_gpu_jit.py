@@ -152,78 +152,6 @@ def test_jit_gated_envelope():
     assert np.array_equal(g, o), (int((g != o).sum()), float(np.abs(g - o).max()))
 
 
-@pytest.mark.parametrize("K", [1, 3, 64, 1000])
-def test_convolver_matches_linear_convolution(K):
-    """Convolver (src/convolve.rs): the reference computes y = x * h with a partitioned FFT (fft-convolver, not vendored), so the
-    bar is the tolerance of the path, 1e-5 of the output peak (the reference's own test, test_basic.rs:698-711, uses 1e-4)."""
-    rng = np.random.default_rng(K)
-    h = rng.uniform(-1, 1, K) * np.exp(-np.arange(K) / max(1.0, K / 4.0))
-    h = (h / np.abs(h).max()).astype(np.float32)
-    V, n = 48, 3000 + 61                       # ragged: the last block has 5 tail samples through the per-sample path
-    mk = lambda i: noise().seed(i) * (0.5 + 0.01 * i) >> convolve(h)
-    b, g, o = run_case(mk, V, n)
-    assert b.classes()[0]["voices"] == V       # one class: the impulse response is shared, class-uniform data
-    peak = float(np.abs(o).max())
-    assert peak > 0.1 and float(np.abs(g - o).max()) <= 1e-5 * peak, float(np.abs(g - o).max()) / peak
-    # state carries across calls and process()-sized launches agree with the long render
-    from fundsp_b200.bank import GpuBank
-    b2 = GpuBank([mk(i) for i in range(V)], per_voice=True, sample_rate=SR)
-    parts = np.concatenate([b2.render_samples(m)[0] for m in (64, 7, 1000, 61, n - 64 - 7 - 1000 - 61)], axis=-1)
-    if K < 32:
-        assert np.array_equal(parts, g)
-    else:   # tensor-core form (K >= 32): how a launch is cut into 64-sample tiles changes the order of the partial sums, not the value
-        assert float(np.abs(parts - g).max()) <= 2e-6 * peak, float(np.abs(parts - g).max()) / peak
-
-
-@pytest.mark.parametrize("K", [64, 257, 1000, 4096])
-def test_tensor_core_convolver(K, monkeypatch):
-    """`x >> convolve(h)` as Toeplitz GEMM tiles on tensor cores (csrc/dsp/conv_tc_kernel.cuh: wgmma, TMA operand tiles, 3xTF32):
-    against the f64 linear convolution (what the reference's partitioned FFT computes, src/convolve.rs:9-59) within 1e-5 of the output
-    peak, for responses from one tile chunk to 4096 taps; partly filled voice tile, ragged last time tile, a render longer than the
-    16384-sample chunk (history columns), state across calls, reset, clone, the voice-order mix, and the direct form as a cross-check."""
-    import os
-    from fundsp_b200.bank import GpuBank
-    if K > 1000 and "mock" in os.environ.get("FDSP_B200_LIB", ""):
-        pytest.skip("4096 taps in the direct form on the CPU mock device takes minutes; the tensor-core form is GPU-only")
-    rng = np.random.default_rng(K)
-    h = rng.uniform(-1, 1, K) * np.exp(-np.arange(K) / (K / 3.0))
-    h = (h / np.abs(h).max()).astype(np.float32)
-    V, n = 150, 16384 + 128 * 2 + 77
-    mk = lambda i: noise().seed(i) * (0.5 + 0.003 * i) >> convolve(h)
-    b = GpuBank([mk(i) for i in range(V)], per_voice=True, mix=True, sample_rate=SR)
-    g, mix = b.render_samples(n)
-    x = np.stack([oracle_rows(noise().seed(i) * (0.5 + 0.003 * i), n) for i in (0, 77, V - 1)])
-    want = np.stack([np.convolve(r.astype(np.float64), h.astype(np.float64))[:n] for r in x])
-    peak = float(np.abs(want).max())
-    err = float(np.abs(g[[0, 77, V - 1], 0] - want).max())
-    assert peak > 0.1 and err <= 1e-5 * peak, err / peak
-    acc = g[0, 0].copy()
-    for v in range(1, V):
-        acc = acc + g[v, 0]
-    if "mock" in os.environ.get("FDSP_B200_LIB", ""):   # (the mock runs the direct form, whose mix is the CTA-level tree)
-        assert np.abs(mix[0] - acc).max() <= 1e-5 * np.abs(g).sum(axis=0).max()
-    else:
-        assert np.array_equal(mix[0], acc)      # the mix is the left fold of the rows in voice order (the reference's index-order sum)
-    # continuation / reset / clone
-    b.reset()
-    c = b.clone()
-    p1, _ = b.render_samples(5000); p2, _ = b.render_samples(3000 + 5)
-    assert float(np.abs(np.concatenate([p1, p2], axis=-1) - g[..., :8005]).max()) <= 2e-6 * peak
-    q1, _ = c.render_samples(5000)
-    assert np.array_equal(q1, p1)
-    # the direct form (FP32 pipe) on the same voices
-    if "mock" not in os.environ.get("FDSP_B200_LIB", ""):
-        monkeypatch.setenv("FDSP_TC_CONV", "0")
-        d, _ = GpuBank([mk(i) for i in range(V)], per_voice=True, mix=True, sample_rate=SR).render_samples(2000)
-        assert float(np.abs(d - g[..., :2000]).max()) <= 1e-5 * peak
-
-
-def oracle_rows(expr, n):
-    from oracle import OracleUnit
-    u = OracleUnit(expr); u.set_sample_rate(SR)
-    return u.process_many(n)[0]
-
-
 def test_unsupported_graph_reports_error():
     from fundsp_b200.bank import GpuBank
     from fundsp_b200.capi import ERR_UNSUPPORTED, FdspError

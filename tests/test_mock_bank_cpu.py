@@ -58,7 +58,7 @@ def mock_env():
 
 
 def test_gpu_suite_runs_on_the_mock_device(mock_env):
-    files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_jit.py", "test_gpu_parity.py", "test_gpu_wider.py")]
+    files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_jit.py", "test_gpu_conv.py", "test_gpu_parity.py", "test_gpu_wider.py")]
     r = subprocess.run([sys.executable, "-m", "pytest", *files, "-m", "gpu", "-q", "-n", "8", "-p", "no:cacheprovider", "--tb=short"],
                        capture_output=True, text=True, env=mock_env, cwd=ROOT, timeout=3000)
     tail = r.stdout[-3000:]
