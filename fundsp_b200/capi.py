@@ -51,6 +51,8 @@ _SIG = {
     "fdsp_moog": (P, [F, F, I]), "fdsp_fir": (P, [I, FP]), "fdsp_tick": (P, [I]), "fdsp_delay": (P, [D]), "fdsp_allnest": (P, [F, P, I]),
     "fdsp_phase_osc": (P, [I]), "fdsp_dsf": (P, [I, F, F]), "fdsp_reverb3": (P, [D, D, P]), "fdsp_var": (P, [F]), "fdsp_nl_biquad": (P, [I, I, I, F, F, I, F, F, F]), "fdsp_declick": (P, [F]), "fdsp_slot": (P, [P]), "fdsp_bank_slot_set": (I, [P, U32, I, D, P]), "fdsp_bank_crossfade_voice": (I, [P, U32, I, F, P]), "fdsp_oversample": (P, [P]), "fdsp_monitor": (P, []), "fdsp_envelope": (P, [D, I, I, ENVFN, P, D]), "fdsp_event": (P, [P, D, D, I, D, D]), "fdsp_event_loop": (P, [P, D, D, I, D, D, D]), "fdsp_limiter": (P, [I, F, F]), "fdsp_meter": (P, [I, D]), "fdsp_playwave": (P, [C.POINTER(C.c_float), C.c_uint64, C.c_uint64, C.c_uint64, C.c_int64]), "fdsp_resample": (P, [P]), "fdsp_phase_synth": (P, [I]), "fdsp_pulse": (P, []), "fdsp_mixer": (P, [I, I, C.POINTER(C.c_float)]), "fdsp_rotate": (P, [F, F]), "fdsp_chaos": (P, [I]), "fdsp_morph": (P, [F, F]), "fdsp_rez": (P, [F, F, F, I]), "fdsp_follow": (P, [I, F, F]), "fdsp_shaper": (P, [I, F, F]), "fdsp_onepole": (P, [I, F, I]), "fdsp_convolve": (P, [FP, I]), "fdsp_feedback_unit": (P, [D, P]), "fdsp_mls": (P, [I]), "fdsp_impulse": (P, [I]), "fdsp_tap": (P, [I, I, F, F]), "fdsp_feedback2": (P, [P, P, I]),
     "fdsp_pan": (P, [F]), "fdsp_panner": (P, []), "fdsp_adsr_live": (P, [F, F, F, F]),
+    "fdsp_map": (P, [I, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]), "fdsp_shape_fn": (P, [C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
+    "fdsp_envelope_in": (P, [D, I, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
     "fdsp_pipe": (P, [P, P]), "fdsp_stack": (P, [P, P]), "fdsp_branch": (P, [P, P]), "fdsp_bus": (P, [P, P]), "fdsp_thru": (P, [P]),
     "fdsp_binop": (P, [I, P, P]), "fdsp_unop": (P, [I, F, P]), "fdsp_multi": (P, [I, I, I, C.POINTER(P)]), "fdsp_feedback": (P, [P, I]),
     "fdsp_net_new": (P, [I, I]), "fdsp_net_push": (I, [P, P]), "fdsp_net_connect": (I, [P, I, I, I, I]), "fdsp_net_connect_input": (I, [P, I, I, I]),
@@ -107,6 +109,23 @@ def _farr(v):
     if hasattr(v, "__array__"):   # a wave channel: no per-element conversion (data_as keeps the array alive)
         return np.ascontiguousarray(np.asarray(v, dtype=np.float32)).ctypes.data_as(C.POINTER(C.c_float))
     return (C.c_float * len(v))(*v)
+
+
+def _caps(caps):
+    """Captured values as the C ABI takes them: count, names, f32 values."""
+    names = [k.encode() for k, _ in caps]
+    return len(caps), (C.c_char_p * max(1, len(caps)))(*names), (C.c_float * max(1, len(caps)))(*[v for _, v in caps])
+
+
+def _closure_node(h):
+    """A closure node handle, or the refusal: ArityError for an arity mismatch (the reference's compile-time error), else FdspError."""
+    if not h:
+        msg = lib().fdsp_last_error().decode()
+        if ": arity mismatch" in msg:
+            from .graph import ArityError
+            raise ArityError(msg)
+        raise FdspError(ERR_ARG, msg)
+    return h
 
 
 class GpuBackend:
@@ -174,6 +193,9 @@ class GpuBackend:
     def b_pan(self, p): return _node(self.L.fdsp_pan(p), "pan")
     def b_panner(self): return _node(self.L.fdsp_panner(), "panner")
     def b_adsr_live(self, a, d, s, r): return _node(self.L.fdsp_adsr_live(a, d, s, r), "adsr_live")
+    def b_map(self, text, nin, nout, caps): return _closure_node(self.L.fdsp_map(nin, nout, text.encode(), *_caps(caps)))
+    def b_shape_fn(self, text, caps): return _closure_node(self.L.fdsp_shape_fn(text.encode(), *_caps(caps)))
+    def b_envelope_in(self, interval, text, nin, nout, caps): return _closure_node(self.L.fdsp_envelope_in(interval, nin, nout, text.encode(), *_caps(caps)))
     def b_pipe(self, x, y): return _node(self.L.fdsp_pipe(x, y), "pipe")
     def b_stack(self, x, y): return _node(self.L.fdsp_stack(x, y), "stack")
     def b_branch(self, x, y): return _node(self.L.fdsp_branch(x, y), "branch")

@@ -8,6 +8,7 @@
 #include <vector>
 
 #include "host/bank.h"
+#include "host/closure.h"
 #include "host/group.h"
 #include "host/wavfile.h"
 
@@ -106,6 +107,23 @@ API fdsp_node* fdsp_feedback2(fdsp_node* x, fdsp_node* y, int hadamard) { return
 API fdsp_node* fdsp_pan(float v) { return wrap(mk_pan(v), "pan"); }
 API fdsp_node* fdsp_panner(void) { return wrap(mk_panner(), "panner"); }
 API fdsp_node* fdsp_adsr_live(float a, float d, float s, float r) { return wrap(mk_adsr_live(a, d, s, r), "adsr_live"); }
+namespace {
+fdsp_node* closure_node(int kind, int inputs, int outputs, double interval, const char* closure, int nc, const char* const* names, const float* values) {
+  std::string e;
+  HNode* n = mk_closure(kind, inputs, outputs, interval, closure, nc, names, values, e);
+  if (!n) { g_err = e; return nullptr; }
+  return wrap(n, "closure");
+}
+}  // namespace
+API fdsp_node* fdsp_map(int inputs, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values) {
+  return closure_node(CL_MAP, inputs, outputs, 0.0, closure, ncaptures, names, values);
+}
+API fdsp_node* fdsp_shape_fn(const char* closure, int ncaptures, const char* const* names, const float* values) {
+  return closure_node(CL_SHAPE_FN, 1, 1, 0.0, closure, ncaptures, names, values);
+}
+API fdsp_node* fdsp_envelope_in(double interval, int inputs, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values) {
+  return closure_node(CL_ENVELOPE_IN, inputs, outputs, interval, closure, ncaptures, names, values);
+}
 API fdsp_node* fdsp_pipe(fdsp_node* x, fdsp_node* y) { return wrap(mk_pipe(take(x), take(y)), "pipe (>>)"); }
 API fdsp_node* fdsp_stack(fdsp_node* x, fdsp_node* y) { return wrap(mk_stack(take(x), take(y)), "stack (|)"); }
 API fdsp_node* fdsp_branch(fdsp_node* x, fdsp_node* y) { return wrap(mk_branch(take(x), take(y)), "branch (^)"); }

@@ -2051,6 +2051,201 @@ struct AdsrLive {  // src/envelope.rs:185-358 EnvelopeIn<f32,_,U1,f32> (ID 53) +
   static FDSP_DEV void end_simd(R&) {}
 };
 
+// ---------------------------------------------------------------- closures of the signal: map (ID 5), shape_fn (ID 42), EnvelopeIn (ID 53)
+// A closure crosses the C ABI as text; csrc/host/closure.cpp parses it and writes it into the class signature as a tree of the
+// expression templates below, so it is compiled like any other node. Everything is f32, evaluated as Rust evaluates the closure:
+// each operation individually rounded, no contraction. Literals are f32 bit patterns in the type (class-uniform); captured values
+// are per-voice parameter words (Cap<k>), so voices that share a closure text and differ in what they capture form one class.
+// `let` bindings are de Bruijn indexed (Var<0> is the innermost), so the spelling of names never reaches the signature.
+namespace Ex {
+struct Root {   // the closure's arguments: the input frame (or the shaper's scalar), the captures, the envelope's time
+  const float* x; const float* c; float t;
+  FDSP_HD const Root& root() const { return *this; }
+};
+template <class P> struct Scope { float v; const P& up; FDSP_HD const Root& root() const { return up.root(); } };
+template <int K, class S> FDSP_HD float var(const S& s) { if constexpr (K == 0) return s.v; else return var<K - 1>(s.up); }
+
+FDSP_HD float lerp_(float a, float b, float t) { return a * (1.0f - t) + b * t; }                 // src/math.rs:170-177 (f32 Lerp)
+FDSP_HD float exp10_(float x) { return m::expf_(x * (float)2.302585092994045684); }             // src/math.rs:76-78: (x * LN_10 as f32).exp()
+FDSP_HD float clamp_m(float x, float lo, float hi) { if (x < lo) x = lo; if (x > hi) x = hi; return x; }   // std f32::clamp: NaN propagates
+FDSP_HD float signum_m(float x) { return x != x ? m::fromb(0x7fc00000u) : copysignf(1.0f, x); }   // std f32::signum (fundsp's is copysignf)
+FDSP_HD float softexp_(float x) { const float p = fmaxf(x, 0.0f); return p * p + p + 1.0f / (1.0f + p - x); }   // src/math.rs:394-399
+FDSP_HD float sqr_hz_(float hz, float t) { float x = t * hz; x = x - floorf(x); return x < 0.5f ? 1.0f : -1.0f; }     // src/math.rs:485-493
+FDSP_HD float tri_hz_(float hz, float t) { float x = t * hz - 0.25f; x = x - floorf(x); return fabsf(x - 0.5f) * 4.0f - 1.0f; }   // :507-511
+
+#define FDSP_EX_LEAF(Name, cost_, expr) \
+  struct Name { static constexpr int cost = (cost_); template <class S> static FDSP_HD float ev(const S& s) { return (expr); } };
+#define FDSP_EX1(Name, cost_, expr) \
+  template <class A> struct Name { static constexpr int cost = A::cost + (cost_); \
+    template <class S> static FDSP_HD float ev(const S& s) { const float a = A::ev(s); return (expr); } };
+#define FDSP_EX2(Name, R_, cost_, expr) \
+  template <class A, class B> struct Name { static constexpr int cost = A::cost + B::cost + (cost_); \
+    template <class S> static FDSP_HD R_ ev(const S& s) { const auto a = A::ev(s); const auto b = B::ev(s); return (expr); } };
+#define FDSP_EX3(Name, cost_, expr) \
+  template <class A, class B, class C> struct Name { static constexpr int cost = A::cost + B::cost + C::cost + (cost_); \
+    template <class S> static FDSP_HD float ev(const S& s) { const float a = A::ev(s), b = B::ev(s), c = C::ev(s); return (expr); } };
+
+template <int K> struct In { static constexpr int cost = 0; template <class S> static FDSP_HD float ev(const S& s) { return s.root().x[K]; } };
+template <int K> struct Cap { static constexpr int cost = 0; template <class S> static FDSP_HD float ev(const S& s) { return s.root().c[K]; } };
+template <uint32_t B> struct Lit { static constexpr int cost = 0; template <class S> static FDSP_HD float ev(const S&) { return m::fromb(B); } };
+FDSP_EX_LEAF(T, 0, s.root().t)
+template <int K> struct Var { static constexpr int cost = 0; template <class S> static FDSP_HD float ev(const S& s) { return var<K>(s); } };
+template <int K> struct BVar { static constexpr int cost = 0; template <class S> static FDSP_HD bool ev(const S& s) { return var<K>(s) != 0.0f; } };
+
+FDSP_EX2(Add, float, 1, a + b) FDSP_EX2(Sub, float, 1, a - b) FDSP_EX2(Mul, float, 1, a * b) FDSP_EX2(Div, float, 8, a / b)
+FDSP_EX1(Neg, 1, -a)
+FDSP_EX2(Lt, bool, 1, a < b) FDSP_EX2(Le, bool, 1, a <= b) FDSP_EX2(Gt, bool, 1, a > b) FDSP_EX2(Ge, bool, 1, a >= b)
+FDSP_EX2(Eq, bool, 1, a == b) FDSP_EX2(Ne, bool, 1, a != b)
+FDSP_EX2(And, bool, 1, a && b) FDSP_EX2(Or, bool, 1, a || b)
+template <class A> struct Not { static constexpr int cost = A::cost + 1; template <class S> static FDSP_HD bool ev(const S& s) { return !A::ev(s); } };
+template <class C, class A, class B> struct If {
+  static constexpr int cost = C::cost + A::cost + B::cost + 2;
+  template <class S> static FDSP_HD auto ev(const S& s) { return C::ev(s) ? A::ev(s) : B::ev(s); }
+};
+template <class X, class B> struct Let {
+  static constexpr int cost = X::cost + B::cost;
+  template <class S> static FDSP_HD auto ev(const S& s) { const Scope<S> in{(float)X::ev(s), s}; return B::ev(in); }
+};
+template <class... Es> struct Out { static constexpr int cost = (0 + ... + Es::cost); };
+
+// exact operations (src/math.rs, Rust core), each as written there
+FDSP_EX1(Abs, 1, fabsf(a)) FDSP_EX2(Min, float, 1, fminf(a, b)) FDSP_EX2(Max, float, 1, fmaxf(a, b))
+FDSP_EX3(Clamp, 2, fminf(fmaxf(c, a), b))            // clamp(x0, x1, x) = x.max(x0).min(x1)
+FDSP_EX3(ClampM, 2, clamp_m(a, b, c))                 // x.clamp(lo, hi)
+FDSP_EX1(Clamp01, 2, fminf(fmaxf(a, 0.0f), 1.0f)) FDSP_EX1(Clamp11, 2, fminf(fmaxf(a, -1.0f), 1.0f))
+FDSP_EX1(Floor, 1, floorf(a)) FDSP_EX1(Ceil, 1, ceilf(a)) FDSP_EX1(Round, 2, roundf(a)) FDSP_EX1(Sqrt, 8, sqrtf(a))
+FDSP_EX1(Signum, 1, copysignf(1.0f, a)) FDSP_EX1(SignumM, 2, signum_m(a))
+FDSP_EX3(Lerp, 3, lerp_(a, b, c)) FDSP_EX3(Lerp11, 5, lerp_(a, b, c * 0.5f + 0.5f))
+FDSP_EX3(Delerp, 10, (c - a) / (b - a)) FDSP_EX3(Delerp11, 12, (c - a) / (b - a) * 2.0f - 1.0f)
+FDSP_EX1(Softsign, 10, a / (1.0f + fabsf(a)))
+FDSP_EX1(Softexp, 12, softexp_(a))
+FDSP_EX1(Smooth3, 4, (3.0f - 2.0f * a) * a * a)
+FDSP_EX1(Smooth5, 6, ((a * 6.0f - 15.0f) * a + 10.0f) * a * a * a)
+FDSP_EX1(Smooth7, 8, (a * a) * (a * a) * (35.0f - 84.0f * a + (70.0f - 20.0f * a) * (a * a)))
+FDSP_EX1(Smooth9, 10, ((((70.0f * a - 315.0f) * a + 540.0f) * a - 420.0f) * a + 126.0f) * (a * a) * (a * a) * a)
+template <class Y0, class Y1, class Y2, class Y3, class X> struct Spline {   // src/math.rs:360-366
+  static constexpr int cost = Y0::cost + Y1::cost + Y2::cost + Y3::cost + X::cost + 14;
+  template <class S> static FDSP_HD float ev(const S& s) {
+    const float y0 = Y0::ev(s), y1 = Y1::ev(s), y2 = Y2::ev(s), y3 = Y3::ev(s), x = X::ev(s);
+    return y1 + x * 0.5f * (y2 - y0 + x * (2.0f * y0 - 5.0f * y1 + 4.0f * y2 - y3 + x * (3.0f * (y1 - y2) + y3 - y0)));
+  }
+};
+FDSP_EX2(SqrHz, float, 4, sqr_hz_(a, b)) FDSP_EX2(TriHz, float, 6, tri_hz_(a, b))
+FDSP_EX1(BpmHz, 2, a * (1.0f / 60.0f)) FDSP_EX1(Squared, 1, a * a)
+// musl restatements (csrc/dsp/libm.cuh): what fundsp's Real / Float traits resolve to for f32, and what the project maps std's
+// inherent f32 methods to (DESIGN.md §4)
+FDSP_EX1(Sin, 40, m::sinf_(a)) FDSP_EX1(Cos, 40, m::cosf_(a)) FDSP_EX1(Tan, 50, m::tanf_(a)) FDSP_EX1(Tanh, 96, m::tanhf_(a))
+FDSP_EX1(Exp, 40, m::expf_(a)) FDSP_EX2(Pow, float, 120, m::powf_(a, b)) FDSP_EX1(Exp10, 41, exp10_(a)) FDSP_EX1(DbAmp, 49, exp10_(a / 20.0f))
+FDSP_EX2(SinHz, float, 42, m::sinf_(b * a * TAU_F)) FDSP_EX2(CosHz, float, 42, m::cosf_(b * a * TAU_F))   // sin_hz(hz, t) = sin(t * hz * TAU)
+#undef FDSP_EX_LEAF
+#undef FDSP_EX1
+#undef FDSP_EX2
+#undef FDSP_EX3
+
+// Writes the closure's value into o[0..NO): a tuple (the reference's ConstantFrame return) may stand in tail position, under
+// `let` and in both arms of an `if`.
+template <class X> struct Emit { template <class S> static FDSP_HD void out(const S& s, float* o) { o[0] = X::ev(s); } };
+template <class... Es> struct Emit<Out<Es...>> {
+  template <class S> static FDSP_HD void out(const S& s, float* o) { int i = 0; ((o[i++] = Es::ev(s)), ...); }
+};
+template <class X, class B> struct Emit<Let<X, B>> {
+  template <class S> static FDSP_HD void out(const S& s, float* o) { const Scope<S> in{(float)X::ev(s), s}; Emit<B>::out(in, o); }
+};
+template <class C, class A, class B> struct Emit<If<C, A, B>> {
+  template <class S> static FDSP_HD void out(const S& s, float* o) { if (C::ev(s)) Emit<A>::out(s, o); else Emit<B>::out(s, o); }
+};
+}  // namespace Ex
+
+template <int NI, int NO, int NC, class E> struct Map {   // src/audionode.rs:1328-1371, ID 5: no `process` override, so the block path is the tick loop
+  FDSP_NODE(NI, NO, NC, 0, 0);
+  struct R { float c[NC > 0 ? NC : 1]; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+#pragma unroll
+    for (int k = 0; k < NC; k++) r.c[k] = l.Pf();
+  }
+  static FDSP_DEV void save(const R&, Saver&) {}
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<NI>& in, Fr<NO>& o) {
+    const Ex::Root s{in.v, r.c, 0.0f};
+    Ex::Emit<E>::out(s, o.v);
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+// Shaper<ShapeFn<S>> (src/shape.rs:33-42, ID 42): ShapeFn::simd is the default per-lane `shape`, so tick and block paths coincide
+template <int NC, class E> struct ShaperFn : Map<1, 1, NC, E> {};
+
+// EnvelopeIn<f32, E, I, R> (src/envelope.rs:185-358, ID 53) with the closure E in the type: sampled at jittered points ~interval apart
+// with the input frame of the sample where the segment starts, interpolated linearly. Same run structure as AdsrLive above.
+template <int NI, int NO, int NC, class E> struct EnvelopeInFn {
+  FDSP_NODE(NI, NO, NC + 1, 8 + 4 * NO, 0);
+  struct R {
+    float c[NC > 0 ? NC : 1]; float interval;
+    float t, t0, t1; uint64_t t_hash;
+    float v0[NO], v1[NO], value[NO], delta[NO];
+    uint32_t run, run_len, seg_end;
+  };
+  static FDSP_DEV void load(R& r, Loader& l) {
+#pragma unroll
+    for (int k = 0; k < NC; k++) r.c[k] = l.Pf();
+    r.interval = l.Pf();
+    r.t = l.Sf(); r.t0 = l.Sf(); r.t1 = l.Sf();
+    const uint32_t lo = l.S(), hi = l.S(); r.t_hash = ((uint64_t)hi << 32) | lo;
+#pragma unroll
+    for (int k = 0; k < NO; k++) { r.v0[k] = l.Sf(); r.v1[k] = l.Sf(); r.value[k] = l.Sf(); r.delta[k] = l.Sf(); }
+    r.run = l.S(); r.run_len = l.S(); r.seg_end = l.S();
+  }
+  static FDSP_DEV void save(const R& r, Saver& s) {
+    s.Sf(r.t); s.Sf(r.t0); s.Sf(r.t1);
+    s.S((uint32_t)r.t_hash); s.S((uint32_t)(r.t_hash >> 32));
+#pragma unroll
+    for (int k = 0; k < NO; k++) { s.Sf(r.v0[k]); s.Sf(r.v1[k]); s.Sf(r.value[k]); s.Sf(r.delta[k]); }
+    s.S(r.run); s.S(r.run_len); s.S(r.seg_end);
+  }
+  static FDSP_DEV void call(const R& r, float time, const Fr<NI>& in, float* out) { const Ex::Root s{in.v, r.c, time}; Ex::Emit<E>::out(s, out); }
+  template <class C> static FDSP_DEV void next_segment(R& r, const C& c, const Fr<NI>& in) {   // envelope.rs:251-278
+    if (r.t0 == 0.0f && r.t1 == 0.0f) call(r, r.t0, in, r.v0);
+    else {
+      r.t0 = r.t1;
+#pragma unroll
+      for (int k = 0; k < NO; k++) r.v0[k] = r.v1[k];
+    }
+    const float next_interval = lerpf(0.75f, 1.25f, (float)rnd1(r.t_hash)) * r.interval;
+    r.t1 = r.t0 + next_interval;
+    call(r, r.t1, in, r.v1);
+    r.t_hash = r.t_hash * 6364136223846793005ull + 1ull;
+    const float u = delerpf(r.t0, r.t1, r.t);
+    const float samples = next_interval / c.sd64;
+#pragma unroll
+    for (int k = 0; k < NO; k++) { r.value[k] = lerpf(r.v0[k], r.v1[k], u); r.delta[k] = (r.v1[k] - r.v0[k]) / samples; }
+  }
+  template <class C> static FDSP_DEV void plan(R& r, const C& c, const Fr<NI>& in) {   // the while-loop of :323-341 from block index c.i
+    for (;;) {
+      const unsigned long long left = (unsigned long long)(long long)ceilf((r.t1 - r.t) / c.sd64);
+      const unsigned long long room = (unsigned long long)(c.n - c.i);
+      const unsigned long long loop = left < room ? left : room;
+      if (loop == 0ull) { next_segment(r, c, in); continue; }
+      r.run = (uint32_t)loop; r.run_len = r.run; r.seg_end = (loop == left) ? 1u : 0u;
+      return;
+    }
+  }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<NI>& in, Fr<NO>& o) {
+    if (T) {   // tick :305-313
+      if (r.t >= r.t1) next_segment(r, c, in);
+#pragma unroll
+      for (int k = 0; k < NO; k++) { o.v[k] = r.value[k]; r.value[k] += r.delta[k]; }
+      r.t += c.sd64;
+      return;
+    }
+    // process :315-342: the input is read at the block index where a segment changes
+    if (c.i == 0) { if (r.t >= r.t1) next_segment(r, c, in); plan(r, c, in); }
+    else if (r.run == 0u) { if (r.seg_end) next_segment(r, c, in); plan(r, c, in); }
+#pragma unroll
+    for (int k = 0; k < NO; k++) { o.v[k] = r.value[k]; r.value[k] += r.delta[k]; }
+    r.run -= 1u;
+    if (r.run == 0u) r.t += (float)r.run_len * c.sd64;
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+
 
 // ---------------------------------------------------------------- Dag: a whole Net as ONE fused node (src/net.rs:118-146, 1224-1286)
 // The reference's Net is a dynamic DAG of boxed units processed vertex by vertex in dependency order, each vertex reading the
@@ -2187,6 +2382,9 @@ template <> struct Cost<Biquad> { static constexpr int value = 12; };
 template <> struct Cost<BiquadBank> { static constexpr int value = 96; };
 template <int N> struct Cost<Moog<N>> { static constexpr int value = 200; };
 template <> struct Cost<AdsrLive> { static constexpr int value = 120; };
+template <int NI, int NO, int NC, class E> struct Cost<Map<NI, NO, NC, E>> { static constexpr int value = 2 + E::cost; };
+template <int NC, class E> struct Cost<ShaperFn<NC, E>> { static constexpr int value = 2 + E::cost; };
+template <int NI, int NO, int NC, class E> struct Cost<EnvelopeInFn<NI, NO, NC, E>> { static constexpr int value = 120; };
 template <> struct Cost<Delay> { static constexpr int value = 12; };
 template <int N> struct Cost<Panner<N>> { static constexpr int value = N == 1 ? 2 : 80; };
 template <int K, class X, class Y> struct Cost<Binop<K, X, Y>> { static constexpr int value = Cost<X>::value + Cost<Y>::value + 1; };

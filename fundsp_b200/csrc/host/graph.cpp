@@ -2,6 +2,7 @@
 // the reference checkout). Coefficient formulas are evaluated in f32 with the host libm exactly where the
 // reference evaluates them (constructor / set_sample_rate / Setting), never per sample.
 #include "graph.h"
+#include "closure.h"
 #include "../dsp/libm.cuh"
 
 #include <cmath>
@@ -776,6 +777,34 @@ struct AdsrLive : HNode {
   HCLONE(AdsrLive)
 };
 
+// ---------------------------------------------------------------- closures of the signal (csrc/host/closure.cpp parses the text)
+// The parsed closure is part of the signature; the captured values are per-voice parameter words in Cap<k> order.
+struct ClosureN : HNode {
+  ClosureKind kind; int nin, nout; std::string expr; std::vector<float> caps;
+  float interval = 0.0f; uint64_t hash = 0;   // EnvelopeIn only
+  ClosureN(ClosureKind k, int i, int o, std::string e, std::vector<float> c) : kind(k), nin(i), nout(o), expr(std::move(e)), caps(std::move(c)) {}
+  int inputs() const override { return nin; } int outputs() const override { return nout; }
+  uint64_t id() const override { return kind == CL_MAP ? 5 : (kind == CL_SHAPE_FN ? 42 : 53); }
+  void set(const Setting& s) override { if (kind == CL_ENVELOPE_IN && s.kind == P_INTERVAL) interval = s.v[0]; }   // src/envelope.rs:344-348; map and shape_fn have no parameter
+  void set_hash(uint64_t h) override { if (kind == CL_ENVELOPE_IN) hash = h; }                                       // envelope.rs:350-353
+  void sig(std::string& o) const override {
+    const std::string nc = I((int)caps.size());
+    if (kind == CL_MAP) o += "Map<" + I(nin) + "," + I(nout) + "," + nc + "," + expr + ">";
+    else if (kind == CL_SHAPE_FN) o += "ShaperFn<" + nc + "," + expr + ">";
+    else o += "EnvelopeInFn<" + I(nin) + "," + I(nout) + "," + nc + "," + expr + ">";
+  }
+  void lower(Lowering& l) const override {
+    for (float c : caps) l.p(c);
+    if (kind != CL_ENVELOPE_IN) return;
+    l.p(interval);
+    l.s(0.0f); l.s(0.0f); l.s(0.0f);                      // t, t_0, t_1 (EnvelopeIn::reset)
+    l.su((uint32_t)hash); l.su((uint32_t)(hash >> 32));   // t_hash
+    for (int k = 0; k < nout; k++) { l.s(0.0f); l.s(0.0f); l.s(0.0f); l.s(0.0f); }   // value_0, value_1, value, value_d
+    l.su(0u); l.su(0u); l.su(0u);                         // run, run_len, seg_end
+  }
+  HCLONE(ClosureN)
+};
+
 // ---------------------------------------------------------------- combinators (src/audionode.rs:724-2800)
 struct Binary : HNode {
   enum K { PIPE = 6, STACK = 7, BRANCH = 8, BUS = 10, BINOP = 3 } k; int op; Kid x, y;
@@ -1190,6 +1219,35 @@ HNode* mk_feedback2(HNode* x, HNode* y, int hadamard) {
 HNode* mk_pan(float value) { return new Panner(value, 1); }
 HNode* mk_panner() { return new Panner(0.0f, 2); }
 HNode* mk_adsr_live(float a, float d, float s, float r) { return new AdsrLive(a, d, s, r); }
+HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char* text, int ncaptures, const char* const* names, const float* values,
+                  std::string& err) {
+  const char* what = kind == CL_MAP ? "map" : (kind == CL_SHAPE_FN ? "shape_fn" : "envelope_in");
+  auto bad = [&](const std::string& w) -> HNode* { err = std::string(what) + ": " + w; return nullptr; };
+  if (kind < CL_MAP || kind > CL_ENVELOPE_IN) { err = "closure: bad kind"; return nullptr; }
+  if (inputs < 0 || inputs > 8 || outputs < 1 || outputs > 8) return bad("arity mismatch: 0-8 inputs and 1-8 outputs");
+  if (kind == CL_ENVELOPE_IN && !(interval > 0.0)) return bad("the interval must be positive");   // EnvelopeIn::new asserts it (src/envelope.rs:230)
+  if (ncaptures < 0 || (ncaptures > 0 && (!names || !values))) return bad("bad capture arrays");
+  Closure c;
+  const std::string e = parse_closure(text, (ClosureKind)kind, inputs, outputs, c);
+  if (!e.empty()) return bad(e);
+  std::vector<float> v(c.caps.size());
+  for (size_t k = 0; k < c.caps.size(); k++) {
+    int found = -1;
+    for (int j = 0; j < ncaptures; j++) if (names[j] && c.caps[k] == names[j]) found = j;
+    if (found < 0) return bad("`" + c.caps[k] + "` is neither a parameter nor a captured value: pass its value as a capture");
+    v[k] = values[found];
+  }
+  for (int j = 0; j < ncaptures; j++) {
+    if (!names[j]) return bad("null capture name");
+    bool used = false;
+    for (const std::string& n : c.caps) used = used || n == names[j];
+    if (!used) return bad(std::string("capture `") + names[j] + "` does not occur in the closure");
+    for (int i = 0; i < j; i++) if (names[i] && strcmp(names[i], names[j]) == 0) return bad(std::string("capture `") + names[j] + "` is given twice");
+  }
+  ClosureN* n = new ClosureN((ClosureKind)kind, kind == CL_SHAPE_FN ? 1 : inputs, kind == CL_SHAPE_FN ? 1 : outputs, c.expr, std::move(v));
+  n->interval = (float)interval;   // EnvelopeIn<f32>: F::from_f32 / the f32 interval of prelude32 (src/prelude32.rs:716-724)
+  return n;
+}
 
 static HNode* bad2(HNode* x, HNode* y) { delete x; delete y; return nullptr; }
 HNode* mk_pipe(HNode* x, HNode* y) { if (!x || !y || x->outputs() != y->inputs()) return bad2(x, y); return new Binary(Binary::PIPE, 0, x, y); }
@@ -1213,3 +1271,7 @@ HNode* mk_multi(int kind, int op, int n, HNode** nodes) {
 
 }  // namespace host
 }  // namespace fdsp
+
+// The closure parser is part of this translation unit, so that every build of the host graph (the product library, and the CPU
+// builds of the host runtime that tests/ make) contains it.
+#include "closure.cpp"

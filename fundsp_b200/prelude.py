@@ -549,6 +549,58 @@ def lfo(f, outputs=None, horizon=10.0, time64=False):
     return envelope(f, outputs, horizon, time64)
 
 
+# ---- closures of the signal, run per sample on the GPU (prelude32: src/prelude32.rs:625-740, 1126-1183). The closure is text in a
+# subset of Rust closure syntax (DESIGN.md §2); every other free identifier in it is a captured value, given as a keyword argument:
+#   map_("|x| tanh(x[0] * drive)", 1, 1, drive=0.7)
+# The text is checked here: an arity mismatch raises ArityError, any other refusal FdspError (the message names the token and column).
+def _closure(op, args, nin, nout):
+    from .capi import GpuBackend, lib
+    lib().fdsp_node_free(getattr(GpuBackend(), "b_" + op)(*args))
+    return An(op, args, (), nin, nout)
+
+
+def _captures(captures):
+    return tuple((str(k), f32(v)) for k, v in captures.items())
+
+
+def map_(closure, inputs, outputs, **captures):
+    """`map(f)` (Map ID 5): a per-sample function of the input frame `x[0..inputs)`; a tuple value gives several outputs."""
+    return _closure("map", (closure, int(inputs), int(outputs), _captures(captures)), int(inputs), int(outputs))
+
+
+def shape_fn(closure, **captures):
+    """`shape_fn(f)` (Shaper<ShapeFn> ID 42): a waveshaper `|x| ...` of one scalar."""
+    return _closure("shape_fn", (closure, _captures(captures)), 1, 1)
+
+
+def envelope_in(closure, inputs, outputs=1, **captures):
+    """`envelope_in(f)` (EnvelopeIn ID 53, interval 2 ms): `|t, i| ...` of time and the input frame `i[0..inputs)`, sampled at jittered
+    points ~2 ms apart and interpolated; `|t, x1, .., xN|` takes one scalar per input instead."""
+    return _closure("envelope_in", (f32(0.002), closure, int(inputs), int(outputs), _captures(captures)), int(inputs), int(outputs))
+
+
+def lfo_in(closure, inputs, outputs=1, **captures):
+    return envelope_in(closure, inputs, outputs, **captures)
+
+
+def envelope2(closure, outputs=1, **captures):
+    """`envelope2(|t, x| ...)`: envelope_in of one input."""
+    return envelope_in(closure, 1, outputs, **captures)
+
+
+def lfo2(closure, outputs=1, **captures):
+    return envelope_in(closure, 1, outputs, **captures)
+
+
+def envelope3(closure, outputs=1, **captures):
+    """`envelope3(|t, x, y| ...)`: envelope_in of two inputs."""
+    return envelope_in(closure, 2, outputs, **captures)
+
+
+def lfo3(closure, outputs=1, **captures):
+    return envelope_in(closure, 2, outputs, **captures)
+
+
 # ---- src/prelude.rs:2719-2753 flanger / phaser: the delay (phase) closure is a closure of time, so it lowers like `lfo`
 def flanger(feedback_amount, minimum_delay, maximum_delay, delay_f, horizon=10.0):
     return pass_() & feedback2((pass_() | lfo(lambda t: f32(delay_f(t)), 1, horizon)) >> tap(minimum_delay, maximum_delay), shape(Tanh(feedback_amount)))

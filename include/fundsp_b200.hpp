@@ -202,6 +202,38 @@ inline An fdn2(An x, An y) { return An(fdsp_feedback2(x.release(), y.release(), 
 inline An pan(float p) { return An(fdsp_pan(p)); }
 inline An panner() { return An(fdsp_panner()); }
 inline An adsr_live(float a, float d, float s, float r) { return An(fdsp_adsr_live(a, d, s, r)); }
+// closures of the signal, run per sample on the device (DESIGN.md §2 / row f.12): the closure as text, captured values by name, e.g.
+//   map("|x| tanh(x[0] * drive)", 1, 1, {{"drive", 0.7f}})
+// A refused text throws Error with the token and its column (FDSP_ERR_ARITY for arity mismatches, else FDSP_ERR_ARG).
+using Captures = std::initializer_list<std::pair<const char*, float>>;
+namespace detail {
+inline An closure_node(fdsp_node* h) {
+  if (h) return An(h);
+  const std::string e = fdsp_last_error();
+  throw Error(e.find(": arity mismatch") != std::string::npos ? FDSP_ERR_ARITY : FDSP_ERR_ARG, e);
+}
+struct CaptureArrays {
+  std::vector<const char*> names; std::vector<float> values;
+  explicit CaptureArrays(Captures c) { for (const auto& p : c) { names.push_back(p.first); values.push_back(p.second); } }
+};
+}  // namespace detail
+inline An map(const char* closure, int inputs, int outputs, Captures captures = {}) {
+  detail::CaptureArrays c(captures);
+  return detail::closure_node(fdsp_map(inputs, outputs, closure, (int)c.names.size(), c.names.data(), c.values.data()));
+}
+inline An shape_fn(const char* closure, Captures captures = {}) {
+  detail::CaptureArrays c(captures);
+  return detail::closure_node(fdsp_shape_fn(closure, (int)c.names.size(), c.names.data(), c.values.data()));
+}
+inline An envelope_in(const char* closure, int inputs, int outputs = 1, Captures captures = {}) {
+  detail::CaptureArrays c(captures);
+  return detail::closure_node(fdsp_envelope_in(0.002, inputs, outputs, closure, (int)c.names.size(), c.names.data(), c.values.data()));
+}
+inline An lfo_in(const char* closure, int inputs, int outputs = 1, Captures captures = {}) { return envelope_in(closure, inputs, outputs, captures); }
+inline An envelope2(const char* closure, int outputs = 1, Captures captures = {}) { return envelope_in(closure, 1, outputs, captures); }
+inline An lfo2(const char* closure, int outputs = 1, Captures captures = {}) { return envelope_in(closure, 1, outputs, captures); }
+inline An envelope3(const char* closure, int outputs = 1, Captures captures = {}) { return envelope_in(closure, 2, outputs, captures); }
+inline An lfo3(const char* closure, int outputs = 1, Captures captures = {}) { return envelope_in(closure, 2, outputs, captures); }
 inline An feedback(An x) { return An(fdsp_feedback(x.release(), 0)); }
 inline An fdn(An x) { return An(fdsp_feedback(x.release(), 1)); }
 template <class F> An stacki(int n, F f) { std::vector<fdsp_node*> v; for (int i = 0; i < n; i++) v.push_back(f(i).release()); return An(fdsp_multi(30, 0, n, v.data())); }

@@ -53,6 +53,9 @@ extern "C" {
     fn fdsp_delay(seconds: f64) -> *mut FdspNode;
     fn fdsp_pan(value: f32) -> *mut FdspNode;
     fn fdsp_adsr_live(a: f32, d: f32, s: f32, r: f32) -> *mut FdspNode;
+    fn fdsp_map(inputs: c_int, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
+    fn fdsp_shape_fn(closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
+    fn fdsp_envelope_in(interval: f64, inputs: c_int, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_convolve(response: *const f32, n: c_int) -> *mut FdspNode;
     fn fdsp_pipe(x: *mut FdspNode, y: *mut FdspNode) -> *mut FdspNode;
     fn fdsp_stack(x: *mut FdspNode, y: *mut FdspNode) -> *mut FdspNode;
@@ -288,6 +291,73 @@ impl<N: Size<f32> + Size<X>, X: AudioNode + Lower, B: FrameBinop<X::Outputs> + B
 /// `adsr_live(a, d, s, r)` is `EnvelopeIn` with the closure of adsr.rs:21-70: closures do not cross a C ABI, the closed form does.
 pub struct AdsrLive { pub attack: f32, pub decay: f32, pub sustain: f32, pub release: f32 }
 impl Lower for AdsrLive { unsafe fn lower(&self) -> *mut FdspNode { fdsp_adsr_live(self.attack, self.decay, self.sustain, self.release) } }
+
+/// A closure of the signal that can also run on the GPU: the reference's node `X` (what runs on the CPU) plus the closure's text and
+/// captured values, which `Lower` hands to `fdsp_map` / `fdsp_shape_fn` / `fdsp_envelope_in`. Made by `gpu_map!`, `gpu_shape_fn!` and
+/// `gpu_envelope_in!`, which take the closure ONCE: it is compiled by rustc for the CPU node and `stringify!`-ed for the GPU node, so
+/// the two cannot drift apart. The text must stay inside the closure language of DESIGN.md §2 (f32 literals, the listed functions);
+/// `fdsp_*` refuses anything else with the token and its column, and `GpuBank::new` returns that error.
+#[derive(Clone)]
+pub struct GpuClosure<X> { pub node: X, pub kind: c_int, pub interval: f64, pub text: &'static str, pub names: Vec<&'static str>, pub values: Vec<f32> }
+impl<X: AudioNode> AudioNode for GpuClosure<X> {
+    const ID: u64 = X::ID;
+    type Inputs = X::Inputs;
+    type Outputs = X::Outputs;
+    fn reset(&mut self) { self.node.reset() }
+    fn set_sample_rate(&mut self, sample_rate: f64) { self.node.set_sample_rate(sample_rate) }
+    fn tick(&mut self, input: &Frame<f32, Self::Inputs>) -> Frame<f32, Self::Outputs> { self.node.tick(input) }
+    fn process(&mut self, size: usize, input: &BufferRef, output: &mut BufferMut) { self.node.process(size, input, output) }
+    fn set(&mut self, setting: Setting) { if let Parameter::Interval(t) = setting.parameter() { self.interval = *t as f64; } self.node.set(setting) }
+    fn set_hash(&mut self, hash: u64) { self.node.set_hash(hash) }
+    fn route(&mut self, input: &SignalFrame, frequency: f64) -> SignalFrame { self.node.route(input, frequency) }
+}
+impl<X: AudioNode> Lower for GpuClosure<X> {
+    unsafe fn lower(&self) -> *mut FdspNode {
+        let text: Vec<u8> = self.text.bytes().chain(core::iter::once(0)).collect();
+        let names: Vec<Vec<u8>> = self.names.iter().map(|n| n.bytes().chain(core::iter::once(0)).collect()).collect();
+        let ptrs: Vec<*const c_char> = names.iter().map(|n| n.as_ptr() as *const c_char).collect();
+        let (i, o, nc) = (X::Inputs::I32, X::Outputs::I32, self.values.len() as c_int);
+        let t = text.as_ptr() as *const c_char;
+        match self.kind {
+            0 => fdsp_map(i, o, t, nc, ptrs.as_ptr(), self.values.as_ptr()),
+            1 => fdsp_shape_fn(t, nc, ptrs.as_ptr(), self.values.as_ptr()),
+            _ => fdsp_envelope_in(self.interval, i, o, t, nc, ptrs.as_ptr(), self.values.as_ptr()),
+        }
+    }
+}
+/// `gpu_map!(U1, U1, [drive], |x: &Frame<f32, U1>| tanh(x[0] * drive))`: `map(..)` (prelude.rs:1126) that lowers to `fdsp_map`.
+/// The bracket lists the captured f32 variables.
+#[macro_export]
+macro_rules! gpu_map {
+    ($i:ty, $o:ty, [$($c:ident),*], $($f:tt)+) => {
+        $crate::combinator::An($crate::gpu::GpuClosure {
+            node: $crate::audionode::Map::<_, $i, $o>::new($($f)+, $crate::signal::Routing::Arbitrary(0.0)),
+            kind: 0, interval: 0.0, text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
+        })
+    };
+}
+/// `gpu_shape_fn!([h], |x: f32| tanh(x * h))`: `shape_fn(..)` (prelude.rs:1181) that lowers to `fdsp_shape_fn`.
+#[macro_export]
+macro_rules! gpu_shape_fn {
+    ([$($c:ident),*], $($f:tt)+) => {
+        $crate::combinator::An($crate::gpu::GpuClosure {
+            node: $crate::shape::Shaper::new($crate::shape::ShapeFn($($f)+)),
+            kind: 1, interval: 0.0, text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
+        })
+    };
+}
+/// `gpu_envelope_in!(U2, [k], |t: f32, i: &Frame<f32, U2>| i[0] * k + t)`: `envelope_in(..)` (prelude32.rs:716, interval 2 ms) that lowers to
+/// `fdsp_envelope_in`; the output count is the closure's return type. envelope2 / envelope3 are this with `|t, x| ..` / `|t, x, y| ..`
+/// written over `i[0]` / `i[1]` (prelude32.rs:625-708).
+#[macro_export]
+macro_rules! gpu_envelope_in {
+    ($i:ty, [$($c:ident),*], $($f:tt)+) => {
+        $crate::combinator::An($crate::gpu::GpuClosure {
+            node: $crate::envelope::EnvelopeIn::<f32, _, $i, _>::new(0.002, $($f)+),
+            kind: 2, interval: 0.002f32 as f64, text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
+        })
+    };
+}
 
 /// V voices of typed graphs evaluated in lockstep on one GPU; to the host ONE `AudioUnit` (audiounit.rs:21-95).
 pub struct GpuBank { h: *mut FdspBank, inputs: usize, outputs: usize, failed: bool }

@@ -62,6 +62,14 @@ def jobs():
         add("Xfade<" + sg(x) + "," + sg(y) + ">", (1,))
     add(capi.NodeHandle(workloads.build("saw_svf_events", 1)[0]).signature(), (2, 3))      # bench --workload saw_svf_events and its parity test
     add(capi.NodeHandle(slot(W.arp_voice(100.0))).signature(), (1,))                        # test_slot_crossfades_to_a_new_unit
+    # closures of the signal (tests/test_gpu_closures.py: rows, rows + mix; tools/bench_closures.py: mix): NVRTC-only classes
+    import test_gpu_closures as CL
+    from fundsp_b200.prelude import envelope2, map_, saw_hz, shape, Tanh
+    for mk in CL.CASES.values():
+        add(sg(mk(0)), (1, 2, 3))
+    add(sg(envelope2("|t, x| x * x * a + t", a=1.0)), (1,))
+    for g in (saw_hz(50.0) >> map_("|x| tanh(x[0] * drive)", 1, 1, drive=1.0), saw_hz(50.0) >> shape(Tanh(1.0))):
+        add(sg(g), (1, 2, 3))
     return sorted(out)
 
 
