@@ -3,8 +3,9 @@ path, settings on a live bank, sequencer clock / edit / push / growth in place, 
 
 tests/cpp/mock/ builds the host sources against a stand-in <cuda_runtime.h> ("device" memory is host memory, calls are synchronous) and
 replaces the kernels by the device node library compiled for the CPU (FDSP_HOST_EMUL), one small shared object per graph class walking
-every voice through bank_kernel's per-thread block structure. The whole GPU test-suite then runs against that library in a subprocess
-(FDSP_B200_LIB selects it there and only there). What this does NOT cover is the CUDA side proper — the CTA mix tile, TMA table
+every voice through bank_kernel's per-thread block structure, and summing each CTA's partial mix in the association of the kernel's mix
+tile (so the exact mix model of tests/test_gpu_mix.py holds on the mock too). The whole GPU test-suite then runs against that library in a
+subprocess (FDSP_B200_LIB selects it there and only there). What this does NOT cover is the CUDA side proper — the shared-memory tile itself, TMA table
 staging, the warp-per-voice FDN kernel itself (the mock runs the equivalent generic reverb program on its argument block, so the host side of
 the two-stage classes IS covered), stream concurrency — which the same tests check on a B200.
 The mock is test infrastructure: it is never built into, or loaded by, the product."""
@@ -58,7 +59,7 @@ def mock_env():
 
 
 def test_gpu_suite_runs_on_the_mock_device(mock_env):
-    files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_jit.py", "test_gpu_conv.py", "test_gpu_parity.py", "test_gpu_wider.py")]
+    files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_jit.py", "test_gpu_conv.py", "test_gpu_parity.py", "test_gpu_wider.py", "test_gpu_mix.py")]
     r = subprocess.run([sys.executable, "-m", "pytest", *files, "-m", "gpu", "-q", "-n", "8", "-p", "no:cacheprovider", "--tb=short"],
                        capture_output=True, text=True, env=mock_env, cwd=ROOT, timeout=3000)
     tail = r.stdout[-3000:]

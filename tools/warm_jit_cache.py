@@ -70,6 +70,18 @@ def jobs():
     add(sg(envelope2("|t, x| x * x * a + t", a=1.0)), (1,))
     for g in (saw_hz(50.0) >> map_("|x| tanh(x[0] * drive)", 1, 1, drive=1.0), saw_hz(50.0) >> shape(Tanh(1.0))):
         add(sg(g), (1, 2, 3))
+    # the exact mix model (tests/test_gpu_mix.py): 2..5-output stacks (rows, rows + mix, mix alone; twins of process() banks), the
+    # 2-input stereo voice of the resident process() kernel, the plain classes beside two-stage and reverb classes
+    import test_gpu_mix as MX
+    for k in (2, 3, 4, 5):
+        add(sg(MX.stack_voice(k)(0)), (1, 2, 3))
+    for i in (1, 2):
+        add(sg(MX.mixed_voice(i)), (1, 2, 3))
+    add(sg(MX.reverb_input_voice(5)), (1, 2, 3))
+    for name in ("in2_stereo", "five_out"):
+        s = sg(MX.RT_CASES[name][0](0))
+        add(s, (1, 2))
+        out[(s, 2, (1 if has_table(s) else 0) | (255 << 8))] = True   # the resident process() kernel
     return sorted(out)
 
 
