@@ -52,6 +52,7 @@ _SIG = {
     "fdsp_phase_osc": (P, [I]), "fdsp_dsf": (P, [I, F, F]), "fdsp_reverb3": (P, [D, D, P]), "fdsp_var": (P, [F]), "fdsp_nl_biquad": (P, [I, I, I, F, F, I, F, F, F]), "fdsp_declick": (P, [F]), "fdsp_slot": (P, [P]), "fdsp_bank_slot_set": (I, [P, U32, I, D, P]), "fdsp_bank_crossfade_voice": (I, [P, U32, I, F, P]), "fdsp_oversample": (P, [P]), "fdsp_monitor": (P, []), "fdsp_envelope": (P, [D, I, I, ENVFN, P, D]), "fdsp_event": (P, [P, D, D, I, D, D]), "fdsp_event_loop": (P, [P, D, D, I, D, D, D]), "fdsp_limiter": (P, [I, F, F]), "fdsp_meter": (P, [I, D]), "fdsp_playwave": (P, [C.POINTER(C.c_float), C.c_uint64, C.c_uint64, C.c_uint64, C.c_int64]), "fdsp_resample": (P, [P]), "fdsp_phase_synth": (P, [I]), "fdsp_pulse": (P, []), "fdsp_mixer": (P, [I, I, C.POINTER(C.c_float)]), "fdsp_rotate": (P, [F, F]), "fdsp_chaos": (P, [I]), "fdsp_morph": (P, [F, F]), "fdsp_rez": (P, [F, F, F, I]), "fdsp_follow": (P, [I, F, F]), "fdsp_shaper": (P, [I, F, F]), "fdsp_onepole": (P, [I, F, I]), "fdsp_convolve": (P, [FP, I]), "fdsp_feedback_unit": (P, [D, P]), "fdsp_mls": (P, [I]), "fdsp_impulse": (P, [I]), "fdsp_tap": (P, [I, I, F, F]), "fdsp_feedback2": (P, [P, P, I]),
     "fdsp_pan": (P, [F]), "fdsp_panner": (P, []), "fdsp_adsr_live": (P, [F, F, F, F]),
     "fdsp_map": (P, [I, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]), "fdsp_shape_fn": (P, [C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
+    "fdsp_shaper_adaptive": (P, [D, I, F, F]), "fdsp_nl_biquad_adaptive": (P, [I, I, D, I, F, F, I, F, F, F]),
     "fdsp_envelope_in": (P, [D, I, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
     "fdsp_pipe": (P, [P, P]), "fdsp_stack": (P, [P, P]), "fdsp_branch": (P, [P, P]), "fdsp_bus": (P, [P, P]), "fdsp_thru": (P, [P]),
     "fdsp_binop": (P, [I, P, P]), "fdsp_unop": (P, [I, F, P]), "fdsp_multi": (P, [I, I, I, C.POINTER(P)]), "fdsp_feedback": (P, [P, I]),
@@ -184,6 +185,9 @@ class GpuBackend:
     def b_rotate(self, angle, gain): return _node(self.L.fdsp_rotate(angle, gain), "rotate")
     def b_netnode(self, net): return net.lower(self)
     def b_nl_biquad(self, fb, mode, shape, p0, p1, nin, ce, q, g): return _node(self.L.fdsp_nl_biquad(fb, mode, shape, p0, p1, nin, ce, q, g), "nl_biquad")
+    def b_shaper_adaptive(self, timescale, kind, p0, p1): return _node(self.L.fdsp_shaper_adaptive(timescale, kind, p0, p1), "shaper_adaptive")
+    def b_nl_biquad_adaptive(self, fb, mode, timescale, kind, p0, p1, nin, ce, q, g):
+        return _node(self.L.fdsp_nl_biquad_adaptive(fb, mode, timescale, kind, p0, p1, nin, ce, q, g), "nl_biquad_adaptive")
     def b_var(self, value): return _node(self.L.fdsp_var(value), "var")
     def b_dsf(self, n, spacing, rough): return _node(self.L.fdsp_dsf(n, spacing, rough), "dsf")
     def b_mls(self, bits): return _node(self.L.fdsp_mls(bits), "mls")

@@ -124,6 +124,18 @@ API fdsp_node* fdsp_shape_fn(const char* closure, int ncaptures, const char* con
 API fdsp_node* fdsp_envelope_in(double interval, int inputs, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values) {
   return closure_node(CL_ENVELOPE_IN, inputs, outputs, interval, closure, ncaptures, names, values);
 }
+API fdsp_node* fdsp_shaper_adaptive(double timescale, int inner_kind, float p0, float p1) {
+  std::string e;
+  HNode* n = mk_shaper_adaptive(timescale, inner_kind, p0, p1, e);
+  if (!n) { g_err = "shaper_adaptive: " + e; return nullptr; }
+  return wrap(n, "shaper_adaptive");
+}
+API fdsp_node* fdsp_nl_biquad_adaptive(int fb, int mode, double timescale, int inner_kind, float p0, float p1, int inputs, float center, float q, float gain) {
+  std::string e;
+  HNode* n = mk_nl_biquad_adaptive(fb, mode, timescale, inner_kind, p0, p1, inputs, center, q, gain, e);
+  if (!n) { g_err = "nl_biquad_adaptive: " + e; return nullptr; }
+  return wrap(n, "nl_biquad_adaptive");
+}
 API fdsp_node* fdsp_pipe(fdsp_node* x, fdsp_node* y) { return wrap(mk_pipe(take(x), take(y)), "pipe (>>)"); }
 API fdsp_node* fdsp_stack(fdsp_node* x, fdsp_node* y) { return wrap(mk_stack(take(x), take(y)), "stack (|)"); }
 API fdsp_node* fdsp_branch(fdsp_node* x, fdsp_node* y) { return wrap(mk_branch(take(x), take(y)), "branch (^)"); }

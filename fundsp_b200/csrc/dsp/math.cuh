@@ -96,6 +96,27 @@ FDSP_DEV float wide_sinf(float v) {
   return __uint_as_float(__float_as_uint(r) ^ sign);
 }
 
+// `wide` f32x8::atan as called by the block path of Shaper<Atan> (src/shape.rs:101-103): Cephes/VCL atan_f, lane-wise. Three ranges
+// of t = |v| give z = t (t < sqrt2 - 1, offset 0), (t - 1) / (t + 1) (offset pi/4) or -1 / t (t > sqrt2 + 1, offset pi/2); a NaN falls
+// in none of them and comes out of 0 / 0. polynomial_3 and mul_add without FMA, as wide_sinf; the sign is copied from v's sign bit.
+FDSP_DEV float wide_atanf(float v) {
+  const float P3 = 8.05374449538E-2f, P2 = -1.38776856032E-1f, P1 = 1.99777106478E-1f, P0 = -3.33329491539E-1f;
+  const float SQRT_2 = 1.41421356237309504880f, FRAC_PI_4 = 0.785398163397448309616f, FRAC_PI_2 = 1.57079632679489661923f;
+  const float t = fabsf(v);
+  const bool notsmal = t >= SQRT_2 - 1.0f, notbig = t <= SQRT_2 + 1.0f;
+  const float s = notsmal ? (notbig ? FRAC_PI_4 : FRAC_PI_2) : 0.0f;
+  float a = notbig ? t : 0.0f;
+  a = notsmal ? a - 1.0f : a;
+  float b = notbig ? 1.0f : 0.0f;
+  b = notsmal ? b + t : b;
+  const float z = a / b;
+  const float zz = z * z;
+  const float x2 = zz * zz;
+  float re = x2 * (P3 * zz + P2) + (P1 * zz + P0);
+  re = (re * (zz * z) + z) + s;
+  return (__float_as_uint(v) >> 31) ? -re : re;
+}
+
 // reference src/wavetable.rs:24-38 optimal4x44 (T = f32; f64 literals are rounded to f32 first)
 FDSP_DEV float optimal4x44(float a0, float a1, float a2, float a3, float x) {
   float z = x - 0.5f;
@@ -128,6 +149,9 @@ FDSP_DEV void optimal4x44_8(const float* a0, const float* a1, const float* a2, c
 }
 FDSP_DEV void wide_sinf8(const float* v, float* out) {
   FDSP_L8 out[j] = wide_sinf(v[j]);
+}
+FDSP_DEV void wide_atanf8(const float* v, float* out) {
+  FDSP_L8 out[j] = wide_atanf(v[j]);
 }
 
 }  // namespace fdsp

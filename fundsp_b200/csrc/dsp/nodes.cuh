@@ -1096,10 +1096,12 @@ template <int ASYM> struct Follower {
 };
 
 // ---------------------------------------------------------------- Shaper<S> (src/shape.rs, ID 42)
-// KIND 0 Clip(h), 1 ClipTo(lo, hi), 2 Tanh(h), 3 Softsign(h), 4 Crush(levels), 5 SoftCrush(levels); the block path follows
-// Shape::simd (round-to-even, F32x::floor, |x|*h), tail and tick follow Shape::shape.
+// KIND 0 Clip(h), 1 ClipTo(lo, hi), 2 Tanh(h), 3 Softsign(h), 4 Crush(levels), 5 SoftCrush(levels), 6 Atan(h) with p0 = h * PI * 0.5
+// (folded on the host, src/shape.rs:97-103); the block path follows Shape::simd (round-to-even, F32x::floor, |x|*h, wide's atan), tail
+// and tick follow Shape::shape.
 FDSP_DEV float smooth9f(float x) { const float x2 = x * x; return ((((70.0f * x - 315.0f) * x + 540.0f) * x - 420.0f) * x + 126.0f) * x2 * x2 * x; }
 template <int KIND> FDSP_DEV float shape_tick(float p0, float p1, float x) {   // Shape::shape (src/shape.rs), per shape kind
+  if (KIND == 6) return m::atanf_(x * p0) * (2.0f / PI_F);
   if (KIND == 0) return fminf(fmaxf(x * p0, -1.0f), 1.0f);
   if (KIND == 1) return fminf(fmaxf(x, p0), p1);
   if (KIND == 2) return m::tanhf_(x * p0);
@@ -1108,44 +1110,6 @@ template <int KIND> FDSP_DEV float shape_tick(float p0, float p1, float x) {   /
   const float v = x * p0, fl = floorf(v);
   return (fl + smooth9f(v - fl)) / p0;
 }
-// Nonlinear biquads (src/biquad.rs:494-920): transposed direct form II with a waveshaper in the loop.
-//   FB = 1: FbBiquad (ID 88) / FixedFbBiquad (ID 90): feedback is shape(y0);  FB = 0: DirtyBiquad (89) / FixedDirtyBiquad (91):
-//   both state updates are shaped. MODE 0 resonator, 1 lowpass, 2 highpass, 3 bell; SHAPE as in Shaper; NIN 1 = fixed coefficients,
-//   3 / 4 = audio-rate (center, q[, gain]) with the reference's change test squared(dc) + squared(dq) [+ squared(dg)] != 0.
-template <int FB, int MODE, int SHAPE, int NIN> struct NlBiquad {
-  FDSP_NODE(NIN, 1, 2 + (NIN == 1 ? 5 : 0), 2 + (NIN > 1 ? 8 : 0), 0);
-  struct R { float p0, p1; BqCoefs k; float center, q, gain, s1, s2; };
-  static FDSP_DEV void load(R& r, Loader& l) {
-    r.p0 = l.Pf(); r.p1 = l.Pf();
-    if (NIN == 1) { r.k.a1 = l.Pf(); r.k.a2 = l.Pf(); r.k.b0 = l.Pf(); r.k.b1 = l.Pf(); r.k.b2 = l.Pf(); r.center = r.q = r.gain = 0.0f; }
-    else { r.center = l.Sf(); r.q = l.Sf(); r.gain = l.Sf(); r.k.a1 = l.Sf(); r.k.a2 = l.Sf(); r.k.b0 = l.Sf(); r.k.b1 = l.Sf(); r.k.b2 = l.Sf(); }
-    r.s1 = l.Sf(); r.s2 = l.Sf();
-  }
-  static FDSP_DEV void save(const R& r, Saver& s) {
-    if (NIN > 1) { s.Sf(r.center); s.Sf(r.q); s.Sf(r.gain); s.Sf(r.k.a1); s.Sf(r.k.a2); s.Sf(r.k.b0); s.Sf(r.k.b1); s.Sf(r.k.b2); }
-    s.Sf(r.s1); s.Sf(r.s2);
-  }
-  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<NIN>& in, Fr<1>& o) {
-    if (NIN > 1) {
-      const float ce = in.v[NIN > 1 ? 1 : 0], qq = in.v[NIN > 2 ? 2 : 0], gg = NIN > 3 ? in.v[NIN > 3 ? 3 : 0] : r.gain;
-      const float dc = ce - r.center, dq = qq - r.q, dg = gg - r.gain;
-      const float test = NIN > 3 ? dc * dc + dq * dq + dg * dg : dc * dc + dq * dq;
-      if (test != 0.0f) { r.center = ce; r.q = qq; r.gain = gg; r.k = bq_mode(MODE, c.sr, ce, qq, gg); }
-    }
-    const float x0 = in.v[0];
-    const float y0 = r.k.b0 * x0 + r.s1;
-    if (FB) {
-      const float fb = shape_tick<SHAPE>(r.p0, r.p1, y0);
-      r.s1 = r.s2 + r.k.b1 * x0 - fb * r.k.a1;
-      r.s2 = r.k.b2 * x0 - fb * r.k.a2;
-    } else {
-      r.s1 = shape_tick<SHAPE>(r.p0, r.p1, r.s2 + r.k.b1 * x0 - y0 * r.k.a1);
-      r.s2 = shape_tick<SHAPE>(r.p0, r.p1, r.k.b2 * x0 - y0 * r.k.a2);
-    }
-    o.v[0] = y0;
-  }
-  static FDSP_DEV void end_simd(R&) {}
-};
 template <int KIND> struct Shaper {
   FDSP_NODE(1, 1, 2, 0, 0);
   struct R { float p0, p1; };
@@ -1160,11 +1124,93 @@ template <int KIND> struct Shaper {
     else if (KIND == 2) y = m::tanhf_(x * r.p0);
     else if (KIND == 3) y = tick ? (x * r.p0) / (1.0f + fabsf(x * r.p0)) : x * r.p0 / (1.0f + fabsf(x) * r.p0);
     else if (KIND == 4) y = (tick ? roundf(x * r.p0) : wide_roundf(x * r.p0)) / r.p0;
+    else if (KIND == 6) y = (tick ? m::atanf_(x * r.p0) : wide_atanf(x * r.p0)) * (2.0f / PI_F);
     else { const float v = x * r.p0, fl = tick ? floorf(v) : wide_floorf(v); y = (fl + smooth9f(v - fl)) / r.p0; }
     o.v[0] = y;
   }
   static FDSP_DEV void end_simd(R&) {}
 };
+// Shaper<Adaptive<S>> (src/shape.rs:156-200, ID 42): the level estimate `state` follows smoothing * state + (1 - smoothing) * (1e-6 + x^2)
+// and the inner shape INNER (0..6 as above) sees x / sqrt(state). Adaptive::simd is the trait default (lane by lane through `shape`), so
+// the inner shape takes its tick form on both paths. Words: P smoothing, p0, p1; S state (0.0 after construction, 1e-3 after reset()).
+FDSP_DEV float adaptive_level(float smoothing, float state, float x) { return smoothing * state + (1.0f - smoothing) * (1.0e-6f + x * x); }
+template <int INNER> struct ShaperAdaptive {
+  FDSP_NODE(1, 1, 3, 1, 0);
+  struct R { float sm, p0, p1, st; };
+  static FDSP_DEV void load(R& r, Loader& l) { r.sm = l.Pf(); r.p0 = l.Pf(); r.p1 = l.Pf(); r.st = l.Sf(); }
+  static FDSP_DEV void save(const R& r, Saver& s) { s.Sf(r.st); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<1>& in, Fr<1>& o) {
+    const float x = in.v[0];
+    r.st = adaptive_level(r.sm, r.st, x);
+    o.v[0] = shape_tick<INNER>(r.p0, r.p1, x / sqrtf(r.st));
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+// Nonlinear biquads (src/biquad.rs:494-920): transposed direct form II with a waveshaper in the loop.
+//   FB = 1: FbBiquad (ID 88) / FixedFbBiquad (ID 90): feedback is shape(y0);  FB = 0: DirtyBiquad (89) / FixedDirtyBiquad (91):
+//   both state updates are shaped, by two clones of the shape (shape1 for s1, then shape2 for s2, src/biquad.rs:711-720, :780-795).
+//   MODE 0 resonator, 1 lowpass, 2 highpass, 3 bell; NIN 1 = fixed coefficients, 3 / 4 = audio-rate (center, q[, gain]) with the
+//   reference's change test squared(dc) + squared(dq) [+ squared(dg)] != 0. The shape SH is evaluated on its tick path:
+//   BqShape<KIND>: a Shaper kind (0..6) with its words p0, p1;
+//   BqShapeAdaptive<INNER>: Adaptive around a Shaper kind, words smoothing, p0, p1 and one level estimate per clone. The biquads'
+//   set_sample_rate does not reach the shape (:536-539, :745-748), so `smoothing` is the one Adaptive::new computed at 44.1 kHz.
+// Words: P shape words [, a1, a2, b0, b1, b2 for NIN 1]; S [center, q, gain, a1, a2, b0, b1, b2 for NIN > 1], s1, s2, shape1 [, shape2] state.
+template <int KIND> struct BqShape {
+  static constexpr int NP = 2, NS = 0;
+  struct P { float p0, p1; };
+  struct S {};
+  static FDSP_DEV void load_p(P& p, Loader& l) { p.p0 = l.Pf(); p.p1 = l.Pf(); }
+  static FDSP_DEV void load_s(S&, Loader&) {}
+  static FDSP_DEV void save_s(const S&, Saver&) {}
+  static FDSP_DEV float shape(const P& p, S&, float x) { return shape_tick<KIND>(p.p0, p.p1, x); }
+};
+template <int INNER> struct BqShapeAdaptive {
+  static constexpr int NP = 3, NS = 1;
+  struct P { float sm, p0, p1; };
+  struct S { float st; };
+  static FDSP_DEV void load_p(P& p, Loader& l) { p.sm = l.Pf(); p.p0 = l.Pf(); p.p1 = l.Pf(); }
+  static FDSP_DEV void load_s(S& s, Loader& l) { s.st = l.Sf(); }
+  static FDSP_DEV void save_s(const S& s, Saver& sv) { sv.Sf(s.st); }
+  static FDSP_DEV float shape(const P& p, S& s, float x) { s.st = adaptive_level(p.sm, s.st, x); return shape_tick<INNER>(p.p0, p.p1, x / sqrtf(s.st)); }
+};
+template <int FB, int MODE, class SH, int NIN> struct NlBiquadT {
+  FDSP_NODE(NIN, 1, SH::NP + (NIN == 1 ? 5 : 0), 2 + (NIN > 1 ? 8 : 0) + (FB ? 1 : 2) * SH::NS, 0);
+  struct R { typename SH::P sp; BqCoefs k; float center, q, gain, s1, s2; typename SH::S sh1, sh2; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+    SH::load_p(r.sp, l);
+    if (NIN == 1) { r.k.a1 = l.Pf(); r.k.a2 = l.Pf(); r.k.b0 = l.Pf(); r.k.b1 = l.Pf(); r.k.b2 = l.Pf(); r.center = r.q = r.gain = 0.0f; }
+    else { r.center = l.Sf(); r.q = l.Sf(); r.gain = l.Sf(); r.k.a1 = l.Sf(); r.k.a2 = l.Sf(); r.k.b0 = l.Sf(); r.k.b1 = l.Sf(); r.k.b2 = l.Sf(); }
+    r.s1 = l.Sf(); r.s2 = l.Sf();
+    SH::load_s(r.sh1, l); if (!FB) SH::load_s(r.sh2, l);
+  }
+  static FDSP_DEV void save(const R& r, Saver& s) {
+    if (NIN > 1) { s.Sf(r.center); s.Sf(r.q); s.Sf(r.gain); s.Sf(r.k.a1); s.Sf(r.k.a2); s.Sf(r.k.b0); s.Sf(r.k.b1); s.Sf(r.k.b2); }
+    s.Sf(r.s1); s.Sf(r.s2);
+    SH::save_s(r.sh1, s); if (!FB) SH::save_s(r.sh2, s);
+  }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<NIN>& in, Fr<1>& o) {
+    if (NIN > 1) {
+      const float ce = in.v[NIN > 1 ? 1 : 0], qq = in.v[NIN > 2 ? 2 : 0], gg = NIN > 3 ? in.v[NIN > 3 ? 3 : 0] : r.gain;
+      const float dc = ce - r.center, dq = qq - r.q, dg = gg - r.gain;
+      const float test = NIN > 3 ? dc * dc + dq * dq + dg * dg : dc * dc + dq * dq;
+      if (test != 0.0f) { r.center = ce; r.q = qq; r.gain = gg; r.k = bq_mode(MODE, c.sr, ce, qq, gg); }
+    }
+    const float x0 = in.v[0];
+    const float y0 = r.k.b0 * x0 + r.s1;
+    if (FB) {
+      const float fb = SH::shape(r.sp, r.sh1, y0);
+      r.s1 = r.s2 + r.k.b1 * x0 - fb * r.k.a1;
+      r.s2 = r.k.b2 * x0 - fb * r.k.a2;
+    } else {
+      r.s1 = SH::shape(r.sp, r.sh1, r.s2 + r.k.b1 * x0 - y0 * r.k.a1);
+      r.s2 = SH::shape(r.sp, r.sh2, r.k.b2 * x0 - y0 * r.k.a2);
+    }
+    o.v[0] = y0;
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+template <int FB, int MODE, int SHAPE, int NIN> struct NlBiquad : NlBiquadT<FB, MODE, BqShape<SHAPE>, NIN> {};
+template <int FB, int MODE, int INNER, int NIN> struct NlBiquadAdaptive : NlBiquadT<FB, MODE, BqShapeAdaptive<INNER>, NIN> {};
 
 // ---------------------------------------------------------------- Convolver (src/convolve.rs:9-59, ID 100)
 // Direct-form linear convolution with an impulse response shared by the voice class (class-uniform words: K, ring length,
@@ -2404,8 +2450,10 @@ template <int K> struct Cost<Chaos<K>> { static constexpr int value = 32; };
 template <> struct Cost<Morph> { static constexpr int value = 64; };
 template <int N> struct Cost<Rez<N>> { static constexpr int value = N > 1 ? 180 : 120; };
 template <int A> struct Cost<Follower<A>> { static constexpr int value = 16; };
-template <int FB, int M, int S, int N> struct Cost<NlBiquad<FB, M, S, N>> { static constexpr int value = (S == 2 ? 120 : 30) * (FB ? 1 : 2) + (N > 1 ? 60 : 0); };
-template <int K> struct Cost<Shaper<K>> { static constexpr int value = K == 2 ? 100 : 12; };
+template <int FB, int M, int S, int N> struct Cost<NlBiquad<FB, M, S, N>> { static constexpr int value = (S == 2 ? 120 : S == 6 ? 60 : 30) * (FB ? 1 : 2) + (N > 1 ? 60 : 0); };
+template <int K> struct Cost<Shaper<K>> { static constexpr int value = K == 2 ? 100 : K == 6 ? 40 : 12; };
+template <int K> struct Cost<ShaperAdaptive<K>> { static constexpr int value = Cost<Shaper<K>>::value + 20; };
+template <int FB, int M, int S, int N> struct Cost<NlBiquadAdaptive<FB, M, S, N>> { static constexpr int value = Cost<NlBiquad<FB, M, S, N>>::value + (FB ? 20 : 40); };
 template <> struct Cost<Convolver> { static constexpr int value = 48; };
 template <class X> struct WaveKind<Resample<X>> : WaveKind<X> {};
 template <class X> struct Cost<Resample<X>> { static constexpr int value = 4 * Cost<X>::value + 120; };

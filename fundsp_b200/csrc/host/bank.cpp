@@ -218,6 +218,8 @@ std::string Bank::lower_and_upload(bool upload_state) {
       rows[i] = c.voices[i] * (uint32_t)nout;
     }
     c.state0 = S; c.state0_stale = true;
+    for (uint32_t i = 0; i < V; i++)   // the words whose reset value differs from their starting value (Lowering::resetS)
+      for (auto& w : lows[c.voices[i]].l.resetS) if (w.first < (uint32_t)NS) c.state0[(size_t)w.first * V + i] = w.second;
     if (!same_shape) {
       std::string e;
       if (!(e = dev_alloc(&c.d_params, P.size())).empty()) return e;
@@ -295,7 +297,11 @@ std::string Bank::lower_and_upload(bool upload_state) {
 std::string Bank::set_sample_rate(double s) {  // AudioUnit::set_sample_rate
   sr = s;
   const double unit_rate = net_rate ? (double)(float)s : s;
-  for (auto& n : nodes) n->set_sample_rate(unit_rate);
+  for (auto& n : nodes) {   // the bank of a sequencer is re-rated like the sequencer: its events' units are reset (a unit pushed later is not)
+    const bool reset = event_rerate_resets(n.get(), unit_rate);
+    n->set_sample_rate(unit_rate);
+    if (reset) n->reset();
+  }
   // Parameters always follow the new rate. State is re-initialised only while nothing has been rendered
   // (or when delay lengths change, which resets the lines like src/delay.rs:105-113).
   return lower_and_upload(!dirty);
@@ -322,7 +328,8 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
     // construction-time state (what reset() restores) follows the setting like the reference's stored phase/seed
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
     CU(cudaStreamSynchronize(stream));  // `l` is pageable and goes out of scope
-    for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = l.S[k];
+    const std::vector<uint32_t> S0 = l.reset_image();
+    for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];
     c.state0_stale = true;
     nodes[voice] = std::move(trial);
     return "";
@@ -366,7 +373,8 @@ std::string Bank::upload_voice(uint32_t voice, const Lowering& l, bool with_stat
       return "#U the voice does not fit its class: a class-uniform word (delay length, table, wave) or the word layout differs; rebuild the bank instead";
     if (with_state && c.fdn) return "#U voices of a two-stage (FDN reverb) class cannot be replaced in place";
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
-    for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = reset_state ? (*reset_state)[k] : l.S[k];
+    const std::vector<uint32_t> S0 = reset_state ? *reset_state : l.reset_image();
+    for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];
     c.state0_stale = true;
     if (with_state) {
       if (c.ns) CU(cudaMemcpy2DAsync(c.d_state + i, (size_t)Vc * 4, l.S.data(), 4, 4, c.ns, cudaMemcpyHostToDevice, stream));
@@ -409,7 +417,8 @@ std::string Bank::replace_voice(uint32_t voice, HNode* node) {
   n->lower(l);
   if (ev) event_set_clock(n.get(), 0.0);
   if (!l.ok) return "#U " + l.why;
-  std::string e = upload_voice(voice, l, true, &l0.S);
+  const std::vector<uint32_t> S0 = l0.reset_image();
+  std::string e = upload_voice(voice, l, true, &S0);
   if (!e.empty()) return e;
   nodes[voice] = std::move(n);
   return "";
@@ -482,7 +491,8 @@ std::string Bank::regroup(HNode* node, int at, uint32_t* voice, const Carry* car
     for (uint32_t i = 0; i < Vc; i++) {
       const uint32_t v = c.voices[i];
       if (v == nv) {   // the newcomer: live state (an event's clock = now); what reset() restores is its construction-time state
-        for (uint32_t k = 0; k < c.ns && k < l.S.size(); k++) { S[(size_t)k * Vc + i] = l.S[k]; c.state0[(size_t)k * Vc + i] = l0.S[k]; }
+        const std::vector<uint32_t> S0 = l0.reset_image();
+        for (uint32_t k = 0; k < c.ns && k < l.S.size(); k++) { S[(size_t)k * Vc + i] = l.S[k]; c.state0[(size_t)k * Vc + i] = S0[k]; }
         c.state0_stale = true;
         if (carry) {   // a unit that keeps RUNNING inside the newcomer (the fading-out side of a crossfade): its words and delay lines move over
           for (auto& sv : saved) {
@@ -615,7 +625,8 @@ std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode
     const uint32_t arm[3] = {1u, 0u, 0u};   // has_next = 1, fade_phase = 0.0
     CU(cudaMemcpy2DAsync(c.d_state + (size_t)1 * Vc + i, (size_t)Vc * 4, arm, 4, 4, 3, cudaMemcpyHostToDevice, stream));
     CU(cudaStreamSynchronize(stream));
-    for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = l.S[k];   // reset() adopts the newest unit (:156-172)
+    const std::vector<uint32_t> S0 = l.reset_image();
+    for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];   // reset() adopts the newest unit (:156-172)
     c.state0_stale = true;
     nodes[voice] = std::move(trial);
     return "";
@@ -731,7 +742,8 @@ std::string Bank::push_event(HNode* node, uint32_t* voice) {   // Sequencer::pus
     for (uint32_t v : c.voices) {
       if (!event_times(nodes[v].get(), &s0, &e0)) break;
       if (!(e0 <= seq_time + 0.5 * sd)) continue;   // Event::plan's end-of-event test at the start of the next block: still sounding
-      std::string e = upload_voice(v, l, true, &l0.S);
+      const std::vector<uint32_t> S0 = l0.reset_image();
+      std::string e = upload_voice(v, l, true, &S0);
       if (!e.empty()) return e;
       nodes[v] = std::move(n);
       if (voice) *voice = v;

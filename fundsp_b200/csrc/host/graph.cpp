@@ -520,14 +520,35 @@ struct LimiterN : HNode {  // src/dynamics.rs:128-243
   }
   HCLONE(LimiterN)
 };
+// the first parameter word of a shape kind: Atan(h) multiplies its input by h * PI * 0.5, evaluated left to right in f32 (src/shape.rs:98)
+static float shape_word0(int kind, float p0) { return kind == 6 ? p0 * fdsp::PI_F * 0.5f : p0; }
 struct ShaperN : HNode {  // src/shape.rs:205-249
   int kind; float p0, p1;
   ShaperN(int k, float a, float b) : kind(k), p0(a), p1(b) {}
   int inputs() const override { return 1; } int outputs() const override { return 1; }
   uint64_t id() const override { return 42; }
   void sig(std::string& o) const override { o += "Shaper<" + I(kind) + ">"; }
-  void lower(Lowering& l) const override { l.p(p0); l.p(p1); }
+  void lower(Lowering& l) const override { l.p(shape_word0(kind, p0)); l.p(p1); }
   HCLONE(ShaperN)
+};
+// Adaptive<S> (src/shape.rs:156-200): timescale is an f32 field, widened to f64 for the smoothing factor. `reset` is false from
+// construction (state 0.0) until the first HNode::reset (state 1e-3).
+struct AdaptiveShape {
+  int inner; float p0, p1, timescale; bool reset = false;
+  float smoothing(double sr) const { return (float)pow(0.5, 1.0 / ((double)timescale * sr)); }
+  void lower_params(Lowering& l, double sr) const { l.p(smoothing(sr)); l.p(shape_word0(inner, p0)); l.p(p1); }
+  void lower_state(Lowering& l) const { l.s_reset(reset ? 1.0e-3f : 0.0f, 1.0e-3f); }
+};
+struct ShaperAdaptiveN : HNode {  // Shaper<Adaptive<S>>: Shaper::set_sample_rate reaches the shape (src/shape.rs:226-228)
+  AdaptiveShape a; double sr = DEFAULT_SR;
+  explicit ShaperAdaptiveN(const AdaptiveShape& s) : a(s) {}
+  int inputs() const override { return 1; } int outputs() const override { return 1; }
+  uint64_t id() const override { return 42; }
+  void reset() override { a.reset = true; }
+  void set_sample_rate(double s) override { sr = s; }
+  void sig(std::string& o) const override { o += "ShaperAdaptive<" + I(a.inner) + ">"; }
+  void lower(Lowering& l) const override { a.lower_params(l, sr); a.lower_state(l); }
+  HCLONE(ShaperAdaptiveN)
 };
 struct NlBiquadN : HNode {  // src/biquad.rs:494-920
   int fb, mode, shape, nin; float p0, p1, sr = (float)DEFAULT_SR, center = 440.0f, q = 1.0f, gain = 1.0f; BqCoefs c;
@@ -547,12 +568,29 @@ struct NlBiquadN : HNode {  // src/biquad.rs:494-920
   }
   void sig(std::string& o) const override { o += "NlBiquad<" + I(fb) + "," + I(mode) + "," + I(shape) + "," + I(nin) + ">"; }
   void lower(Lowering& l) const override {
-    l.p(p0); l.p(p1);
+    l.p(shape_word0(shape, p0)); l.p(p1);
+    lower_filter(l);
+  }
+  void lower_filter(Lowering& l) const {
     if (nin == 1) { l.p(c.a1); l.p(c.a2); l.p(c.b0); l.p(c.b1); l.p(c.b2); }
     else { l.s(center); l.s(q); l.s(gain); l.s(c.a1); l.s(c.a2); l.s(c.b0); l.s(c.b1); l.s(c.b2); }
     l.s(0.0f); l.s(0.0f);
   }
   HCLONE(NlBiquadN)
+};
+// a nonlinear biquad with an Adaptive shape: one level estimate for FbBiquad, two (shape1, shape2) for DirtyBiquad. The biquads'
+// set_sample_rate does not reach the shape (src/biquad.rs:536-539, :745-748): the smoothing stays at Adaptive::new's 44.1 kHz.
+struct NlBiquadAdaptiveN : NlBiquadN {
+  AdaptiveShape a;
+  NlBiquadAdaptiveN(int fb_, int mode_, const AdaptiveShape& s, int nin_, float ce, float qq, float gg) : NlBiquadN(fb_, mode_, s.inner, s.p0, s.p1, nin_, ce, qq, gg), a(s) {}
+  void reset() override { a.reset = true; }
+  void sig(std::string& o) const override { o += "NlBiquadAdaptive<" + I(fb) + "," + I(mode) + "," + I(a.inner) + "," + I(nin) + ">"; }
+  void lower(Lowering& l) const override {
+    a.lower_params(l, DEFAULT_SR);
+    lower_filter(l);
+    a.lower_state(l); if (!fb) a.lower_state(l);
+  }
+  HCLONE(NlBiquadAdaptiveN)
 };
 struct ConvolverN : HNode {  // src/convolve.rs:9-59: the impulse response is class-uniform data (voices with the same response share a class)
   std::vector<float> h;
@@ -1153,6 +1191,10 @@ HNode* mk_event_loop(HNode* x, double start, double end, int fade_ease, double f
   if (n) static_cast<EventN*>(n)->loop_arg = loop_seconds;
   return n;
 }
+bool event_rerate_resets(const HNode* n, double s) {
+  const EventN* e = dynamic_cast<const EventN*>(n);
+  return e && s != e->sr && !(e->loop_arg > 0.0);
+}
 bool event_set_clock(HNode* n, double time) {
   EventN* e = dynamic_cast<EventN*>(n);
   if (!e) return false;
@@ -1190,15 +1232,32 @@ HNode* mk_rotate(float angle, float gain) {   // src/prelude.rs:2876-2884 (f32 c
   return mk_mixer(2, 2, w);
 }
 HNode* mk_nl_biquad(int fb, int mode, int shape, float p0, float p1, int inputs, float center, float q, float gain) {
-  if (mode < 0 || mode > 3 || shape < 0 || shape > 5 || !(inputs == 1 || inputs == (mode == 3 ? 4 : 3))) return nullptr;
+  if (mode < 0 || mode > 3 || shape < 0 || shape > 6 || !(inputs == 1 || inputs == (mode == 3 ? 4 : 3))) return nullptr;
   return new NlBiquadN(fb ? 1 : 0, mode, shape, p0, p1, inputs, center, q, gain);
+}
+static bool adaptive_shape(double timescale, int inner, float p0, float p1, AdaptiveShape* a, std::string& err) {
+  if (inner < 0 || inner > 6) { err = "Adaptive: the inner shape must be one of the kinds 0..6 (Clip .. Atan); an Adaptive or a shape_fn inside Adaptive is not supported"; return false; }
+  const float ts = (float)timescale;
+  if (!(ts > 0.0f) || !std::isfinite(ts)) { err = "Adaptive: the timescale must be a positive finite number of seconds"; return false; }
+  a->inner = inner; a->p0 = p0; a->p1 = p1; a->timescale = ts;
+  return true;
+}
+HNode* mk_shaper_adaptive(double timescale, int inner, float p0, float p1, std::string& err) {
+  AdaptiveShape a;
+  return adaptive_shape(timescale, inner, p0, p1, &a, err) ? new ShaperAdaptiveN(a) : nullptr;
+}
+HNode* mk_nl_biquad_adaptive(int fb, int mode, double timescale, int inner, float p0, float p1, int inputs, float center, float q, float gain, std::string& err) {
+  if (mode < 0 || mode > 3 || !(inputs == 1 || inputs == (mode == 3 ? 4 : 3))) { err = "nl_biquad: mode must be 0..3 and inputs 1 or 3 (4 for the bell)"; return nullptr; }
+  AdaptiveShape a;
+  if (!adaptive_shape(timescale, inner, p0, p1, &a, err)) return nullptr;
+  return new NlBiquadAdaptiveN(fb ? 1 : 0, mode, a, inputs, center, q, gain);
 }
 HNode* mk_declick(float duration) { return new DeclickN(duration); }
 HNode* mk_chaos(int kind) { return (kind < 0 || kind > 1) ? nullptr : new ChaosN(kind); }
 HNode* mk_morph(float cutoff, float q) { return new MorphN(cutoff, q); }
 HNode* mk_rez(float bandpass, float cutoff, float q, int inputs) { return (inputs != 1 && inputs != 3) ? nullptr : new RezN(bandpass, cutoff, q, inputs); }
 HNode* mk_follow(int asym, float attack, float release) { return new FollowerN(asym != 0, attack, asym ? release : attack); }
-HNode* mk_shaper(int kind, float p0, float p1) { return (kind < 0 || kind > 5) ? nullptr : new ShaperN(kind, p0, p1); }
+HNode* mk_shaper(int kind, float p0, float p1) { return (kind < 0 || kind > 6) ? nullptr : new ShaperN(kind, p0, p1); }
 HNode* mk_onepole(int kind, float param, int inputs) {
   if (kind < 0 || kind > 4 || inputs < 1 || inputs > 2 || ((kind == 3 || kind == 4) && inputs != 1) || (kind == 2 && inputs == 1 && !(param > 0.0f))) return nullptr;
   return new OnePoleN(kind, param, inputs);

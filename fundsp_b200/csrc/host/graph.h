@@ -57,10 +57,15 @@ struct Lowering {
   // [begin, end) of state words / of `dlen` entries that AudioUnit::reset leaves ALONE where the reference's reset does (Reverb::reset keeps
   // its pre-delay allpasses, src/reverb.rs:215-228; Limiter::reset keeps its follower, src/dynamics.rs:181-195): Bank::reset skips them
   std::vector<std::pair<uint32_t, uint32_t>> keepS, keepD;
+  // (state word, value) pairs where what reset() restores differs from the state a freshly built unit starts from (Adaptive's level
+  // estimate: 0.0 after Adaptive::new, 1e-3 after reset, src/shape.rs:173-196). Every other word resets to its lowered value.
+  std::vector<std::pair<uint32_t, uint32_t>> resetS;
   bool ok = true; std::string why; // set when a node has no device lowering
   void p(float f) { P.push_back(f2u(f)); }
   void s(float f) { S.push_back(f2u(f)); }
   void su(uint32_t u) { S.push_back(u); }
+  void s_reset(float now, float on_reset) { resetS.emplace_back((uint32_t)S.size(), f2u(on_reset)); s(now); }
+  std::vector<uint32_t> reset_image() const { std::vector<uint32_t> r = S; for (auto& w : resetS) if (w.first < r.size()) r[w.first] = w.second; return r; }
   void fail(const std::string& w) { if (ok) { ok = false; why = w; } }
 };
 
@@ -124,6 +129,9 @@ bool event_times(const HNode* n, double* start, double* end);
 HNode* mk_event_loop(HNode* x, double start, double end, int fade_ease, double fade_in, double fade_out, double loop_seconds);  // an event of a ReplayMode::Loop(loop_seconds) sequencer
 bool event_loop(const HNode* n, double* loop_seconds);               // false when n is not an event; 0 = the event's sequencer does not loop
 bool event_set_clock(HNode* n, double time);                         // the sequencer time the event's own clock starts from
+// Sequencer::set_sample_rate to a new rate (src/sequencer.rs:750-765) ends in Sequencer::reset, which without a loop resets the unit of every
+// event (:720-733): true when n is such an event and `s` differs from its rate. Sequencer::push only re-rates a unit (:369), never resets it.
+bool event_rerate_resets(const HNode* n, double s);
 // Envelope<F, E, R> (ID 14): `f(t, out[outputs], user)` is the closure E, evaluated ON THE HOST at the reference's sample points when the
 // graph is lowered (bank creation, sample-rate change, settings) for t <= horizon seconds; time_f64: F = f64 (else f32)
 typedef void (*EnvelopeFn)(double t, double* out, void* user);
@@ -142,7 +150,11 @@ HNode* mk_chaos(int kind);                                           // 0 Rossle
 HNode* mk_morph(float cutoff, float q);                               // Morph ID 62
 HNode* mk_rez(float bandpass, float cutoff, float q, int inputs);    // Rez ID 75 (bandpass 0 lowrez / 1 bandrez)
 HNode* mk_follow(int asymmetric, float attack, float release);        // Follow ID 24 / AFollow ID 29
-HNode* mk_shaper(int kind, float p0, float p1);                       // Shaper ID 42: 0 Clip 1 ClipTo 2 Tanh 3 Softsign 4 Crush 5 SoftCrush
+HNode* mk_shaper(int kind, float p0, float p1);                       // Shaper ID 42: 0 Clip 1 ClipTo 2 Tanh 3 Softsign 4 Crush 5 SoftCrush 6 Atan
+// Shaper<Adaptive<S>> ID 42 / nonlinear biquads with an Adaptive shape: `inner` is one of the Shaper kinds 0..6 with its (p0, p1);
+// on failure null with the reason in `err`
+HNode* mk_shaper_adaptive(double timescale, int inner, float p0, float p1, std::string& err);
+HNode* mk_nl_biquad_adaptive(int fb, int mode, double timescale, int inner, float p0, float p1, int inputs, float center, float q, float gain, std::string& err);
 HNode* mk_onepole(int kind, float param, int inputs);                  // 0 Lowpole 18, 1 Highpole 47, 2 Allpole 46, 3 DCBlock 22, 4 Pinkpass 26
 HNode* mk_convolve(const float* response, int n);                     // Convolver ID 100
 HNode* mk_feedback_unit(double delay, HNode* x);                      // FeedbackUnit ID 79                                          // Var ID 68

@@ -859,9 +859,22 @@ def Tanh(hardness): return ("shape", 2, f32(hardness), 0.0)
 def Softsign(hardness): return ("shape", 3, f32(hardness), 0.0)
 def Crush(levels): return ("shape", 4, f32(levels), 0.0)
 def SoftCrush(levels): return ("shape", 5, f32(levels), 0.0)
+def Atan(hardness): return ("shape", 6, f32(hardness), 0.0)
+
+
+def Adaptive(timescale, inner):
+    """`Adaptive::new(timescale, inner)` (src/shape.rs:156-200): the input divided by its running RMS level (halfway to a new level in
+    `timescale` seconds) before the inner shape. The inner shape is one of Clip .. Atan; an Adaptive cannot be nested."""
+    if not (isinstance(inner, tuple) and inner and inner[0] == "shape"):
+        raise ValueError("Adaptive: the inner shape must be one of Clip, ClipTo, Tanh, Softsign, Crush, SoftCrush or Atan")
+    _, kind, p0, p1 = inner
+    return ("adaptive", f32(timescale), kind, p0, p1)
 
 
 def shape(mode):
+    if mode[0] == "adaptive":
+        _, timescale, kind, p0, p1 = mode
+        return An("shaper_adaptive", (timescale, kind, p0, p1), (), 1, 1)
     _, kind, p0, p1 = mode
     return An("shaper", (kind, p0, p1), (), 1, 1)
 
@@ -936,6 +949,9 @@ def declick_s(t):
 
 # ---- src/prelude.rs:2900-3110 nonlinear biquads: d* = DirtyBiquad (shaped state), f* = FbBiquad (shaped feedback)
 def _nlb(fb, mode, shape_mode, nin, center=440.0, q=1.0, gain=1.0):
+    if shape_mode[0] == "adaptive":
+        _, timescale, kind, p0, p1 = shape_mode
+        return An("nl_biquad_adaptive", (fb, mode, timescale, kind, p0, p1, nin, f32(center), f32(q), f32(gain)), (), nin, 1)
     _, kind, p0, p1 = shape_mode
     return An("nl_biquad", (fb, mode, kind, p0, p1, nin, f32(center), f32(q), f32(gain)), (), nin, 1)
 

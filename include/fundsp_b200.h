@@ -71,7 +71,7 @@ fdsp_node* fdsp_reverb3(double time, double diffusion, fdsp_node* filter); /* Re
 fdsp_node* fdsp_feedback_unit(double delay, fdsp_node* x);   /* FeedbackUnit ID 79 src/feedback.rs:347: feedback with integrated delay (>= 1 sample) */
 fdsp_node* fdsp_convolve(const float* response, int n);       /* Convolver ID 100 src/convolve.rs:14: linear convolution with `response` (shared by all voices that pass the same one) */
 fdsp_node* fdsp_onepole(int kind, float param, int inputs);   /* src/filter.rs: kind 0 Lowpole ID 18 (cutoff), 1 Highpole 47 (cutoff), 2 Allpole 46 (delay), 3 DCBlock 22 (cutoff), 4 Pinkpass 26; inputs 2 = audio-rate parameter */
-fdsp_node* fdsp_shaper(int kind, float p0, float p1);         /* Shaper<S> ID 42 src/shape.rs: kind 0 Clip(h) 1 ClipTo(lo,hi) 2 Tanh(h) 3 Softsign(h) 4 Crush(levels) 5 SoftCrush(levels) */
+fdsp_node* fdsp_shaper(int kind, float p0, float p1);         /* Shaper<S> ID 42 src/shape.rs: kind 0 Clip(h) 1 ClipTo(lo,hi) 2 Tanh(h) 3 Softsign(h) 4 Crush(levels) 5 SoftCrush(levels) 6 Atan(h) */
 fdsp_node* fdsp_follow(int asymmetric, float attack, float release); /* Follow ID 24 (asymmetric 0: response time = attack) / AFollow ID 29, src/follow.rs */
 fdsp_node* fdsp_morph(float cutoff, float q);                  /* Morph ID 62 src/svf.rs:1040: inputs (audio, cutoff, q, morph -1..1) */
 fdsp_node* fdsp_rez(float bandpass, float cutoff, float q, int inputs); /* Rez ID 75 src/rez.rs: bandpass 0 = lowrez, 1 = bandrez; inputs 1 or 3 (audio, cutoff, q) */
@@ -108,6 +108,13 @@ fdsp_node* fdsp_rotate(float angle, float gain);               /* `rotate(angle,
 /* nonlinear biquads src/biquad.rs:494-920: fb 1 = FbBiquad 88 / FixedFbBiquad 90, 0 = DirtyBiquad 89 / FixedDirtyBiquad 91; mode 0 resonator,
    1 lowpass, 2 highpass, 3 bell; shape kind + (p0, p1) as in fdsp_shaper; inputs 1 = fixed (center, q, gain given), 3 (4 for bell) = audio rate */
 fdsp_node* fdsp_nl_biquad(int fb, int mode, int shape, float p0, float p1, int inputs, float center, float q, float gain);
+/* Adaptive<S> src/shape.rs:156-200 (`Adaptive::new(timescale, inner)`): the input is divided by its running RMS estimate (halfway to a new
+   level in `timescale` seconds, taken as f32) before the inner shape, one of the fdsp_shaper kinds 0..6 with its (p0, p1). The estimate
+   starts at 0 in a new unit and at 1e-3 after a reset. In Shaper<Adaptive> the smoothing follows the sample rate; the nonlinear biquads
+   keep the one computed at 44.1 kHz (their set_sample_rate does not reach the shape). NULL with the reason for an inner kind outside
+   0..6 (an Adaptive or a shape_fn cannot be nested) or a timescale that is not positive. */
+fdsp_node* fdsp_shaper_adaptive(double timescale, int inner_kind, float p0, float p1);
+fdsp_node* fdsp_nl_biquad_adaptive(int fb, int mode, double timescale, int inner_kind, float p0, float p1, int inputs, float center, float q, float gain);
 fdsp_node* fdsp_var(float value);                              /* Var ID 68 src/shared.rs:84: control value, changed with Setting::value (fdsp_node_set / fdsp_bank_set) */
 fdsp_node* fdsp_dsf(int inputs, float harmonic_spacing, float roughness); /* Dsf<N> ID 55 src/oscillator.rs:114 (dsf_saw / dsf_square) */
 fdsp_node* fdsp_mls(int bits);                                 /* Mls           ID 19 src/noise.rs:100 */

@@ -140,12 +140,16 @@ inline An brown() { return white() >> lowpole_hz(10.0f) * dc(13.7f); }
 inline An clip() { return An(fdsp_shaper(0, 1.0f, 0.0f)); }
 inline An clip_to(float lo, float hi) { return An(fdsp_shaper(1, lo, hi)); }
 struct Clip { float h; }; struct ClipTo { float lo, hi; }; struct Tanh { float h; }; struct Softsign { float h; }; struct Crush { float levels; }; struct SoftCrush { float levels; };
+struct Atan { float h; };
+/* Adaptive::new(timescale, inner) (src/shape.rs:156-200): inner is one of the structs above (not another Adaptive) */
+template <class S> struct Adaptive { double timescale; S inner; };
 inline An shape(Clip s) { return An(fdsp_shaper(0, s.h, 0.0f)); }
 inline An shape(ClipTo s) { return An(fdsp_shaper(1, s.lo, s.hi)); }
 inline An shape(Tanh s) { return An(fdsp_shaper(2, s.h, 0.0f)); }
 inline An shape(Softsign s) { return An(fdsp_shaper(3, s.h, 0.0f)); }
 inline An shape(Crush s) { return An(fdsp_shaper(4, s.levels, 0.0f)); }
 inline An shape(SoftCrush s) { return An(fdsp_shaper(5, s.levels, 0.0f)); }
+inline An shape(Atan s) { return An(fdsp_shaper(6, s.h, 0.0f)); }
 inline An follow(float response_time) { return An(fdsp_follow(0, response_time, response_time)); }
 inline An afollow(float attack, float release) { return An(fdsp_follow(1, attack, release)); }
 inline An morph() { return An(fdsp_morph(440.0f, 1.0f)); }
@@ -160,14 +164,21 @@ inline An declick() { return An(fdsp_declick(0.010f)); }
 inline An declick_s(float t) { return An(fdsp_declick(t)); }
 /* nonlinear biquads (src/prelude.rs:2900-3110): d* = DirtyBiquad (shaped state), f* = FbBiquad (shaped feedback); the shape is any of the
    Shaper structs above. The plain forms take (audio, center, q[, gain]) at audio rate. */
-struct ShapeMode { int kind; float p0, p1; };
+struct ShapeMode { int kind; float p0, p1; double timescale; };   /* timescale > 0: Adaptive around the kind */
 inline ShapeMode shape_mode(Clip s) { return {0, s.h, 0.0f}; }
 inline ShapeMode shape_mode(ClipTo s) { return {1, s.lo, s.hi}; }
 inline ShapeMode shape_mode(Tanh s) { return {2, s.h, 0.0f}; }
 inline ShapeMode shape_mode(Softsign s) { return {3, s.h, 0.0f}; }
 inline ShapeMode shape_mode(Crush s) { return {4, s.levels, 0.0f}; }
 inline ShapeMode shape_mode(SoftCrush s) { return {5, s.levels, 0.0f}; }
+inline ShapeMode shape_mode(Atan s) { return {6, s.h, 0.0f}; }
+template <class S> inline ShapeMode shape_mode(Adaptive<S> s) {   /* a nested Adaptive lowers to kind -1, which the C ABI refuses */
+    ShapeMode m = shape_mode(s.inner);
+    return {m.timescale > 0.0 ? -1 : m.kind, m.p0, m.p1, s.timescale};
+}
+template <class S> inline An shape(Adaptive<S> s) { ShapeMode m = shape_mode(s); return An(fdsp_shaper_adaptive(m.timescale, m.kind, m.p0, m.p1)); }
 inline An nl_biquad(int fb, int mode, ShapeMode m, int inputs, float center = 440.0f, float q = 1.0f, float gain = 1.0f) {
+    if (m.timescale > 0.0) return An(fdsp_nl_biquad_adaptive(fb, mode, m.timescale, m.kind, m.p0, m.p1, inputs, center, q, gain));
     return An(fdsp_nl_biquad(fb, mode, m.kind, m.p0, m.p1, inputs, center, q, gain));
 }
 #define FDSP_NLB(NAME, FB, MODE, NIN)                                                                                   \

@@ -57,6 +57,10 @@ extern "C" {
     fn fdsp_shape_fn(closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_envelope_in(interval: f64, inputs: c_int, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_convolve(response: *const f32, n: c_int) -> *mut FdspNode;
+    fn fdsp_shaper(kind: c_int, p0: f32, p1: f32) -> *mut FdspNode;
+    fn fdsp_shaper_adaptive(timescale: f64, inner_kind: c_int, p0: f32, p1: f32) -> *mut FdspNode;
+    fn fdsp_nl_biquad(fb: c_int, mode: c_int, shape: c_int, p0: f32, p1: f32, inputs: c_int, center: f32, q: f32, gain: f32) -> *mut FdspNode;
+    fn fdsp_nl_biquad_adaptive(fb: c_int, mode: c_int, timescale: f64, inner_kind: c_int, p0: f32, p1: f32, inputs: c_int, center: f32, q: f32, gain: f32) -> *mut FdspNode;
     fn fdsp_pipe(x: *mut FdspNode, y: *mut FdspNode) -> *mut FdspNode;
     fn fdsp_stack(x: *mut FdspNode, y: *mut FdspNode) -> *mut FdspNode;
     fn fdsp_branch(x: *mut FdspNode, y: *mut FdspNode) -> *mut FdspNode;
@@ -183,6 +187,34 @@ impl<N: Size<f32>> Lower for Constant<N> {
     unsafe fn lower(&self) -> *mut FdspNode { let v = self.value(); fdsp_constant(N::I32, v.as_ptr()) }        // audionode.rs:465
 }
 impl Lower for Pass { unsafe fn lower(&self) -> *mut FdspNode { fdsp_pass() } }
+/// A `Shape` as the C ABI names it: kind 0 Clip .. 6 Atan with its two parameters, or one of those inside `Adaptive` (timescale > 0).
+/// Needs the `timescale()` / `inner()` accessors of Adaptive and `shape()` of Shaper.
+pub trait ShapeCode { fn code(&self) -> (c_int, f32, f32, f64); }
+impl ShapeCode for crate::shape::Clip { fn code(&self) -> (c_int, f32, f32, f64) { (0, self.0, 0.0, 0.0) } }
+impl ShapeCode for crate::shape::ClipTo { fn code(&self) -> (c_int, f32, f32, f64) { (1, self.0, self.1, 0.0) } }
+impl ShapeCode for crate::shape::Tanh { fn code(&self) -> (c_int, f32, f32, f64) { (2, self.0, 0.0, 0.0) } }
+impl ShapeCode for crate::shape::Softsign { fn code(&self) -> (c_int, f32, f32, f64) { (3, self.0, 0.0, 0.0) } }
+impl ShapeCode for crate::shape::Crush { fn code(&self) -> (c_int, f32, f32, f64) { (4, self.0, 0.0, 0.0) } }
+impl ShapeCode for crate::shape::SoftCrush { fn code(&self) -> (c_int, f32, f32, f64) { (5, self.0, 0.0, 0.0) } }
+impl ShapeCode for crate::shape::Atan { fn code(&self) -> (c_int, f32, f32, f64) { (6, self.0, 0.0, 0.0) } }
+impl<S: crate::shape::Shape + ShapeCode> ShapeCode for crate::shape::Adaptive<S> {
+    fn code(&self) -> (c_int, f32, f32, f64) {   // shape.rs:156-200; a nested Adaptive gives kind -1, which the C ABI refuses
+        let (k, p0, p1, t) = self.inner().code();
+        (if t > 0.0 { -1 } else { k }, p0, p1, self.timescale() as f64)
+    }
+}
+impl<S: crate::shape::Shape + ShapeCode> Lower for crate::shape::Shaper<S> {
+    unsafe fn lower(&self) -> *mut FdspNode {   // shape.rs:205-249
+        let (k, p0, p1, t) = self.shape().code();
+        if t > 0.0 { fdsp_shaper_adaptive(t, k, p0, p1) } else { fdsp_shaper(k, p0, p1) }
+    }
+}
+/// The nonlinear biquads (biquad.rs:494-920) with a fixed (center, q[, gain]): `fb` 1 FixedFbBiquad, 0 FixedDirtyBiquad; `mode` 0
+/// resonator, 1 lowpass, 2 highpass, 3 bell. Needs the `shape()` / `center()` / `q()` / `gain()` accessors.
+pub unsafe fn lower_nl_biquad<S: ShapeCode>(fb: c_int, mode: c_int, shape: &S, center: f32, q: f32, gain: f32) -> *mut FdspNode {
+    let (k, p0, p1, t) = shape.code();
+    if t > 0.0 { fdsp_nl_biquad_adaptive(fb, mode, t, k, p0, p1, 1, center, q, gain) } else { fdsp_nl_biquad(fb, mode, k, p0, p1, 1, center, q, gain) }
+}
 impl<N: Size<f32>> Lower for MultiPass<N> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_multipass(N::I32) } }
 impl<N: Size<f32>> Lower for Sink<N> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_sink(N::I32) } }
 impl Lower for crate::oscillator::Sine<f32> {

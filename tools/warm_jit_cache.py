@@ -70,6 +70,17 @@ def jobs():
     add(sg(envelope2("|t, x| x * x * a + t", a=1.0)), (1,))
     for g in (saw_hz(50.0) >> map_("|x| tanh(x[0] * drive)", 1, 1, drive=1.0), saw_hz(50.0) >> shape(Tanh(1.0))):
         add(sg(g), (1, 2, 3))
+    # the Atan and Adaptive waveshapes (tests/test_gpu_shapes.py: rows, rows + mix, the resident process() kernel of its ragged cases;
+    # tools/bench_shapes.py: mix)
+    import test_gpu_shapes as SH
+    from fundsp_b200.prelude import Adaptive, Atan
+    for mk in SH.CASES.values():
+        add(sg(mk(0)), (1, 2, 3))
+    for name in ("shape_atan", "shape_adaptive_4", "nlb_resonator_audio_adaptive"):
+        s = sg(SH.CASES[name](0))
+        out[(s, 2, (1 if has_table(s) else 0) | (255 << 8))] = True
+    for g in (saw_hz(50.0) >> shape(Atan(1.0)), saw_hz(50.0) >> shape(Adaptive(0.01, Tanh(1.0)))):
+        add(sg(g), (1, 2, 3))
     # the exact mix model (tests/test_gpu_mix.py): 2..5-output stacks (rows, rows + mix, mix alone; twins of process() banks), the
     # 2-input stereo voice of the resident process() kernel, the plain classes beside two-stage and reverb classes
     import test_gpu_mix as MX
