@@ -47,6 +47,8 @@ _SIG = {
     "fdsp_constant": (P, [I, FP]), "fdsp_pass": (P, []), "fdsp_multipass": (P, [I]), "fdsp_sink": (P, [I]), "fdsp_split": (P, [I]),
     "fdsp_multisplit": (P, [I, I]), "fdsp_join": (P, [I]), "fdsp_multijoin": (P, [I, I]), "fdsp_reverse": (P, [I]), "fdsp_sine": (P, []),
     "fdsp_wavesynth": (P, [I, I]), "fdsp_noise": (P, []), "fdsp_fixed_svf": (P, [I, F, F, F]), "fdsp_svf": (P, [I, F, F, F]),
+    "fdsp_sine_f64": (P, []), "fdsp_fixed_svf_f64": (P, [I, F, F, F]), "fdsp_svf_f64": (P, [I, F, F, F]),
+    "fdsp_biquad_f64": (P, [F, F, F, F, F]), "fdsp_butterpass_f64": (P, [F, I]), "fdsp_resonator_f64": (P, [F, F, I]), "fdsp_onepole_f64": (P, [I, F, I]),
     "fdsp_biquad": (P, [F, F, F, F, F]), "fdsp_biquad_bank": (P, []), "fdsp_butterpass": (P, [F, I]), "fdsp_resonator": (P, [F, F, I]),
     "fdsp_moog": (P, [F, F, I]), "fdsp_fir": (P, [I, FP]), "fdsp_tick": (P, [I]), "fdsp_delay": (P, [D]), "fdsp_allnest": (P, [F, P, I]),
     "fdsp_phase_osc": (P, [I]), "fdsp_dsf": (P, [I, F, F]), "fdsp_reverb3": (P, [D, D, P]), "fdsp_var": (P, [F]), "fdsp_nl_biquad": (P, [I, I, I, F, F, I, F, F, F]), "fdsp_declick": (P, [F]), "fdsp_slot": (P, [P]), "fdsp_bank_slot_set": (I, [P, U32, I, D, P]), "fdsp_bank_crossfade_voice": (I, [P, U32, I, F, P]), "fdsp_oversample": (P, [P]), "fdsp_monitor": (P, []), "fdsp_envelope": (P, [D, I, I, ENVFN, P, D]), "fdsp_event": (P, [P, D, D, I, D, D]), "fdsp_event_loop": (P, [P, D, D, I, D, D, D]), "fdsp_limiter": (P, [I, F, F]), "fdsp_meter": (P, [I, D]), "fdsp_playwave": (P, [C.POINTER(C.c_float), C.c_uint64, C.c_uint64, C.c_uint64, C.c_int64]), "fdsp_resample": (P, [P]), "fdsp_phase_synth": (P, [I]), "fdsp_pulse": (P, []), "fdsp_mixer": (P, [I, I, C.POINTER(C.c_float)]), "fdsp_rotate": (P, [F, F]), "fdsp_chaos": (P, [I]), "fdsp_morph": (P, [F, F]), "fdsp_rez": (P, [F, F, F, I]), "fdsp_follow": (P, [I, F, F]), "fdsp_shaper": (P, [I, F, F]), "fdsp_onepole": (P, [I, F, I]), "fdsp_convolve": (P, [FP, I]), "fdsp_feedback_unit": (P, [D, P]), "fdsp_mls": (P, [I]), "fdsp_impulse": (P, [I]), "fdsp_tap": (P, [I, I, F, F]), "fdsp_feedback2": (P, [P, P, I]),
@@ -149,6 +151,13 @@ class GpuBackend:
     def b_noise(self): return _node(self.L.fdsp_noise(), "noise")
     def b_fixed_svf(self, mode, f, q, g): return _node(self.L.fdsp_fixed_svf(mode, f, q, g), "fixed_svf")
     def b_svf(self, mode, f, q, g): return _node(self.L.fdsp_svf(mode, f, q, g), "svf")
+    def b_sine_f64(self): return _node(self.L.fdsp_sine_f64(), "sine_f64")
+    def b_fixed_svf_f64(self, mode, f, q, g): return _node(self.L.fdsp_fixed_svf_f64(mode, f, q, g), "fixed_svf_f64")
+    def b_svf_f64(self, mode, f, q, g): return _node(self.L.fdsp_svf_f64(mode, f, q, g), "svf_f64")
+    def b_biquad_f64(self, a1, a2, b0, b1, b2): return _node(self.L.fdsp_biquad_f64(a1, a2, b0, b1, b2), "biquad_f64")
+    def b_butterpass_f64(self, f, nin): return _node(self.L.fdsp_butterpass_f64(f, nin), "butterpass_f64")
+    def b_resonator_f64(self, f, q, nin): return _node(self.L.fdsp_resonator_f64(f, q, nin), "resonator_f64")
+    def b_onepole_f64(self, kind, param, nin): return _node(self.L.fdsp_onepole_f64(kind, param, nin), "onepole_f64")
     def b_biquad(self, a1, a2, b0, b1, b2): return _node(self.L.fdsp_biquad(a1, a2, b0, b1, b2), "biquad")
     def b_biquad_bank(self): return _node(self.L.fdsp_biquad_bank(), "biquad_bank")
     def b_butterpass(self, f, nin): return _node(self.L.fdsp_butterpass(f, nin), "butterpass")

@@ -61,6 +61,13 @@ API fdsp_node* fdsp_wavesynth(int table, int outputs) { return wrap(mk_wavesynth
 API fdsp_node* fdsp_noise(void) { return wrap(mk_noise(), "noise"); }
 API fdsp_node* fdsp_fixed_svf(int mode, float c, float q, float g) { return wrap(mk_fixed_svf(mode, c, q, g), "fixed_svf"); }
 API fdsp_node* fdsp_svf(int mode, float c, float q, float g) { return wrap(mk_svf(mode, c, q, g), "svf"); }
+API fdsp_node* fdsp_sine_f64(void) { return wrap(mk_sine64(), "sine_f64"); }
+API fdsp_node* fdsp_fixed_svf_f64(int mode, float c, float q, float g) { return wrap(mk_fixed_svf64(mode, c, q, g), "fixed_svf_f64"); }
+API fdsp_node* fdsp_svf_f64(int mode, float c, float q, float g) { return wrap(mk_svf64(mode, c, q, g), "svf_f64"); }
+API fdsp_node* fdsp_biquad_f64(float a1, float a2, float b0, float b1, float b2) { return wrap(mk_biquad64(a1, a2, b0, b1, b2), "biquad_f64"); }
+API fdsp_node* fdsp_butterpass_f64(float c, int nin) { return wrap(mk_butterpass64(c, nin), "butterpass_f64"); }
+API fdsp_node* fdsp_resonator_f64(float c, float q, int nin) { return wrap(mk_resonator64(c, q, nin), "resonator_f64"); }
+API fdsp_node* fdsp_onepole_f64(int kind, float param, int inputs) { return wrap(mk_onepole64(kind, param, inputs), "onepole_f64"); }
 API fdsp_node* fdsp_biquad(float a1, float a2, float b0, float b1, float b2) { return wrap(mk_biquad(a1, a2, b0, b1, b2), "biquad"); }
 API fdsp_node* fdsp_biquad_bank(void) { return wrap(mk_biquad_bank(), "biquad_bank"); }
 API fdsp_node* fdsp_butterpass(float c, int nin) { return wrap((nin < 1 || nin > 2) ? nullptr : mk_butterpass(c, nin), "butterpass"); }

@@ -13,6 +13,7 @@
 // order; `NP/NS/NU` are the totals the host checks against.
 #pragma once
 #include "libm.cuh"
+#include "libm64.cuh"
 #include "bank_args.h"
 
 namespace fdsp {
@@ -2473,6 +2474,184 @@ template <int N> struct Cost<Dsf<N>> { static constexpr int value = 700; };
 template <int NT_, int LIN> struct Cost<Tap<NT_, LIN>> { static constexpr int value = 40 * NT_; };
 template <int HAD, class X> struct Cost<Feedback<HAD, X>> { static constexpr int value = Cost<X>::value + (HAD ? 6 * X::IN : X::IN); };
 
+
+// ---------------------------------------------------------------- prelude64: f64 state (F = f64 in the reference's generic nodes)
+// Node inputs and outputs stay f32: each input sample is widened to f64 (`convert`), each output rounded to f32. Every f64 parameter
+// or state word takes two u32 words, low word first (as Event's). The sample rate a node uses is its own f64 parameter word, lowered
+// from the rate the host node received (a Net hands its units the f32-rounded rate). These classes compile through NVRTC only.
+FDSP_DEV double ld64p(Loader& l) { const uint32_t lo = l.P(), hi = l.P(); return __longlong_as_double((long long)(((unsigned long long)hi << 32) | lo)); }
+FDSP_DEV double ld64s(Loader& l) { const uint32_t lo = l.S(), hi = l.S(); return __longlong_as_double((long long)(((unsigned long long)hi << 32) | lo)); }
+FDSP_DEV void sv64(Saver& s, double v) { const unsigned long long b = (unsigned long long)__double_as_longlong(v); s.S((uint32_t)b); s.S((uint32_t)(b >> 32)); }
+
+struct Sine64 {  // Sine<f64> src/oscillator.rs:18-102, ID 21: f64 phase and sample duration; the output is still sin(phase as f32 * f32::TAU)
+  FDSP_NODE(1, 1, 2, 2, 0);
+  struct R { double sd, phase; };
+  static FDSP_DEV void load(R& r, Loader& l) { r.sd = ld64p(l); r.phase = ld64s(l); }
+  static FDSP_DEV void save(const R& r, Saver& s) { sv64(s, r.phase); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<1>& in, Fr<1>& o) {
+    const double p = r.phase;
+    r.phase += (double)in.v[0] * r.sd;
+    if (T || c.rem) {  // tick path :67-72
+      r.phase -= floor(r.phase);
+      o.v[0] = m::sinf_((float)p * TAU_F);
+    } else {           // block path :74-86
+      o.v[0] = wide_sinf((float)p * TAU_F);
+    }
+  }
+  typedef void GroupStep;
+  template <class C> static FDSP_DEV void step8(R& r, C&, const Fr8<1>& in, Fr8<1>& o) {
+    float p[8];
+    FDSP_G8 { p[j] = (float)r.phase * TAU_F; r.phase += (double)in.v[0][j] * r.sd; }
+    wide_sinf8(p, o.v[0]);
+  }
+  static FDSP_DEV void end_simd(R& r) { r.phase = r.phase - floor(r.phase); }
+};
+struct Svf64K { double a1, a2, a3, m0, m1, m2; };
+FDSP_DEV void svf64_tick(const Svf64K& k, double& ic1, double& ic2, float x, float& y) {   // src/svf.rs:995-1006 with F = f64
+  const double v0 = (double)x;
+  const double v3 = v0 - ic2;
+  const double v1 = k.a1 * ic1 + k.a2 * v3;
+  const double v2 = ic2 + k.a2 * ic1 + k.a3 * v3;
+  ic1 = 2.0 * v1 - ic1;
+  ic2 = 2.0 * v2 - ic2;
+  y = (float)(k.m0 * v0 + k.m1 * v1 + k.m2 * v2);
+}
+struct FixedSvf64 {  // FixedSvf<f64, M> src/svf.rs:857-1031, ID 43: coefficients computed on the host (libm64.cuh)
+  FDSP_NODE(1, 1, 12, 4, 0);
+  struct R { Svf64K k; double ic1, ic2; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+    r.k.a1 = ld64p(l); r.k.a2 = ld64p(l); r.k.a3 = ld64p(l); r.k.m0 = ld64p(l); r.k.m1 = ld64p(l); r.k.m2 = ld64p(l);
+    r.ic1 = ld64s(l); r.ic2 = ld64s(l);
+  }
+  static FDSP_DEV void save(const R& r, Saver& s) { sv64(s, r.ic1); sv64(s, r.ic2); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<1>& in, Fr<1>& o) { svf64_tick(r.k, r.ic1, r.ic2, in.v[0], o.v[0]); }
+  static FDSP_DEV void end_simd(R&) {}
+};
+template <int MODE> struct Svf64 {  // Svf<f64, M> src/svf.rs:744-855, ID 36: f64 parameters from the f32 inputs, coefficients recomputed on change
+  // `ksr` is the rate the coefficients were computed at: a rate change recomputes them at the next sample, as set_sample_rate's
+  // update_frequency does at once (:823-826; the inputs of that sample then decide as usual)
+  static constexpr int NI = MODE >= 6 ? 4 : 3;
+  FDSP_NODE(NI, 1, 2, 24, 0);
+  struct R { double sr, cutoff, q, gain, ksr; Svf64K k; double ic1, ic2; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+    r.sr = ld64p(l);
+    r.cutoff = ld64s(l); r.q = ld64s(l); r.gain = ld64s(l); r.ksr = ld64s(l);
+    r.k.a1 = ld64s(l); r.k.a2 = ld64s(l); r.k.a3 = ld64s(l); r.k.m0 = ld64s(l); r.k.m1 = ld64s(l); r.k.m2 = ld64s(l);
+    r.ic1 = ld64s(l); r.ic2 = ld64s(l);
+  }
+  static FDSP_DEV void save(const R& r, Saver& s) {
+    sv64(s, r.cutoff); sv64(s, r.q); sv64(s, r.gain); sv64(s, r.ksr);
+    sv64(s, r.k.a1); sv64(s, r.k.a2); sv64(s, r.k.a3); sv64(s, r.k.m0); sv64(s, r.k.m1); sv64(s, r.k.m2);
+    sv64(s, r.ic1); sv64(s, r.ic2);
+  }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<NI>& in, Fr<1>& o) {   // update_inputs :299-313
+    const double cu = (double)in.v[1], qq = (double)in.v[2], gg = (double)in.v[NI - 1];
+    bool ch = cu != r.cutoff || qq != r.q || r.ksr != r.sr;
+    if (MODE >= 6) ch = ch || gg != r.gain;
+    if (ch) {
+      r.cutoff = cu; r.q = qq; if (MODE >= 6) r.gain = gg; r.ksr = r.sr;
+      const SvfCoefs64 k = svf_coefs64<MODE>(r.sr, r.cutoff, r.q, r.gain);
+      r.k.a1 = k.a1; r.k.a2 = k.a2; r.k.a3 = k.a3; r.k.m0 = k.m0; r.k.m1 = k.m1; r.k.m2 = k.m2;
+    }
+    svf64_tick(r.k, r.ic1, r.ic2, in.v[0], o.v[0]);
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+// ---- biquads with f64 state (src/biquad.rs:130-370, F = f64): DF1, left to right
+struct Bq64 { double a1, a2, b0, b1, b2, x1, x2, y1, y2; };
+FDSP_DEV void bq64_ld_coefs(Bq64& b, Loader& l, bool state) {
+  if (state) { b.a1 = ld64s(l); b.a2 = ld64s(l); b.b0 = ld64s(l); b.b1 = ld64s(l); b.b2 = ld64s(l); }
+  else { b.a1 = ld64p(l); b.a2 = ld64p(l); b.b0 = ld64p(l); b.b1 = ld64p(l); b.b2 = ld64p(l); }
+}
+FDSP_DEV void bq64_ld_state(Bq64& b, Loader& l) { b.x1 = ld64s(l); b.x2 = ld64s(l); b.y1 = ld64s(l); b.y2 = ld64s(l); }
+FDSP_DEV void bq64_sv_coefs(const Bq64& b, Saver& s) { sv64(s, b.a1); sv64(s, b.a2); sv64(s, b.b0); sv64(s, b.b1); sv64(s, b.b2); }
+FDSP_DEV void bq64_sv_state(const Bq64& b, Saver& s) { sv64(s, b.x1); sv64(s, b.x2); sv64(s, b.y1); sv64(s, b.y2); }
+FDSP_DEV void bq64_set(Bq64& b, const BqCoefs64& k) { b.a1 = k.a1; b.a2 = k.a2; b.b0 = k.b0; b.b1 = k.b1; b.b2 = k.b2; }
+FDSP_DEV float bq64_tick(Bq64& b, float x) {   // :184-194
+  const double x0 = (double)x;
+  const double y0 = b.b0 * x0 + b.b1 * b.x1 + b.b2 * b.x2 - b.a1 * b.y1 - b.a2 * b.y2;
+  b.x2 = b.x1; b.x1 = x0; b.y2 = b.y1; b.y1 = y0;
+  return (float)y0;
+}
+struct Biquad64 {  // Biquad<f64> ID 15, and the fixed ButterLowpass<f64, U1> ID 16 / Resonator<f64, U1> ID 17 (coefficients from the host)
+  FDSP_NODE(1, 1, 10, 8, 0);
+  typedef Bq64 R;
+  static FDSP_DEV void load(R& r, Loader& l) { bq64_ld_coefs(r, l, false); bq64_ld_state(r, l); }
+  static FDSP_DEV void save(const R& r, Saver& s) { bq64_sv_state(r, s); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<1>& in, Fr<1>& o) { o.v[0] = bq64_tick(r, in.v[0]); }
+  static FDSP_DEV void end_simd(R&) {}
+};
+// ButterLowpass<f64, U2> (KIND 0, inputs audio, cutoff) and Resonator<f64, U3> (KIND 1, inputs audio, center, q): coefficients recomputed
+// when an input changes (:270-278, :355-366) or the rate did (`ksr`, as in Svf64)
+template <int KIND> struct BiquadAudio64 {
+  static constexpr int NI = KIND == 0 ? 2 : 3;
+  FDSP_NODE(NI, 1, 2, 24, 0);
+  struct R { double sr, f, q, ksr; Bq64 b; };
+  static FDSP_DEV void load(R& r, Loader& l) { r.sr = ld64p(l); r.f = ld64s(l); r.q = ld64s(l); r.ksr = ld64s(l); bq64_ld_coefs(r.b, l, true); bq64_ld_state(r.b, l); }
+  static FDSP_DEV void save(const R& r, Saver& s) { sv64(s, r.f); sv64(s, r.q); sv64(s, r.ksr); bq64_sv_coefs(r.b, s); bq64_sv_state(r.b, s); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<NI>& in, Fr<1>& o) {
+    const double f = (double)in.v[1], q = KIND == 0 ? r.q : (double)in.v[NI - 1];
+    if (f != r.f || q != r.q || r.ksr != r.sr) {
+      r.f = f; r.q = q; r.ksr = r.sr;
+      bq64_set(r.b, KIND == 0 ? bq_butter_lowpass64(r.sr, r.f) : bq_resonator64(r.sr, r.f, r.q));
+    }
+    o.v[0] = bq64_tick(r.b, in.v[0]);
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+// ---- one-pole family with f64 state (src/filter.rs, F = f64): KIND 0 Lowpole (ID 18), 1 Highpole (ID 47), 2 Allpole (ID 46),
+// 3 DCBlock (ID 22); NIN = 2 adds the audio-rate parameter input (cutoff: recomputed on change or after a rate change; allpole delay:
+// every sample, :315-317)
+template <int KIND, int NIN> struct OnePole64 {
+  FDSP_NODE(NIN, 1, 2, (KIND == 0 ? 2 : 4) + (NIN > 1 ? 6 : 0), 0);
+  struct R { double sr, coeff, param, ksr, x1, y1; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+    if (NIN == 1) { r.coeff = ld64p(l); r.sr = r.param = r.ksr = 0.0; } else { r.sr = ld64p(l); r.param = ld64s(l); r.ksr = ld64s(l); r.coeff = ld64s(l); }
+    r.x1 = (KIND == 0) ? 0.0 : ld64s(l); r.y1 = ld64s(l);
+  }
+  static FDSP_DEV void save(const R& r, Saver& s) { if (NIN > 1) { sv64(s, r.param); sv64(s, r.ksr); sv64(s, r.coeff); } if (KIND != 0) sv64(s, r.x1); sv64(s, r.y1); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<NIN>& in, Fr<1>& o) {
+    if (NIN > 1) {
+      const double p = (double)in.v[NIN > 1 ? 1 : 0];
+      if (KIND == 2) r.coeff = onepole_coeff64(2, r.sr, p);
+      else if (p != r.param || r.ksr != r.sr) { r.param = p; r.ksr = r.sr; r.coeff = onepole_coeff64(KIND, r.sr, p); }
+    }
+    const double x = (double)in.v[0];
+    double y0;
+    if (KIND == 0) y0 = (1.0 - r.coeff) * x + r.coeff * r.y1;
+    else if (KIND == 1) y0 = r.coeff * (r.y1 + x - r.x1);
+    else if (KIND == 2) y0 = r.coeff * (x - r.y1) + r.x1;
+    else y0 = x - r.x1 + r.coeff * r.y1;
+    r.x1 = x; r.y1 = y0;
+    o.v[0] = (float)y0;
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+struct Pinkpass64 {  // Pinkpass<f64> src/filter.rs:178-262, ID 26
+  FDSP_NODE(1, 1, 0, 14, 0);
+  struct R { double b[7]; };
+  static FDSP_DEV void load(R& r, Loader& l) { for (int k = 0; k < 7; k++) r.b[k] = ld64s(l); }
+  static FDSP_DEV void save(const R& r, Saver& s) { for (int k = 0; k < 7; k++) sv64(s, r.b[k]); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<1>& in, Fr<1>& o) {
+    const double x = (double)in.v[0];
+    r.b[0] = 0.99886 * r.b[0] + x * 0.0555179;
+    r.b[1] = 0.99332 * r.b[1] + x * 0.0750759;
+    r.b[2] = 0.96900 * r.b[2] + x * 0.1538520;
+    r.b[3] = 0.86650 * r.b[3] + x * 0.3104856;
+    r.b[4] = 0.55000 * r.b[4] + x * 0.5329522;
+    r.b[5] = -0.7616 * r.b[5] - x * 0.0168980;
+    o.v[0] = (float)((r.b[0] + r.b[1] + r.b[2] + r.b[3] + r.b[4] + r.b[5] + r.b[6] + x * 0.5362) * 0.115830421);
+    r.b[6] = x * 0.115926;
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+template <> struct Cost<Sine64> { static constexpr int value = 48; };
+template <> struct Cost<FixedSvf64> { static constexpr int value = 24; };
+template <int M> struct Cost<Svf64<M>> { static constexpr int value = 80; };
+template <> struct Cost<Biquad64> { static constexpr int value = 16; };
+template <int K> struct Cost<BiquadAudio64<K>> { static constexpr int value = 90; };
+template <int K, int N> struct Cost<OnePole64<K, N>> { static constexpr int value = N > 1 ? 60 : 10; };
+template <> struct Cost<Pinkpass64> { static constexpr int value = 30; };
 
 // ---- traits of a Dag: sums / first match over its vertices
 template <int... X> struct FirstNonNeg { static constexpr int value = -1; };

@@ -4,6 +4,7 @@
 #include "graph.h"
 #include "closure.h"
 #include "../dsp/libm.cuh"
+#include "../dsp/libm64.cuh"
 
 #include <cmath>
 #include <limits>
@@ -233,6 +234,97 @@ struct Svf : HNode {  // FixedSvf (ID 43, :857-1031) and Svf (ID 36, :744-855)
     else { l.s(cutoff); l.s(q); l.s(gain); l.s(c.a1); l.s(c.a2); l.s(c.a3); l.s(c.m0); l.s(c.m1); l.s(c.m2); l.s(0.0f); l.s(0.0f); }
   }
   HCLONE(Svf)
+};
+
+// ---------------------------------------------------------------- prelude64 (F = f64): f64 parameters and state, two words each
+struct Sine64 : HNode {  // Sine<f64> src/oscillator.rs:18-102: the initial phase is rnd1(hash) unrounded, or the f32 `.phase()` widened
+  uint64_t hash = 0; bool has_phase = false; float initial_phase = 0; double sr = DEFAULT_SR;
+  int inputs() const override { return 1; } int outputs() const override { return 1; }
+  uint64_t id() const override { return 21; }
+  void set_sample_rate(double s) override { sr = s; }
+  void set(const Setting& s) override { if (s.kind == P_PHASE) { has_phase = true; initial_phase = s.v[0]; } }
+  void set_hash(uint64_t h) override { hash = h; }
+  void sig(std::string& o) const override { o += "Sine64"; }
+  void lower(Lowering& l) const override { l.p64(1.0 / sr); l.s64(has_phase ? (double)initial_phase : rnd1(hash)); }
+  HCLONE(Sine64)
+};
+SvfCoefs64 svf_coefs64(int mode, double sr, double cutoff, double q, double gain) {  // src/svf.rs:26-221 with F = f64 (shared host/device code)
+  switch (mode) {
+    case 0: return fdsp::svf_coefs64<0>(sr, cutoff, q, gain); case 1: return fdsp::svf_coefs64<1>(sr, cutoff, q, gain);
+    case 2: return fdsp::svf_coefs64<2>(sr, cutoff, q, gain); case 3: return fdsp::svf_coefs64<3>(sr, cutoff, q, gain);
+    case 4: return fdsp::svf_coefs64<4>(sr, cutoff, q, gain); case 5: return fdsp::svf_coefs64<5>(sr, cutoff, q, gain);
+    case 6: return fdsp::svf_coefs64<6>(sr, cutoff, q, gain); case 7: return fdsp::svf_coefs64<7>(sr, cutoff, q, gain);
+    default: return fdsp::svf_coefs64<8>(sr, cutoff, q, gain);
+  }
+}
+struct Svf64 : HNode {  // FixedSvf<f64, M> (ID 43) and Svf<f64, M> (ID 36): the sample rate is convert(sample_rate), settings F::from_f32
+  int mode; bool fixed; double sr, cutoff, q, gain;
+  Svf64(int m, bool f, float c, float q_, float g) : mode(m), fixed(f), sr(DEFAULT_SR), cutoff(c), q(q_), gain(g) {}
+  int inputs() const override { return fixed ? 1 : (mode >= 6 ? 4 : 3); } int outputs() const override { return 1; }
+  uint64_t id() const override { return fixed ? 43 : 36; }
+  void set_sample_rate(double s) override { sr = s; }
+  void set(const Setting& s) override {
+    if (!fixed) return;
+    if (s.kind == P_CENTER) cutoff = s.v[0];
+    else if (s.kind == P_CENTER_Q) { cutoff = s.v[0]; q = s.v[1]; }
+    else if (s.kind == P_CENTER_Q_GAIN) { cutoff = s.v[0]; q = s.v[1]; gain = s.v[2]; }
+  }
+  void sig(std::string& o) const override { if (fixed) o += "FixedSvf64"; else o += "Svf64<" + I(mode) + ">"; }
+  void lower(Lowering& l) const override {
+    const SvfCoefs64 c = svf_coefs64(mode, sr, cutoff, q, gain);
+    if (!fixed) { l.p64(sr); l.s64(cutoff); l.s64(q); l.s64(gain); l.s64(sr); }
+    if (fixed) { l.p64(c.a1); l.p64(c.a2); l.p64(c.a3); l.p64(c.m0); l.p64(c.m1); l.p64(c.m2); }
+    else { l.s64(c.a1); l.s64(c.a2); l.s64(c.a3); l.s64(c.m0); l.s64(c.m1); l.s64(c.m2); }
+    l.s64(0.0); l.s64(0.0);
+  }
+  HCLONE(Svf64)
+};
+
+// Biquad<f64> (ID 15), ButterLowpass<f64, N> (ID 16), Resonator<f64, N> (ID 17): kind 0 arbitrary, 1 butterpass, 2 resonator. The f32
+// arguments and settings are widened (F::from_f32); Biquad<f64>::set_sample_rate keeps its coefficients (src/biquad.rs:179-181).
+struct Biquad64N : HNode {
+  int kind, nin; BqCoefs64 c; double sr, f, q;
+  Biquad64N(int kind_, int nin_, const float* k, float f_, float q_) : kind(kind_), nin(nin_), c{0, 0, 0, 0, 0}, sr(DEFAULT_SR), f(f_), q(q_) {
+    if (k) { c.a1 = k[0]; c.a2 = k[1]; c.b0 = k[2]; c.b1 = k[3]; c.b2 = k[4]; }
+    update();
+  }
+  void update() { if (kind == 1) c = fdsp::bq_butter_lowpass64(sr, f); else if (kind == 2) c = fdsp::bq_resonator64(sr, f, q); }
+  int inputs() const override { return nin; } int outputs() const override { return 1; }
+  uint64_t id() const override { return kind == 0 ? 15 : (kind == 1 ? 16 : 17); }
+  void set_sample_rate(double s) override { sr = s; update(); }
+  void set(const Setting& s) override {
+    if (kind == 0 && s.kind == P_BIQUAD) { c.a1 = s.v[0]; c.a2 = s.v[1]; c.b0 = s.v[2]; c.b1 = s.v[3]; c.b2 = s.v[4]; }
+    else if (kind == 1 && s.kind == P_CENTER) { f = s.v[0]; update(); }
+    else if (kind == 2 && s.kind == P_CENTER_Q) { f = s.v[0]; q = s.v[1]; update(); }
+  }
+  void sig(std::string& o) const override { if (nin == 1) o += "Biquad64"; else o += "BiquadAudio64<" + I(kind == 1 ? 0 : 1) + ">"; }
+  void lower(Lowering& l) const override {
+    if (nin == 1) { l.p64(c.a1); l.p64(c.a2); l.p64(c.b0); l.p64(c.b1); l.p64(c.b2); }
+    else { l.p64(sr); l.s64(f); l.s64(q); l.s64(sr); l.s64(c.a1); l.s64(c.a2); l.s64(c.b0); l.s64(c.b1); l.s64(c.b2); }
+    for (int k = 0; k < 4; k++) l.s64(0.0);
+  }
+  HCLONE(Biquad64N)
+};
+// Lowpole / Highpole / Allpole / DCBlock / Pinkpass with F = f64 (src/filter.rs); kinds as mk_onepole
+struct OnePole64N : HNode {
+  int kind, nin; double param, sr = DEFAULT_SR;
+  OnePole64N(int k, float p, int n) : kind(k), nin(n), param(p) {}
+  int inputs() const override { return nin; } int outputs() const override { return 1; }
+  uint64_t id() const override { static const uint64_t ids[5] = {18, 47, 46, 22, 26}; return ids[kind]; }
+  void set_sample_rate(double s) override { sr = s; }
+  void set(const Setting& s) override {
+    if ((kind == 0 || kind == 1 || kind == 3) && s.kind == P_CENTER) param = s.v[0];
+    else if (kind == 2 && s.kind == P_DELAY) param = s.v[0];
+  }
+  void sig(std::string& o) const override { if (kind == 4) o += "Pinkpass64"; else o += "OnePole64<" + I(kind) + "," + I(nin) + ">"; }
+  void lower(Lowering& l) const override {
+    if (kind == 4) { for (int k = 0; k < 7; k++) l.s64(0.0); return; }
+    const double coeff = fdsp::onepole_coeff64(kind, sr, param);
+    if (nin == 1) l.p64(coeff); else { l.p64(sr); l.s64(param); l.s64(sr); l.s64(coeff); }
+    if (kind != 0) l.s64(0.0);
+    l.s64(0.0);
+  }
+  HCLONE(OnePole64N)
 };
 
 struct DeclickN : HNode {  // src/dynamics.rs:245-315
@@ -1121,6 +1213,16 @@ HNode* mk_wavesynth(int kind, int outputs) { return (kind < 0 || kind > 5 || out
 HNode* mk_noise() { return new Noise(); }
 HNode* mk_fixed_svf(int mode, float cutoff, float q, float gain) { return (mode < 0 || mode > 8) ? nullptr : new Svf(mode, true, cutoff, q, gain); }
 HNode* mk_svf(int mode, float cutoff, float q, float gain) { return (mode < 0 || mode > 8) ? nullptr : new Svf(mode, false, cutoff, q, gain); }
+HNode* mk_sine64() { return new Sine64(); }
+HNode* mk_biquad64(float a1, float a2, float b0, float b1, float b2) { const float k[5] = {a1, a2, b0, b1, b2}; return new Biquad64N(0, 1, k, 0, 0); }
+HNode* mk_butterpass64(float cutoff, int nin) { return (nin < 1 || nin > 2) ? nullptr : new Biquad64N(1, nin, nullptr, cutoff, 0); }
+HNode* mk_resonator64(float center, float q, int nin) { return (nin != 1 && nin != 3) ? nullptr : new Biquad64N(2, nin, nullptr, center, q); }
+HNode* mk_onepole64(int kind, float param, int inputs) {
+  if (kind < 0 || kind > 4 || inputs < 1 || inputs > 2 || ((kind == 3 || kind == 4) && inputs != 1)) return nullptr;
+  return new OnePole64N(kind, param, inputs);
+}
+HNode* mk_fixed_svf64(int mode, float cutoff, float q, float gain) { return (mode < 0 || mode > 8) ? nullptr : new Svf64(mode, true, cutoff, q, gain); }
+HNode* mk_svf64(int mode, float cutoff, float q, float gain) { return (mode < 0 || mode > 8) ? nullptr : new Svf64(mode, false, cutoff, q, gain); }
 HNode* mk_biquad(float a1, float a2, float b0, float b1, float b2) { BqCoefs c{0, 0, 0, 0, 0}; c.a1 = a1; c.a2 = a2; c.b0 = b0; c.b1 = b1; c.b2 = b2; return new Biquad(0, 1, c, 0, 0); }
 HNode* mk_biquad_bank() { return new BiquadBank(); }
 HNode* mk_butterpass(float cutoff, int nin) { return new Biquad(1, nin, BqCoefs{0, 0, 0, 0, 0}, cutoff, 0); }

@@ -64,6 +64,9 @@ struct Lowering {
   void p(float f) { P.push_back(f2u(f)); }
   void s(float f) { S.push_back(f2u(f)); }
   void su(uint32_t u) { S.push_back(u); }
+  // an f64 word pair, low word first (the prelude64 nodes)
+  void p64(double d) { uint64_t u; memcpy(&u, &d, 8); P.push_back((uint32_t)u); P.push_back((uint32_t)(u >> 32)); }
+  void s64(double d) { uint64_t u; memcpy(&u, &d, 8); S.push_back((uint32_t)u); S.push_back((uint32_t)(u >> 32)); }
   void s_reset(float now, float on_reset) { resetS.emplace_back((uint32_t)S.size(), f2u(on_reset)); s(now); }
   std::vector<uint32_t> reset_image() const { std::vector<uint32_t> r = S; for (auto& w : resetS) if (w.first < r.size()) r[w.first] = w.second; return r; }
   void fail(const std::string& w) { if (ok) { ok = false; why = w; } }
@@ -102,6 +105,15 @@ HNode* mk_wavesynth(int kind, int outputs);
 HNode* mk_noise();
 HNode* mk_fixed_svf(int mode, float cutoff, float q, float gain);
 HNode* mk_svf(int mode, float cutoff, float q, float gain);
+// prelude64: Sine<f64> (ID 21), FixedSvf<f64, M> (ID 43), Svf<f64, M> (ID 36); f32 arguments widened with F::from_f32
+HNode* mk_sine64();
+HNode* mk_fixed_svf64(int mode, float cutoff, float q, float gain);
+HNode* mk_svf64(int mode, float cutoff, float q, float gain);
+// Biquad<f64> ID 15, ButterLowpass<f64, U1|U2> ID 16, Resonator<f64, U1|U3> ID 17; the one-pole family as mk_onepole with F = f64
+HNode* mk_biquad64(float a1, float a2, float b0, float b1, float b2);
+HNode* mk_butterpass64(float cutoff, int nin);
+HNode* mk_resonator64(float center, float q, int nin);
+HNode* mk_onepole64(int kind, float param, int inputs);
 HNode* mk_biquad(float a1, float a2, float b0, float b1, float b2);
 HNode* mk_biquad_bank();
 HNode* mk_butterpass(float cutoff, int nin);

@@ -57,6 +57,15 @@ fdsp_node* fdsp_wavesynth(int table, int outputs);             /* WaveSynth<N>  
 fdsp_node* fdsp_noise(void);                                   /* Noise         ID 20 src/noise.rs:170 */
 fdsp_node* fdsp_fixed_svf(int mode, float cutoff, float q, float gain); /* FixedSvf ID 43; mode 0 lowpass 1 highpass 2 bandpass 3 notch 4 peak 5 allpass 6 bell 7 lowshelf 8 highshelf */
 fdsp_node* fdsp_svf(int mode, float cutoff, float q, float gain);       /* Svf ID 36 (audio, cutoff, q[, gain] inputs) */
+/* prelude64 (F = f64): the same nodes with f64 internal state, as `fundsp::prelude64` builds them. Arguments and node inputs/outputs stay
+   f32 and are widened to f64; coefficients are computed in f64 (libm tan), the sample rate is the f64 one the node receives. */
+fdsp_node* fdsp_sine_f64(void);                                /* Sine<f64>     ID 21: f64 phase; output sin(phase as f32 * TAU) */
+fdsp_node* fdsp_fixed_svf_f64(int mode, float cutoff, float q, float gain); /* FixedSvf<f64, M> ID 43; modes as fdsp_fixed_svf */
+fdsp_node* fdsp_svf_f64(int mode, float cutoff, float q, float gain);       /* Svf<f64, M> ID 36 (audio, cutoff, q[, gain] inputs) */
+fdsp_node* fdsp_biquad_f64(float a1, float a2, float b0, float b1, float b2); /* Biquad<f64> ID 15 */
+fdsp_node* fdsp_butterpass_f64(float cutoff, int inputs);      /* ButterLowpass<f64, U1|U2> ID 16 (inputs 1 = butterpass_hz) */
+fdsp_node* fdsp_resonator_f64(float center, float q, int inputs); /* Resonator<f64, U1|U3> ID 17 (inputs 1 = resonator_hz) */
+fdsp_node* fdsp_onepole_f64(int kind, float param, int inputs); /* the fdsp_onepole kinds 0..4 with F = f64 (Lowpole, Highpole, Allpole, DCBlock, Pinkpass) */
 fdsp_node* fdsp_biquad(float a1, float a2, float b0, float b1, float b2); /* Biquad<f32> ID 15 */
 fdsp_node* fdsp_biquad_bank(void);                             /* BiquadBank<f32x8> ID 98 */
 fdsp_node* fdsp_butterpass(float cutoff, int inputs);          /* ButterLowpass ID 16 (inputs 1 = butterpass_hz) */

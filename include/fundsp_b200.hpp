@@ -358,4 +358,60 @@ class Bank {
   fdsp_bank* get() { return b_; }
 };
 
+// fundsp::prelude64: the opcodes whose prelude64 type keeps f64 state (Sine<f64>, the SVFs, biquads and one-poles). Everything else is the
+// f32 opcode above; `using namespace fundsp_b200::prelude64;` after `using namespace fundsp_b200;` selects these where the names meet.
+namespace prelude64 {
+inline An sine() { return An(fdsp_sine_f64()); }
+inline An sine_hz(float f) { return dc(f) >> sine(); }
+namespace detail {
+inline An svf(int mode) { return An(fdsp_svf_f64(mode, 440.0f, 1.0f, 1.0f)); }
+inline An svf_hz(int mode, float f, float q, float gain = 1.0f) { return An(fdsp_fixed_svf_f64(mode, f, q, gain)); }
+inline An svf_q(int mode, float q) { return (multipass(2) | dc(q)) >> An(fdsp_svf_f64(mode, 440.0f, q, 1.0f)); }
+inline An svf_q(int mode, float q, float gain) { return (multipass(2) | dc(q, gain)) >> An(fdsp_svf_f64(mode, 440.0f, q, gain)); }
+}  // namespace detail
+inline An lowpass() { return detail::svf(0); }
+inline An lowpass_hz(float f, float q) { return detail::svf_hz(0, f, q); }
+inline An lowpass_q(float q) { return detail::svf_q(0, q); }
+inline An highpass() { return detail::svf(1); }
+inline An highpass_hz(float f, float q) { return detail::svf_hz(1, f, q); }
+inline An highpass_q(float q) { return detail::svf_q(1, q); }
+inline An bandpass() { return detail::svf(2); }
+inline An bandpass_hz(float f, float q) { return detail::svf_hz(2, f, q); }
+inline An bandpass_q(float q) { return detail::svf_q(2, q); }
+inline An notch() { return detail::svf(3); }
+inline An notch_hz(float f, float q) { return detail::svf_hz(3, f, q); }
+inline An notch_q(float q) { return detail::svf_q(3, q); }
+inline An peak() { return detail::svf(4); }
+inline An peak_hz(float f, float q) { return detail::svf_hz(4, f, q); }
+inline An peak_q(float q) { return detail::svf_q(4, q); }
+inline An allpass() { return detail::svf(5); }
+inline An allpass_hz(float f, float q) { return detail::svf_hz(5, f, q); }
+inline An allpass_q(float q) { return detail::svf_q(5, q); }
+inline An bell() { return detail::svf(6); }
+inline An bell_hz(float f, float q, float gain) { return detail::svf_hz(6, f, q, gain); }
+inline An bell_q(float q, float gain) { return detail::svf_q(6, q, gain); }
+inline An lowshelf() { return detail::svf(7); }
+inline An lowshelf_hz(float f, float q, float gain) { return detail::svf_hz(7, f, q, gain); }
+inline An lowshelf_q(float q, float gain) { return detail::svf_q(7, q, gain); }
+inline An highshelf() { return detail::svf(8); }
+inline An highshelf_hz(float f, float q, float gain) { return detail::svf_hz(8, f, q, gain); }
+inline An highshelf_q(float q, float gain) { return detail::svf_q(8, q, gain); }
+inline An biquad(float a1, float a2, float b0, float b1, float b2) { return An(fdsp_biquad_f64(a1, a2, b0, b1, b2)); }
+inline An butterpass() { return An(fdsp_butterpass_f64(440.0f, 2)); }
+inline An butterpass_hz(float f) { return An(fdsp_butterpass_f64(f, 1)); }
+inline An resonator() { return An(fdsp_resonator_f64(440.0f, 1.0f, 3)); }
+inline An resonator_hz(float center, float q) { return An(fdsp_resonator_f64(center, q, 1)); }
+inline An lowpole() { return An(fdsp_onepole_f64(0, 440.0f, 2)); }
+inline An lowpole_hz(float cutoff) { return An(fdsp_onepole_f64(0, cutoff, 1)); }
+inline An highpole() { return An(fdsp_onepole_f64(1, 440.0f, 2)); }
+inline An highpole_hz(float cutoff) { return An(fdsp_onepole_f64(1, cutoff, 1)); }
+inline An allpole() { return An(fdsp_onepole_f64(2, 1.0f, 2)); }
+inline An allpole_delay(float delay) { return An(fdsp_onepole_f64(2, delay, 1)); }
+inline An dcblock_hz(float cutoff) { return An(fdsp_onepole_f64(3, cutoff, 1)); }
+inline An dcblock() { return dcblock_hz(10.0f); }
+inline An pinkpass() { return An(fdsp_onepole_f64(4, 0.0f, 1)); }
+inline An pink() { return noise() >> pinkpass(); }
+inline An brown() { return noise() >> lowpole_hz(10.0f) * dc(13.7f); }
+}  // namespace prelude64
+
 }  // namespace fundsp_b200

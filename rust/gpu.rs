@@ -3,12 +3,14 @@
 //! Written against fundsp v0.23.0. NOT compiled in the fundsp_b200 repository (no Rust toolchain in its build image); the C++ and
 //! Python mirrors of this file are what its tests run. Lives in the crate (`src/gpu.rs`, feature `gpu`) because lowering reads
 //! construction-time parameters that are private fields; it needs these `pub(crate)` accessors added next to the fields:
-//!   Sine::initial_phase() -> Option<f32>            (oscillator.rs:25)     WaveSynth::initial_phase() / table_kind() (wavetable.rs:258)
-//!   Noise::seed() -> Option<u64>                    (noise.rs:175)         FixedSvf::params() -> &SvfParams<f32>     (svf.rs:867)
+//!   Sine::<F>::initial_phase() -> Option<F>         (oscillator.rs:25)     WaveSynth::initial_phase() / table_kind() (wavetable.rs:258)
+//!   Noise::seed() -> Option<u64>                    (noise.rs:175)         FixedSvf::<F, M>::params() -> &SvfParams<F> (svf.rs:867)
 //!   Moog::cutoff_q() -> (f32, f32)                  (moog.rs:20-34)        Fir::weights() -> &[f32]                  (fir.rs:15)
 //!   Delay::length_seconds() -> f64                  (delay.rs:69)          Panner::<U1>::pan_value() -> f32          (pan.rs:19)
 //!   Unop scalar: FrameAddScalar / FrameMulScalar / FrameNegAddScalar ::scalar() (audionode.rs:1114,1155,1197)
-//!   Resonator::center_q() -> (f32, f32)             (biquad.rs:310-318)    ButterLowpass::cutoff() -> f32            (biquad.rs:227-232)
+//!   Resonator::<F, N>::center_q() -> (F, F)         (biquad.rs:310-318)    ButterLowpass::<F, N>::cutoff() -> F      (biquad.rs:227-232)
+//!   (F = f32 and f64: the prelude64 impls call them on the f64 nodes) Lowpole / Highpole / DCBlock ::<F, ..>::cutoff() -> F
+//!   (filter.rs:20-130, :340-380)  Allpole::<F, N>::delay() -> F (filter.rs:270-296: store the delay beside `eta`)
 //!   AllNest::coefficient() / inner() -> &X          (delay.rs:294-302)     Tap / TapLinear::delay_range() -> (f32, f32) (delay.rs:148-160,386)
 //!   Dsf::spacing_roughness() -> (f32, f32)          (oscillator.rs:120)    Mls::bits() -> u32                        (noise.rs:101)
 //!   Feedback::inner() / Feedback2::inner_pair()     (feedback.rs:71,183)   Reverb::time_diffusion_filter()           (reverb.rs:154-162)
@@ -76,6 +78,13 @@ extern "C" {
     fn fdsp_reverse(n: c_int) -> *mut FdspNode;
     fn fdsp_impulse(n: c_int) -> *mut FdspNode;
     fn fdsp_svf(mode: c_int, cutoff: f32, q: f32, gain: f32) -> *mut FdspNode;
+    fn fdsp_sine_f64() -> *mut FdspNode;
+    fn fdsp_fixed_svf_f64(mode: c_int, cutoff: f32, q: f32, gain: f32) -> *mut FdspNode;
+    fn fdsp_svf_f64(mode: c_int, cutoff: f32, q: f32, gain: f32) -> *mut FdspNode;
+    fn fdsp_biquad_f64(a1: f32, a2: f32, b0: f32, b1: f32, b2: f32) -> *mut FdspNode;
+    fn fdsp_butterpass_f64(cutoff: f32, inputs: c_int) -> *mut FdspNode;
+    fn fdsp_resonator_f64(center: f32, q: f32, inputs: c_int) -> *mut FdspNode;
+    fn fdsp_onepole_f64(kind: c_int, param: f32, inputs: c_int) -> *mut FdspNode;
     fn fdsp_biquad(a1: f32, a2: f32, b0: f32, b1: f32, b2: f32) -> *mut FdspNode;
     fn fdsp_biquad_bank() -> *mut FdspNode;
     fn fdsp_butterpass(cutoff: f32, inputs: c_int) -> *mut FdspNode;
@@ -267,6 +276,26 @@ impl<N: Size<f32>> Lower for Impulse<N> { unsafe fn lower(&self) -> *mut FdspNod
 impl<M: crate::svf::SvfMode<f32> + SvfModeIndex> Lower for crate::svf::Svf<f32, M> {
     unsafe fn lower(&self) -> *mut FdspNode { fdsp_svf(M::INDEX, self.cutoff(), self.q(), self.gain()) }
 }
+// prelude64 (F = f64): Sine<f64>, FixedSvf<f64, M>, Svf<f64, M>. Their f64 parameters were set from f32 values (F::from_f32), so
+// `as f32` gives those values back exactly; the f64 state is built on the device (csrc/dsp/nodes.cuh Sine64, FixedSvf64, Svf64).
+impl SvfModeIndex for crate::svf::LowpassMode<f64> { const INDEX: c_int = 0; }
+impl SvfModeIndex for crate::svf::HighpassMode<f64> { const INDEX: c_int = 1; }
+impl SvfModeIndex for crate::svf::BandpassMode<f64> { const INDEX: c_int = 2; }
+impl SvfModeIndex for crate::svf::NotchMode<f64> { const INDEX: c_int = 3; }
+impl SvfModeIndex for crate::svf::PeakMode<f64> { const INDEX: c_int = 4; }
+impl SvfModeIndex for crate::svf::AllpassMode<f64> { const INDEX: c_int = 5; }
+impl SvfModeIndex for crate::svf::BellMode<f64> { const INDEX: c_int = 6; }
+impl SvfModeIndex for crate::svf::LowshelfMode<f64> { const INDEX: c_int = 7; }
+impl SvfModeIndex for crate::svf::HighshelfMode<f64> { const INDEX: c_int = 8; }
+impl Lower for crate::oscillator::Sine<f64> {
+    unsafe fn lower(&self) -> *mut FdspNode { let n = fdsp_sine_f64(); if let Some(p) = self.initial_phase() { fdsp_node_phase(n, p as f32); } n }
+}
+impl<M: crate::svf::SvfMode<f64> + SvfModeIndex> Lower for crate::svf::FixedSvf<f64, M> {
+    unsafe fn lower(&self) -> *mut FdspNode { let p = self.params(); fdsp_fixed_svf_f64(M::INDEX, p.cutoff as f32, p.q as f32, p.gain as f32) }
+}
+impl<M: crate::svf::SvfMode<f64> + SvfModeIndex> Lower for crate::svf::Svf<f64, M> {
+    unsafe fn lower(&self) -> *mut FdspNode { fdsp_svf_f64(M::INDEX, self.cutoff() as f32, self.q() as f32, self.gain() as f32) }
+}
 impl Lower for crate::biquad::Biquad<f32> {
     unsafe fn lower(&self) -> *mut FdspNode { let c = self.coefs(); fdsp_biquad(c.a1, c.a2, c.b0, c.b1, c.b2) }                        // biquad.rs:136-165
 }
@@ -275,6 +304,20 @@ impl<N: Size<f32>> Lower for crate::biquad::ButterLowpass<f32, N> { unsafe fn lo
 impl<N: Size<f32>> Lower for crate::biquad::Resonator<f32, N> {
     unsafe fn lower(&self) -> *mut FdspNode { let (c, q) = self.center_q(); fdsp_resonator(c, q, N::I32) }                              // N = U1 fixed, U3 audio-rate center / Q
 }
+// prelude64 biquads and one-poles (F = f64): their parameters came from f32 values (F::from_f32), so `as f32` is exact. Biquad<f64>'s
+// coefficients are f64 values set from f32 settings or by BiquadCoefs::<f64> formulas; only the former round-trip through f32.
+impl Lower for crate::biquad::Biquad<f64> {
+    unsafe fn lower(&self) -> *mut FdspNode { let c = self.coefs(); fdsp_biquad_f64(c.a1 as f32, c.a2 as f32, c.b0 as f32, c.b1 as f32, c.b2 as f32) }
+}
+impl<N: Size<f32>> Lower for crate::biquad::ButterLowpass<f64, N> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_butterpass_f64(self.cutoff() as f32, N::I32) } }
+impl<N: Size<f32>> Lower for crate::biquad::Resonator<f64, N> {
+    unsafe fn lower(&self) -> *mut FdspNode { let (c, q) = self.center_q(); fdsp_resonator_f64(c as f32, q as f32, N::I32) }
+}
+impl<N: Size<f32>> Lower for crate::filter::Lowpole<f64, N> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_onepole_f64(0, self.cutoff() as f32, N::I32) } }
+impl<N: Size<f32>> Lower for crate::filter::Highpole<f64, N> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_onepole_f64(1, self.cutoff() as f32, N::I32) } }
+impl<N: Size<f32>> Lower for crate::filter::Allpole<f64, N> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_onepole_f64(2, self.delay() as f32, N::I32) } }
+impl Lower for crate::filter::DCBlock<f64> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_onepole_f64(3, self.cutoff() as f32, 1) } }
+impl Lower for crate::filter::Pinkpass<f64> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_onepole_f64(4, 0.0, 1) } }
 impl<N: Size<f32>> Lower for crate::delay::Tick<N> { unsafe fn lower(&self) -> *mut FdspNode { fdsp_tick(N::I32) } }                    // delay.rs:19
 impl<N: Size<f32>, X: AudioNode<Inputs = U1, Outputs = U1> + Lower> Lower for crate::delay::AllNest<N, X> {
     unsafe fn lower(&self) -> *mut FdspNode { fdsp_allnest(self.coefficient(), self.inner().lower(), N::I32) }                          // delay.rs:294 (N = U2: audio-rate coefficient)

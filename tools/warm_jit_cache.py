@@ -81,6 +81,15 @@ def jobs():
         out[(s, 2, (1 if has_table(s) else 0) | (255 << 8))] = True
     for g in (saw_hz(50.0) >> shape(Atan(1.0)), saw_hz(50.0) >> shape(Adaptive(0.01, Tanh(1.0)))):
         add(sg(g), (1, 2, 3))
+    # prelude64: f64-state Sine and SVF classes (tests/test_gpu_prelude64.py: rows, rows + mix, the resident process() kernel of its
+    # ragged cases; tools/bench_prelude64.py: mix)
+    import test_gpu_prelude64 as P64
+    for mk in P64.CASES.values():
+        add(sg(mk(0)), (1, 2, 3))
+    for name in ("sine_fm", "svf_lowpass_audio", "svf_lowshelf_hz", "headline"):
+        s = sg(P64.CASES[name](0))
+        out[(s, 2, (1 if has_table(s) else 0) | (255 << 8))] = True
+    add(sg(saw_hz(50.0) >> lowpass_hz(1000.0, 1.0)), (1, 2, 3))
     # the exact mix model (tests/test_gpu_mix.py): 2..5-output stacks (rows, rows + mix, mix alone; twins of process() banks), the
     # 2-input stereo voice of the resident process() kernel, the plain classes beside two-stage and reverb classes
     import test_gpu_mix as MX
