@@ -52,6 +52,8 @@ _SIG = {
     "fdsp_biquad": (P, [F, F, F, F, F]), "fdsp_biquad_bank": (P, []), "fdsp_butterpass": (P, [F, I]), "fdsp_resonator": (P, [F, F, I]),
     "fdsp_moog": (P, [F, F, I]), "fdsp_fir": (P, [I, FP]), "fdsp_tick": (P, [I]), "fdsp_delay": (P, [D]), "fdsp_allnest": (P, [F, P, I]),
     "fdsp_phase_osc": (P, [I]), "fdsp_dsf": (P, [I, F, F]), "fdsp_reverb3": (P, [D, D, P]), "fdsp_var": (P, [F]), "fdsp_nl_biquad": (P, [I, I, I, F, F, I, F, F, F]), "fdsp_declick": (P, [F]), "fdsp_slot": (P, [P]), "fdsp_bank_slot_set": (I, [P, U32, I, D, P]), "fdsp_bank_crossfade_voice": (I, [P, U32, I, F, P]), "fdsp_oversample": (P, [P]), "fdsp_monitor": (P, []), "fdsp_envelope": (P, [D, I, I, ENVFN, P, D]), "fdsp_event": (P, [P, D, D, I, D, D]), "fdsp_event_loop": (P, [P, D, D, I, D, D, D]), "fdsp_limiter": (P, [I, F, F]), "fdsp_meter": (P, [I, D]), "fdsp_playwave": (P, [C.POINTER(C.c_float), C.c_uint64, C.c_uint64, C.c_uint64, C.c_int64]), "fdsp_resample": (P, [P]), "fdsp_phase_synth": (P, [I]), "fdsp_pulse": (P, []), "fdsp_mixer": (P, [I, I, C.POINTER(C.c_float)]), "fdsp_rotate": (P, [F, F]), "fdsp_chaos": (P, [I]), "fdsp_morph": (P, [F, F]), "fdsp_rez": (P, [F, F, F, I]), "fdsp_follow": (P, [I, F, F]), "fdsp_shaper": (P, [I, F, F]), "fdsp_onepole": (P, [I, F, I]), "fdsp_convolve": (P, [FP, I]), "fdsp_feedback_unit": (P, [D, P]), "fdsp_mls": (P, [I]), "fdsp_impulse": (P, [I]), "fdsp_tap": (P, [I, I, F, F]), "fdsp_feedback2": (P, [P, P, I]),
+    "fdsp_shared_new": (P, [F]), "fdsp_shared_wrap": (P, [C.POINTER(U32), P, P]), "fdsp_shared_free": (None, [P]), "fdsp_shared_set": (None, [P, F]),
+    "fdsp_shared_get": (F, [P]), "fdsp_var_shared": (P, [P]), "fdsp_monitor_shared": (P, [P, I, D]), "fdsp_timer": (P, [P]), "fdsp_var_fn": (P, [P, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
     "fdsp_pan": (P, [F]), "fdsp_panner": (P, []), "fdsp_adsr_live": (P, [F, F, F, F]),
     "fdsp_map": (P, [I, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]), "fdsp_shape_fn": (P, [C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
     "fdsp_shaper_adaptive": (P, [D, I, F, F]), "fdsp_nl_biquad_adaptive": (P, [I, I, D, I, F, F, I, F, F, F]),
@@ -198,6 +200,10 @@ class GpuBackend:
     def b_nl_biquad_adaptive(self, fb, mode, timescale, kind, p0, p1, nin, ce, q, g):
         return _node(self.L.fdsp_nl_biquad_adaptive(fb, mode, timescale, kind, p0, p1, nin, ce, q, g), "nl_biquad_adaptive")
     def b_var(self, value): return _node(self.L.fdsp_var(value), "var")
+    def b_var_shared(self, s): return _node(self.L.fdsp_var_shared(s.handle), "var")
+    def b_monitor_shared(self, s, kind, timescale): return _node(self.L.fdsp_monitor_shared(s.handle, kind, timescale), "monitor")
+    def b_timer(self, s): return _node(self.L.fdsp_timer(s.handle), "timer")
+    def b_var_fn(self, s, text, nout, caps): return _closure_node(self.L.fdsp_var_fn(s.handle, nout, text.encode(), *_caps(caps)))
     def b_dsf(self, n, spacing, rough): return _node(self.L.fdsp_dsf(n, spacing, rough), "dsf")
     def b_mls(self, bits): return _node(self.L.fdsp_mls(bits), "mls")
     def b_impulse(self, n): return _node(self.L.fdsp_impulse(n), "impulse")

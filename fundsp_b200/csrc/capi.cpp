@@ -106,6 +106,23 @@ API fdsp_node* fdsp_nl_biquad(int fb, int mode, int shape, float p0, float p1, i
   return wrap(mk_nl_biquad(fb, mode, shape, p0, p1, inputs, center, q, gain), "nl_biquad");
 }
 API fdsp_node* fdsp_var(float value) { return wrap(mk_var(value), "var"); }
+// ---- Shared controls (src/shared.rs): an fdsp_shared* is the address of a SharedCell; nodes and banks take references of their own
+API fdsp_shared* fdsp_shared_new(float value) { return reinterpret_cast<fdsp_shared*>(new (std::nothrow) SharedCell(value)); }
+API fdsp_shared* fdsp_shared_wrap(uint32_t* cell, void (*release)(void*), void* user) {
+  return cell ? reinterpret_cast<fdsp_shared*>(new (std::nothrow) SharedCell(cell, release, user)) : nullptr;
+}
+API void fdsp_shared_free(fdsp_shared* s) { if (s) reinterpret_cast<SharedCell*>(s)->unref(); }
+API void fdsp_shared_set(fdsp_shared* s, float value) { if (s) reinterpret_cast<SharedCell*>(s)->set(f2u(value)); }
+API float fdsp_shared_get(const fdsp_shared* s) { if (!s) return 0.0f; const uint32_t w = reinterpret_cast<const SharedCell*>(s)->get(); float f; memcpy(&f, &w, 4); return f; }
+API fdsp_node* fdsp_var_shared(fdsp_shared* s) { return wrap(mk_var_shared(reinterpret_cast<SharedCell*>(s)), "var_shared"); }
+API fdsp_node* fdsp_monitor_shared(fdsp_shared* s, int kind, double timescale) { return wrap(mk_monitor_shared(reinterpret_cast<SharedCell*>(s), kind, timescale), "monitor_shared"); }
+API fdsp_node* fdsp_var_fn(fdsp_shared* s, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values) {
+  std::string e;
+  HNode* n = mk_var_fn(reinterpret_cast<SharedCell*>(s), outputs, closure, ncaptures, names, values, e);
+  if (!n) { g_err = e; return nullptr; }
+  return wrap(n, "var_fn");
+}
+API fdsp_node* fdsp_timer(fdsp_shared* s) { return wrap(mk_timer(reinterpret_cast<SharedCell*>(s)), "timer"); }
 API fdsp_node* fdsp_dsf(int inputs, float spacing, float roughness) { return wrap(mk_dsf(inputs, spacing, roughness), "dsf"); }
 API fdsp_node* fdsp_mls(int bits) { return wrap(mk_mls(bits), "mls"); }
 API fdsp_node* fdsp_impulse(int n) { return wrap(mk_impulse(n), "impulse"); }
@@ -391,7 +408,10 @@ API int fdsp_bank_render(fdsp_bank* b, uint64_t n, const float* in, float* out_v
 API int fdsp_bank_render_device(fdsp_bank* b, uint64_t n, const float* in_dev, uint64_t in_stride, float* out_dev, uint64_t out_stride,
                                 float* mix_dev, uint64_t mix_stride) {
   if (!b) return fail(FDSP_ERR_ARG, "null bank");
-  return status(b->b.render_device(n, in_dev, in_stride, out_dev, out_stride, mix_dev, mix_stride));
+  std::string e = b->b.sh_pull();
+  if (e.empty()) e = b->b.render_device(n, in_dev, in_stride, out_dev, out_stride, mix_dev, mix_stride);
+  if (e.empty()) e = b->b.sh_push();   // (a bank with Shared writers synchronises here, to store what they left)
+  return status(e);
 }
 // ---- multi-GPU mix-down (host/group.h)
 struct fdsp_group { fdsp::host::Group* g; };

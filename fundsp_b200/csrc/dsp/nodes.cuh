@@ -1812,6 +1812,41 @@ template <int KIND> struct MeterNode {   // KIND 0 Sample, 1 Peak(timescale), 2 
   static FDSP_DEV void end_simd(R&) {}
 };
 
+// ---------------------------------------------------------------- writers of a Shared: Monitor (ID 56, src/dynamics.rs:441-520), Timer (ID 57,
+// src/shared.rs:203-250). Each leaves the value the reference would store last in a write-back state word of its own; the host stores
+// it into the Shared after the call. Device code never touches the Shared itself.
+template <int KIND> struct MonitorShared {   // the audio passes through; MeterNode<KIND>'s arithmetic on the input
+  FDSP_NODE(1, 1, 1, 2, 0);
+  struct R { typename MeterNode<KIND>::R m; };
+  static FDSP_DEV void load(R& r, Loader& l) { MeterNode<KIND>::load(r.m, l); (void)l.S(); }
+  // Meter::level: the state, or its square root for Rms (the block path of Meter::Sample ticks only the last sample, which leaves the same state)
+  static FDSP_DEV void save(const R& r, Saver& s) { MeterNode<KIND>::save(r.m, s); s.Sf(KIND == 2 ? sqrtf(r.m.state) : r.m.state); }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<1>& in, Fr<1>& o) {
+    Fr<1> level;
+    MeterNode<KIND>::template step<T>(r.m, c, in, level);
+    o.v[0] = in.v[0];
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+struct TimerShared {   // time += size * sample_duration once per block (Timer::process), += sample_duration per tick; stores time as f32
+  FDSP_NODE(0, 0, 2, 3, 0);
+  struct R { double sd, time; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+    uint32_t lo = l.P(), hi = l.P(); r.sd = __longlong_as_double((long long)(((unsigned long long)hi << 32) | lo));
+    lo = l.S(); hi = l.S(); r.time = __longlong_as_double((long long)(((unsigned long long)hi << 32) | lo));
+    (void)l.S();
+  }
+  static FDSP_DEV void save(const R& r, Saver& s) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(r.time);
+    s.S((uint32_t)b); s.S((uint32_t)(b >> 32)); s.Sf((float)r.time);
+  }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<0>&, Fr<0>&) {
+    if (T) r.time += r.sd;
+    else if (c.i == 0) r.time += (double)c.n * r.sd;
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+
 // The wave's samples are class-uniform data (voices playing the same wave share a class); the play region is per voice.
 struct WavePlayer {
   FDSP_NODE(0, 1, 2, 1, 1);   // NU counts the length word; the samples follow it in the uniform block
@@ -2217,6 +2252,27 @@ template <int NI, int NO, int NC, class E> struct Map {   // src/audionode.rs:13
   }
   static FDSP_DEV void end_simd(R&) {}
 };
+// VarFn<F, R> (src/shared.rs:134-200, ID 70): the closure of the Shared's value. The value is a parameter word the host rewrites between
+// calls (Bank::sh_pull), so within one launch value and captures are constant and the closure, evaluated once when the voice is loaded,
+// gives what VarFn::process computes for every block of the call.
+template <int NO, int NC, class E> struct VarFn {
+  FDSP_NODE(0, NO, 1 + NC, 0, 0);
+  struct R { float o[NO]; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+    const float x = l.Pf();
+    float c[NC > 0 ? NC : 1];
+#pragma unroll
+    for (int k = 0; k < NC; k++) c[k] = l.Pf();
+    const Ex::Root s{&x, c, 0.0f};
+    Ex::Emit<E>::out(s, r.o);
+  }
+  static FDSP_DEV void save(const R&, Saver&) {}
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C&, const Fr<0>&, Fr<NO>& o) {
+#pragma unroll
+    for (int k = 0; k < NO; k++) o.v[k] = r.o[k];
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
 // Shaper<ShapeFn<S>> (src/shape.rs:33-42, ID 42): ShapeFn::simd is the default per-lane `shape`, so tick and block paths coincide
 template <int NC, class E> struct ShaperFn : Map<1, 1, NC, E> {};
 
@@ -2418,6 +2474,8 @@ template <int K, int N> struct Cost<WaveSynth<K, N>> { static constexpr int valu
 template <int K> struct Cost<PhaseSynth<K>> { static constexpr int value = 110; };
 template <int M, int N> struct Cost<Mixer<M, N>> { static constexpr int value = 2 * M * N; };
 template <int K> struct Cost<MeterNode<K>> { static constexpr int value = 10; };
+template <int K> struct Cost<MonitorShared<K>> { static constexpr int value = 10; };
+template <> struct Cost<TimerShared> { static constexpr int value = 4; };
 template <> struct Cost<WavePlayer> { static constexpr int value = 12; };
 template <int N> struct Cost<Limiter<N>> { static constexpr int value = 150; };
 template <int N, int T> struct Cost<EnvelopeTab<N, T>> { static constexpr int value = 120; };
@@ -2431,6 +2489,7 @@ template <int N> struct Cost<Moog<N>> { static constexpr int value = 200; };
 template <> struct Cost<AdsrLive> { static constexpr int value = 120; };
 template <int NI, int NO, int NC, class E> struct Cost<Map<NI, NO, NC, E>> { static constexpr int value = 2 + E::cost; };
 template <int NC, class E> struct Cost<ShaperFn<NC, E>> { static constexpr int value = 2 + E::cost; };
+template <int NO, int NC, class E> struct Cost<VarFn<NO, NC, E>> { static constexpr int value = NO; };
 template <int NI, int NO, int NC, class E> struct Cost<EnvelopeInFn<NI, NO, NC, E>> { static constexpr int value = 120; };
 template <> struct Cost<Delay> { static constexpr int value = 12; };
 template <int N> struct Cost<Panner<N>> { static constexpr int value = N == 1 ? 2 : 80; };

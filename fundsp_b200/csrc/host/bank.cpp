@@ -63,6 +63,8 @@ Bank::~Bank() {
   rt_stop();
   if (device >= 0 && device < 64) { std::lock_guard<std::mutex> lock(g_rt_mu); if (g_rt_owner[device] == this) g_rt_owner[device] = nullptr; }
   if (rt_ctl) cudaFreeHost(rt_ctl);
+  if (sh_stage) cudaFreeHost(sh_stage);
+  if (sh_copied) cudaEventDestroy(sh_copied);
   cudaFree(d_rt_relay); cudaFree(d_rt_partial);
   for (auto& c : classes) {
     cudaFree(c.d_params); cudaFree(c.d_state); cudaFree(c.d_state0); cudaFree(c.d_uniform); cudaFree(c.d_rowmap); cudaFree(c.d_dline); cudaFree(c.d_partial); cudaFree(c.d_ring); cudaFree(c.d_dry); cudaFree(c.d_dryrows); cudaFree(c.d_dry2); cudaFree(c.d_partial2); cudaFree(c.d_cx); cudaFree(c.d_cxl); cudaFree(c.d_th); cudaFree(c.d_tl); cudaFree(c.d_crows); for (int q = 0; q < 2; q++) { if (c.e_dry[q]) cudaEventDestroy(c.e_dry[q]); if (c.e_fdn[q]) cudaEventDestroy(c.e_fdn[q]); } if (c.cstream) cudaStreamDestroy(c.cstream); if (c.e_done) cudaEventDestroy(c.e_done);
@@ -192,6 +194,9 @@ std::string Bank::lower_and_upload(bool upload_state) {
     fresh[ci].voices.push_back((uint32_t)v);
     std::string().swap(lo.key); std::vector<uint32_t>().swap(lo.l.U);   // the class keeps the uniform words (a sampler voice's may be a whole wave)
   }
+  sh_uses.assign(nodes.size(), {});
+  for (size_t v = 0; v < nodes.size(); v++) sh_uses[v] = lows[v].l.shared;
+  { std::string se = sh_check(0, sh_uses[0]); if (!se.empty()) return se; }
   if (fresh.size() > 1) {   // the tensor-core convolver form is for one-class banks (its mix-down is the voice-order fold of its own rows)
     for (auto& c : fresh) if (c.conv) {
       std::string jerr;
@@ -291,7 +296,7 @@ std::string Bank::lower_and_upload(bool upload_state) {
     if (changed) CU(cudaMemcpy(d_wt, h_wt, sizeof(h_wt), cudaMemcpyHostToDevice));
   }
   if (upload_state) dirty = false;
-  return "";
+  return sh_rebuild();
 }
 
 std::string Bank::set_sample_rate(double s) {  // AudioUnit::set_sample_rate
@@ -324,6 +329,7 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
     const uint32_t i = (uint32_t)(it - c.voices.begin()), Vc = c.V();
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns)
       return "#U set: the setting changes a class-uniform word (a delay length); rebuild the bank instead";
+    { std::string se = sh_check(voice, l.shared); if (!se.empty()) return se; }
     // parameters take effect at once (one strided column of the [NP][V] block); running state is left alone, the
     // construction-time state (what reset() restores) follows the setting like the reference's stored phase/seed
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
@@ -332,7 +338,8 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
     for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];
     c.state0_stale = true;
     nodes[voice] = std::move(trial);
-    return "";
+    sh_uses[voice] = l.shared;
+    return sh_rebuild();
   }
   return "internal: voice not found in any class";
 }
@@ -372,6 +379,7 @@ std::string Bank::upload_voice(uint32_t voice, const Lowering& l, bool with_stat
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns || (reset_state && reset_state->size() != c.ns))
       return "#U the voice does not fit its class: a class-uniform word (delay length, table, wave) or the word layout differs; rebuild the bank instead";
     if (with_state && c.fdn) return "#U voices of a two-stage (FDN reverb) class cannot be replaced in place";
+    { std::string se = sh_check(voice, l.shared); if (!se.empty()) return se; }
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
     const std::vector<uint32_t> S0 = reset_state ? *reset_state : l.reset_image();
     for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];
@@ -381,7 +389,8 @@ std::string Bank::upload_voice(uint32_t voice, const Lowering& l, bool with_stat
       if (c.dl_floats) CU(cudaMemset2DAsync(c.d_dline + i, (size_t)Vc * 4, 0, 4, (size_t)c.dl_floats, stream));
     }
     CU(cudaStreamSynchronize(stream));  // `l` is pageable
-    return "";
+    sh_uses[voice] = l.shared;
+    return sh_rebuild();
   }
   return "internal: voice not found in any class";
 }
@@ -611,6 +620,7 @@ std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode
     trial->lower(l);
     if (!l.ok) return "#U " + l.why;
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns) return "#U slot: the unit changes a class-uniform word (delay length, table, wave); rebuild the bank instead";
+    { std::string se = sh_check(voice, l.shared); if (!se.empty()) return se; }
     if (fading) {   // SlotBackend::handle_messages with `next` occupied: the update waits as `latest`, a newer one takes its place (:142-150)
       SlotLatest& w = slot_latest[voice];
       w.unit = std::move(parked); w.ease = ease; w.fade_time = fade_time;
@@ -629,7 +639,8 @@ std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode
     for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];   // reset() adopts the newest unit (:156-172)
     c.state0_stale = true;
     nodes[voice] = std::move(trial);
-    return "";
+    sh_uses[voice] = l.shared;
+    return sh_rebuild();
   }
   return "internal: voice not found in any class";
 }
@@ -778,6 +789,7 @@ std::string Bank::reset() {  // AudioUnit::reset: back to the construction-time 
   }
   CU(cudaStreamSynchronize(stream));
   dirty = false; seq_time = 0.0;
+  for (auto& uses : sh_uses) for (auto& u : uses) if (u.kind == SH_TIMER) u.cell->set(0u);   // Timer::reset (src/shared.rs:223-226)
   return "";
 }
 
@@ -845,6 +857,7 @@ std::string Bank::rt_process(uint32_t size, const float* in, float* out, bool* s
   if (classes.size() != 1 || !(out_mode & 2u) || tree_mix || nout > 8 || nin > 8) return "";
   VoiceClass& c = classes[0];
   if (c.fdn || c.conv || !c.k || !c.k->has_rt) return "";
+  if (!sh_cells.empty()) return "";   // Shared controls are exchanged between calls, on the launch path (sh_pull / sh_push)
   uint32_t vpc = (uint32_t)c.k->threads;
   const uint32_t grid = bank_grid(c.V(), (uint32_t)c.k->threads, sm_count(device), &vpc);
   if (grid > sm_count(device)) return "";           // every CTA must be resident at once
@@ -1189,6 +1202,7 @@ std::string Bank::render_host(uint64_t n, const float* in, float* out_voices, fl
   CU(cudaSetDevice(device));
   { std::string re = rt_stop(); if (!re.empty()) return re; }
   if (n == 0) return "";
+  { std::string se = sh_pull(); if (!se.empty()) return se; }
   const size_t rows = (size_t)V() * nout;
   // chunk so that the per-voice staging buffer stays below ~512 MB
   uint32_t chunk = TIME_CHUNK;
@@ -1211,7 +1225,7 @@ std::string Bank::render_host(uint64_t n, const float* in, float* out_voices, fl
     if (out_mix && (out_mode & 2u)) CU(cudaMemcpy2DAsync(out_mix + t0, (size_t)n * 4, d_mix, (size_t)chunk * 4, (size_t)len * 4, nout, cudaMemcpyDeviceToHost, stream));
   }
   CU(cudaStreamSynchronize(stream));
-  return "";
+  return sh_push();
 }
 
 std::string Bank::process(uint32_t size, const float* in, float* out) {  // AudioUnit::process (size <= 64)
@@ -1243,6 +1257,7 @@ std::string Bank::process(uint32_t size, const float* in, float* out) {  // Audi
     memcpy(h_in, in, (size_t)nin * 64 * 4);
     CU(cudaMemcpyAsync(d_in, h_in, (size_t)nin * 64 * 4, cudaMemcpyHostToDevice, stream));
   }
+  { std::string se = sh_pull(); if (!se.empty()) return se; }
   struct NoTiming { bool& t; explicit NoTiming(bool& x) : t(x) { t = false; } ~NoTiming() { t = true; } } no_timing(timing);  // no event records on this path
   struct InProcess { bool& f; explicit InProcess(bool& x) : f(x) { f = true; } ~InProcess() { f = false; } } in_proc(in_process);
   bool two_stage = false;   // pipelined classes clear / accumulate the mix region on the device: keep that in device memory
@@ -1263,7 +1278,7 @@ std::string Bank::process(uint32_t size, const float* in, float* out) {  // Audi
   }
   CU(cudaStreamSynchronize(stream));
   memcpy(out, h_out, rows * 64 * 4);
-  return "";
+  return sh_push();
 }
 
 std::string Bank::clone_into(Bank& dst) const {
@@ -1287,6 +1302,103 @@ std::string Bank::clone_into(Bank& dst) const {
   dst.dirty = dirty; dst.seq_time = seq_time;
   for (auto& kv : slot_latest) { SlotLatest& w = dst.slot_latest[kv.first]; w.unit.reset(kv.second.unit->clone()); w.ease = kv.second.ease; w.fade_time = kv.second.fade_time; }
   for (auto& kv : xfade_latest) { SlotLatest& w = dst.xfade_latest[kv.first]; w.unit.reset(kv.second.unit->clone()); w.ease = kv.second.ease; w.fade_time = kv.second.fade_time; }
+  return "";
+}
+
+// ---- Shared controls
+namespace {
+std::string cell_name(const SharedCell* c) { char b[40]; snprintf(b, sizeof b, "%p", (const void*)c); return std::string("the Shared at ") + b; }
+}
+std::string Bank::sh_check(uint32_t voice, const std::vector<SharedUse>& uses) const {
+  std::map<const SharedCell*, int> how;   // bit 0 read, bit 1 written
+  for (size_t v = 0; v < sh_uses.size(); v++)
+    for (auto& u : (v == voice ? uses : sh_uses[v])) how[u.cell] |= u.kind == SH_READ ? 1 : 2;
+  if (sh_uses.empty()) for (auto& u : uses) how[u.cell] |= u.kind == SH_READ ? 1 : 2;
+  for (auto& kv : how)
+    if (kv.second == 3) return "#U " + cell_name(kv.first) + " is both read (var / var_fn) and written (monitor / timer) in one bank: what a voice reads would depend on the voice order inside a block";
+  return "";
+}
+
+std::string Bank::sh_rebuild() {
+  std::map<const SharedCell*, int> index;
+  sh_cells.clear(); sh_last.clear(); sh_last_writer.clear();
+  size_t stage = 0;
+  auto cell_of = [&](SharedCell* c) { auto it = index.find(c); if (it != index.end()) return it->second; const int k = (int)sh_cells.size(); index[c] = k; sh_cells.emplace_back(c); sh_last_writer.emplace_back(); return k; };
+  for (size_t ci = 0; ci < classes.size(); ci++) {
+    VoiceClass& c = classes[ci];
+    const uint32_t Vc = c.V();
+    c.sh_rows.clear(); c.sh_cell.clear(); c.sh_img.clear();
+    std::map<uint32_t, size_t> row;
+    for (uint32_t i = 0; i < Vc; i++)
+      for (auto& u : sh_uses[c.voices[i]]) {
+        const int k = cell_of(u.cell);
+        if (u.kind != SH_READ) {   // the last voice in bank order, and within it the last writer in evaluation order
+          ShWriter& w = sh_last_writer[k];
+          if (w.cls < 0 || c.voices[i] >= w.voice) { w.cls = (int)ci; w.word = u.word; w.col = i; w.voice = c.voices[i]; }
+          continue;
+        }
+        auto it = row.find(u.word);
+        if (it == row.end()) { it = row.emplace(u.word, c.sh_rows.size()).first; c.sh_rows.push_back(u.word); c.sh_cell.resize(c.sh_rows.size() * Vc, -1); }
+        c.sh_cell[it->second * Vc + i] = k;
+      }
+    if (c.sh_rows.empty()) continue;
+    // the image starts from what the device holds: a row can mix readers with other voices' plain parameter words
+    c.sh_img.resize(c.sh_rows.size() * Vc);
+    stage += c.sh_img.size();
+    CU(cudaStreamSynchronize(stream));
+    for (size_t r = 0; r < c.sh_rows.size(); r++) CU(cudaMemcpy(c.sh_img.data() + r * Vc, c.d_params + (size_t)c.sh_rows[r] * Vc, (size_t)Vc * 4, cudaMemcpyDeviceToHost));
+  }
+  if (stage > sh_stage_cap) {
+    if (sh_pending) { CU(cudaEventSynchronize(sh_copied)); sh_pending = false; }
+    if (sh_stage) cudaFreeHost(sh_stage);
+    sh_stage = nullptr; sh_stage_cap = 0;
+    CU(cudaMallocHost((void**)&sh_stage, stage * 4));
+    sh_stage_cap = stage;
+  }
+  if (stage && !sh_copied) CU(cudaEventCreateWithFlags(&sh_copied, cudaEventDisableTiming));
+  return "";
+}
+
+std::string Bank::sh_pull() {
+  if (sh_cells.empty()) return "";
+  std::vector<uint32_t> now(sh_cells.size());
+  for (size_t k = 0; k < now.size(); k++) now[k] = sh_cells[k].c->get();   // one snapshot for the whole call
+  if (now == sh_last) return "";
+  CU(cudaSetDevice(device));
+  if (sh_pending) { CU(cudaEventSynchronize(sh_copied)); sh_pending = false; }   // (the previous call's row copies: long done by now)
+  size_t at = 0;
+  for (auto& c : classes) {
+    const uint32_t Vc = c.V();
+    for (size_t r = 0; r < c.sh_rows.size(); r++, at += Vc) {
+      bool changed = false;
+      for (uint32_t i = 0; i < Vc; i++) {
+        const int32_t k = c.sh_cell[r * Vc + i];
+        if (k >= 0 && c.sh_img[r * Vc + i] != now[k]) { c.sh_img[r * Vc + i] = now[k]; changed = true; }
+      }
+      if (!changed) continue;
+      if (at + Vc > sh_stage_cap) return "internal: Shared staging too small";
+      memcpy(sh_stage + at, c.sh_img.data() + r * Vc, (size_t)Vc * 4);
+      CU(cudaMemcpyAsync(c.d_params + (size_t)c.sh_rows[r] * Vc, sh_stage + at, (size_t)Vc * 4, cudaMemcpyHostToDevice, stream));
+      sh_pending = true;
+    }
+  }
+  if (sh_pending) CU(cudaEventRecord(sh_copied, stream));
+  sh_last = std::move(now);
+  return "";
+}
+
+std::string Bank::sh_push() {
+  if (!sh_writes()) return "";
+  CU(cudaSetDevice(device));
+  CU(cudaStreamSynchronize(stream));
+  for (size_t k = 0; k < sh_cells.size(); k++) {
+    const ShWriter& w = sh_last_writer[k];
+    if (w.cls < 0) continue;
+    const VoiceClass& c = classes[(size_t)w.cls];
+    uint32_t word = 0;
+    CU(cudaMemcpy(&word, c.d_state + (size_t)w.word * c.V() + w.col, 4, cudaMemcpyDeviceToHost));
+    sh_cells[k].c->set(word);
+  }
   return "";
 }
 

@@ -42,6 +42,9 @@ struct VoiceClass {
   std::vector<uint32_t> state0;     // initial state, SoA [NS][V]
   // what AudioUnit::reset leaves alone (Lowering::keepS / keepD): state word ranges and delay-line float ranges (per voice), ascending
   std::vector<std::pair<uint64_t, uint64_t>> keep_s, keep_d;
+  // Shared readers (Bank::sh_pull): the parameter rows in which some voice reads a Shared, the bank's cell index per voice there (-1: that
+  // voice's word there is no reader) and the host image of those rows, [row][V]
+  std::vector<uint32_t> sh_rows; std::vector<int32_t> sh_cell; std::vector<uint32_t> sh_img;
   // looping sequencer banks: the reset image also lives on the device (Event<X> resets its unit from it when the event ends, src/sequencer.rs:631-633)
   uint32_t* d_state0 = nullptr; bool state0_stale = true;
   uint32_t* d_params = nullptr; uint32_t* d_state = nullptr; uint32_t* d_uniform = nullptr; uint32_t* d_rowmap = nullptr;
@@ -118,6 +121,21 @@ struct Bank {
   std::string render_host(uint64_t n, const float* in, float* out_voices, float* out_mix);
   std::string process(uint32_t size, const float* in, float* out);
   std::string clone_into(Bank& dst) const;
+  // Shared controls (graph.h SharedCell). Before a call, sh_pull writes the cells' values into the readers' parameter words; after it,
+  // sh_push stores into each written cell the word its last writer in processing order (voice order, then evaluation order) left.
+  // A cell is either read or written in one bank: reading what another voice writes would depend on the voice order inside a block.
+  std::vector<std::vector<SharedUse>> sh_uses;   // per voice, in evaluation order
+  std::vector<SharedRef> sh_cells;               // every cell the voices use (the bank holds a reference)
+  std::vector<uint32_t> sh_last;                 // the cells' values at the last sh_pull (empty: compare every reader word)
+  struct ShWriter { int cls = -1; uint32_t word = 0, col = 0, voice = 0; };
+  std::vector<ShWriter> sh_last_writer;          // per cell: the write-back word stored after a call (cls < 0: the cell is read)
+  uint32_t* sh_stage = nullptr; size_t sh_stage_cap = 0;   // pinned staging of the reader rows sh_pull copies ([row][V] of every class in turn)
+  cudaEvent_t sh_copied = nullptr; bool sh_pending = false; // recorded behind those copies: the staging is rewritten only after they have landed
+  std::string sh_check(uint32_t voice, const std::vector<SharedUse>& uses) const;   // "" or the refusal when `voice` would use `uses`
+  std::string sh_rebuild();
+  std::string sh_pull();
+  std::string sh_push();
+  bool sh_writes() const { for (auto& w : sh_last_writer) if (w.cls >= 0) return true; return false; }
 };
 
 }  // namespace host

@@ -8,7 +8,7 @@
 namespace fdsp {
 namespace host {
 
-enum ClosureKind { CL_MAP = 0, CL_SHAPE_FN = 1, CL_ENVELOPE_IN = 2 };
+enum ClosureKind { CL_MAP = 0, CL_SHAPE_FN = 1, CL_ENVELOPE_IN = 2, CL_VAR_FN = 3 };   // CL_VAR_FN: var_fn's |x| of the Shared's value
 constexpr int CLOSURE_MAX_TEXT = 4096;   // bytes
 constexpr int CLOSURE_MAX_OPS = 256;     // operators, calls and literals: bounds the template depth NVRTC sees
 

@@ -773,7 +773,9 @@ struct EventN : HNode {  // one Sequencer event as a voice (src/sequencer.rs:55-
     const double cs0 = shifted ? cs : start, ce0 = shifted ? ce : end;
     uint64_t sb, eb; memcpy(&sb, &cs0, 8); memcpy(&eb, &ce0, 8);
     l.su((uint32_t)sb); l.su((uint32_t)(sb >> 32)); l.su((uint32_t)eb); l.su((uint32_t)(eb >> 32));   // current start / end (a loop wrap moves them while the event sounds)
+    const size_t k = l.shared.size();
     x->lower(l);
+    l.no_writers_since(k, "a sequencer event");
   }
   HCLONE(EventN)
 };
@@ -840,7 +842,9 @@ struct SlotN : HNode {  // src/slot.rs: two instances of one class in the voice 
   void lower(Lowering& l) const override {
     p64(l, sr); p64(l, fade_time); l.P.push_back((uint32_t)ease);
     l.su((uint32_t)newest); l.su(0u); l.su(0u); l.su(0u);   // which, has_next, fade_phase = 0.0
+    const size_t k = l.shared.size();
     u[0]->lower(l); u[1]->lower(l);
+    l.no_writers_since(k, "a slot");
   }
   HCLONE(SlotN)
 };
@@ -859,7 +863,9 @@ struct XfadeN : HNode {  // a Net vertex fading from unit x to unit y of any cla
     const float srf = (float)sr;                                                        // the Net's rate is f32 (src/net.rs:132)
     uint32_t w; memcpy(&w, &srf, 4); l.P.push_back(w); memcpy(&w, &fade_time, 4); l.P.push_back(w); l.P.push_back((uint32_t)ease);
     l.su(done ? 1u : 0u); l.su(0u);                                                     // done, fade_phase = 0.0f
+    const size_t k = l.shared.size();
     x->lower(l); y->lower(l);
+    l.no_writers_since(k, "a crossfade");
   }
   HCLONE(XfadeN)
 };
@@ -871,6 +877,58 @@ struct VarN : HNode {  // the shared value is control-plane state: it enters as 
   void sig(std::string& o) const override { o += "Constant<1>"; }   // per block it is a constant (src/shared.rs:118-121)
   void lower(Lowering& l) const override { l.p(value); }
   HCLONE(VarN)
+};
+// Var over a Shared (src/shared.rs:84-131): the cell's value is a parameter word. The bank rewrites it from the cell before every call
+// (Bank::sh_pull), so a set between two calls holds from the first sample of the next call to its end, as a render sees it when nobody
+// sets during the call. The device never reaches the cell.
+struct VarSharedN : HNode {
+  SharedRef s; explicit VarSharedN(SharedCell* c) : s(c) {}
+  int inputs() const override { return 0; } int outputs() const override { return 1; }
+  uint64_t id() const override { return 68; }
+  void sig(std::string& o) const override { o += "Constant<1>"; }
+  void lower(Lowering& l) const override { l.shared.push_back({(uint32_t)l.P.size(), s.c, SH_READ}); l.P.push_back(s.c->get()); }
+  HCLONE(VarSharedN)
+};
+// Monitor (src/dynamics.rs:441-520) and Timer (src/shared.rs:203-250) over a Shared: the device leaves the value they would store in a
+// state word of their own (nodes.cuh MonitorShared / TimerShared); after a call the bank stores the last writer's word into the cell.
+struct VarFnN : HNode {   // VarFn (src/shared.rs:134-200): the closure (closure.cpp) of the cell's value; its word as Var's, then the captures
+  SharedRef s; int nout; std::string expr; std::vector<float> caps;
+  VarFnN(SharedCell* c, int n, std::string e, std::vector<float> cp) : s(c), nout(n), expr(std::move(e)), caps(std::move(cp)) {}
+  int inputs() const override { return 0; } int outputs() const override { return nout; }
+  uint64_t id() const override { return 70; }
+  void sig(std::string& o) const override { o += "VarFn<" + I(nout) + "," + I((int)caps.size()) + "," + expr + ">"; }
+  void lower(Lowering& l) const override {
+    l.shared.push_back({(uint32_t)l.P.size(), s.c, SH_READ}); l.P.push_back(s.c->get());
+    for (float c : caps) l.p(c);
+  }
+  HCLONE(VarFnN)
+};
+struct MonitorSharedN : HNode {
+  SharedRef s; int kind; double timescale, sr = DEFAULT_SR;
+  MonitorSharedN(SharedCell* c, int k, double t) : s(c), kind(k), timescale(t) {}
+  int inputs() const override { return 1; } int outputs() const override { return 1; }
+  uint64_t id() const override { return 56; }
+  void set_sample_rate(double r) override { sr = r; }
+  void sig(std::string& o) const override { o += "MonitorShared<" + I(kind) + ">"; }
+  void lower(Lowering& l) const override {   // MeterState: smoothing, state; then the write-back word
+    l.p(kind == 0 ? 0.0f : (float)pow(0.5, 1.0 / (timescale * sr))); l.s(0.0f);
+    l.shared.push_back({(uint32_t)l.S.size(), s.c, SH_MONITOR}); l.s(0.0f);
+  }
+  HCLONE(MonitorSharedN)
+};
+struct TimerN : HNode {
+  SharedRef s; double sr = DEFAULT_SR;
+  explicit TimerN(SharedCell* c) : s(c) { c->set(0u); }   // Timer::new stores 0.0
+  int inputs() const override { return 0; } int outputs() const override { return 0; }
+  uint64_t id() const override { return 57; }
+  void reset() override { s.c->set(0u); }
+  void set_sample_rate(double r) override { sr = r; }
+  void sig(std::string& o) const override { o += "TimerShared"; }
+  void lower(Lowering& l) const override {   // sample_duration (f64), time (f64), the write-back word
+    l.p64(1.0 / sr); l.s64(0.0);
+    l.shared.push_back({(uint32_t)l.S.size(), s.c, SH_TIMER}); l.s(0.0f);
+  }
+  HCLONE(TimerN)
 };
 
 // ---------------------------------------------------------------- pan / envelope (src/pan.rs, src/envelope.rs, src/adsr.rs)
@@ -1238,6 +1296,11 @@ HNode* mk_reverb3(double time, double diffusion, HNode* filter) {
   return new ReverbN(time, diffusion, filter);
 }
 HNode* mk_var(float value) { return new VarN(value); }
+HNode* mk_var_shared(SharedCell* s) { return s ? new VarSharedN(s) : nullptr; }
+HNode* mk_monitor_shared(SharedCell* s, int kind, double timescale) {
+  return (!s || kind < 0 || kind > 2 || (kind > 0 && !(timescale > 0.0))) ? nullptr : new MonitorSharedN(s, kind, timescale);
+}
+HNode* mk_timer(SharedCell* s) { return s ? new TimerN(s) : nullptr; }
 HNode* mk_slot(HNode* x) { return x ? new SlotN(x) : nullptr; }
 HNode* mk_oversample(HNode* x) {   // the block path decimates as many channels as X has inputs (:207): more inputs than outputs would index past the outputs
   if (!x || x->outputs() < 1 || x->inputs() > x->outputs()) { delete x; return nullptr; }
@@ -1380,11 +1443,11 @@ HNode* mk_feedback2(HNode* x, HNode* y, int hadamard) {
 HNode* mk_pan(float value) { return new Panner(value, 1); }
 HNode* mk_panner() { return new Panner(0.0f, 2); }
 HNode* mk_adsr_live(float a, float d, float s, float r) { return new AdsrLive(a, d, s, r); }
-HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char* text, int ncaptures, const char* const* names, const float* values,
-                  std::string& err) {
-  const char* what = kind == CL_MAP ? "map" : (kind == CL_SHAPE_FN ? "shape_fn" : "envelope_in");
+static HNode* mk_closure_of(SharedCell* cell, int kind, int inputs, int outputs, double interval, const char* text, int ncaptures,
+                            const char* const* names, const float* values, std::string& err) {
+  const char* what = kind == CL_MAP ? "map" : (kind == CL_SHAPE_FN ? "shape_fn" : (kind == CL_VAR_FN ? "var_fn" : "envelope_in"));
   auto bad = [&](const std::string& w) -> HNode* { err = std::string(what) + ": " + w; return nullptr; };
-  if (kind < CL_MAP || kind > CL_ENVELOPE_IN) { err = "closure: bad kind"; return nullptr; }
+  if (kind < CL_MAP || kind > CL_VAR_FN || (kind == CL_VAR_FN) != (cell != nullptr)) { err = "closure: bad kind"; return nullptr; }
   if (inputs < 0 || inputs > 8 || outputs < 1 || outputs > 8) return bad("arity mismatch: 0-8 inputs and 1-8 outputs");
   if (kind == CL_ENVELOPE_IN && !(interval > 0.0)) return bad("the interval must be positive");   // EnvelopeIn::new asserts it (src/envelope.rs:230)
   if (ncaptures < 0 || (ncaptures > 0 && (!names || !values))) return bad("bad capture arrays");
@@ -1405,9 +1468,19 @@ HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char
     if (!used) return bad(std::string("capture `") + names[j] + "` does not occur in the closure");
     for (int i = 0; i < j; i++) if (names[i] && strcmp(names[i], names[j]) == 0) return bad(std::string("capture `") + names[j] + "` is given twice");
   }
+  if (kind == CL_VAR_FN) return new VarFnN(cell, outputs, c.expr, std::move(v));
   ClosureN* n = new ClosureN((ClosureKind)kind, kind == CL_SHAPE_FN ? 1 : inputs, kind == CL_SHAPE_FN ? 1 : outputs, c.expr, std::move(v));
   n->interval = (float)interval;   // EnvelopeIn<f32>: F::from_f32 / the f32 interval of prelude32 (src/prelude32.rs:716-724)
   return n;
+}
+HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char* text, int ncaptures, const char* const* names, const float* values,
+                  std::string& err) {
+  if (kind == CL_VAR_FN) { err = "closure: bad kind"; return nullptr; }
+  return mk_closure_of(nullptr, kind, inputs, outputs, interval, text, ncaptures, names, values, err);
+}
+HNode* mk_var_fn(SharedCell* s, int outputs, const char* text, int ncaptures, const char* const* names, const float* values, std::string& err) {
+  if (!s) { err = "var_fn: null Shared"; return nullptr; }
+  return mk_closure_of(s, CL_VAR_FN, 0, outputs, 0.0, text, ncaptures, names, values, err);
 }
 
 static HNode* bad2(HNode* x, HNode* y) { delete x; delete y; return nullptr; }

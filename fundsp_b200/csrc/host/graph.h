@@ -48,6 +48,36 @@ struct Setting {
 
 inline uint32_t f2u(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
 
+// ---- Shared (src/shared.rs:47-81): a 32-bit cell that any thread sets and reads with relaxed atomics, like the AtomicU32 behind a
+// Rust Shared. Reference counted: the creator's handle and every node (and bank) that uses the cell hold one reference each, as an
+// Arc clone does. `external`: the cell is memory the caller owns (the AtomicU32 of a Rust Shared); `release(user)` runs when the last
+// reference goes, so the owner can keep the memory alive until then (the Rust binding passes a leaked Arc clone and drops it there).
+struct SharedCell {
+  uint32_t own = 0; uint32_t* cell; int refs = 1;
+  void (*release)(void*) = nullptr; void* user = nullptr;
+  explicit SharedCell(float v) : own(f2u(v)), cell(&own) {}
+  SharedCell(uint32_t* external, void (*rel)(void*), void* u) : cell(external), release(rel), user(u) {}
+  ~SharedCell() { if (release) release(user); }
+  SharedCell(const SharedCell&) = delete;
+  SharedCell& operator=(const SharedCell&) = delete;
+  uint32_t get() const { return __atomic_load_n(cell, __ATOMIC_RELAXED); }
+  void set(uint32_t w) { __atomic_store_n(cell, w, __ATOMIC_RELAXED); }
+  SharedCell* ref() { __atomic_add_fetch(&refs, 1, __ATOMIC_RELAXED); return this; }
+  void unref() { if (__atomic_sub_fetch(&refs, 1, __ATOMIC_ACQ_REL) == 0) delete this; }
+};
+struct SharedRef {   // one counted reference
+  SharedCell* c = nullptr;
+  SharedRef() {}
+  explicit SharedRef(SharedCell* x) : c(x ? x->ref() : nullptr) {}
+  SharedRef(const SharedRef& o) : c(o.c ? o.c->ref() : nullptr) {}
+  SharedRef& operator=(const SharedRef& o) { if (this != &o) { SharedCell* n = o.c ? o.c->ref() : nullptr; if (c) c->unref(); c = n; } return *this; }
+  ~SharedRef() { if (c) c->unref(); }
+};
+// A word of a lowered voice that is tied to a Shared: the parameter word of a reader (Var, VarFn input), or the state word in which a
+// writer (Monitor, Timer) leaves the value it stores.
+enum SharedUseKind { SH_READ = 0, SH_MONITOR = 1, SH_TIMER = 2 };
+struct SharedUse { uint32_t word; SharedCell* cell; int kind; };
+
 struct Lowering {
   std::vector<uint32_t> P, S, U;   // words in DFS order
   std::vector<uint32_t> dlen;      // delay-line lengths (floats per voice) in DFS order
@@ -60,6 +90,9 @@ struct Lowering {
   // (state word, value) pairs where what reset() restores differs from the state a freshly built unit starts from (Adaptive's level
   // estimate: 0.0 after Adaptive::new, 1e-3 after reset, src/shape.rs:173-196). Every other word resets to its lowered value.
   std::vector<std::pair<uint32_t, uint32_t>> resetS;
+  std::vector<SharedUse> shared;   // Shared readers and writers in evaluation order
+  // writers are refused inside units that run on a clock of their own (events, slots, crossfades): the order of their stores is not the bank's
+  void no_writers_since(size_t k, const char* where) { for (; k < shared.size(); k++) if (shared[k].kind != SH_READ) { fail(std::string("monitor / timer writing a Shared inside ") + where + " is not supported"); return; } }
   bool ok = true; std::string why; // set when a node has no device lowering
   void p(float f) { P.push_back(f2u(f)); }
   void s(float f) { S.push_back(f2u(f)); }
@@ -126,6 +159,12 @@ HNode* mk_allnest(float coefficient, HNode* x, int nin);
 HNode* mk_phase_osc(int kind);                      // 0 ramp, 1 poly_saw, 2 poly_square, 3 poly_pulse
 HNode* mk_reverb3(double time, double diffusion, HNode* filter);   // Reverb<F> ID 85; consumes `filter` (1 -> 1)
 HNode* mk_var(float value);
+// Shared controls (src/shared.rs, src/dynamics.rs:441-520). Each node takes a reference to the cell.
+HNode* mk_var_shared(SharedCell* s);                                  // Var ID 68: the cell's value, fixed for one call
+HNode* mk_monitor_shared(SharedCell* s, int kind, double timescale);  // Monitor ID 56: passes through, stores the meter level (kind as mk_meter)
+HNode* mk_timer(SharedCell* s);
+// VarFn ID 70: the closure (text, as mk_closure's, one parameter |x|) of the cell's value, with 1-8 outputs; null with the reason in `err`
+HNode* mk_var_fn(SharedCell* s, int outputs, const char* text, int ncaptures, const char* const* names, const float* values, std::string& err);                                       // Timer ID 57: stores the stream time; sets the cell to 0 now
 HNode* mk_nl_biquad(int fb, int mode, int shape, float p0, float p1, int inputs, float center, float q, float gain);  // IDs 88-91
 HNode* mk_phase_synth(int kind);                                     // PhaseSynth ID 35
 HNode* mk_pulse();                                                   // PulseWave ID 44

@@ -107,6 +107,7 @@ std::string group_create(int nranks, int rank, const void* id128, int device, Gr
 }
 
 std::string group_reduce_device(Bank& b, Group& g, uint64_t n, float* mix_dev, uint64_t mix_stride, int root) {
+  if (b.sh_writes()) return "#U reduce: a bank whose monitor / timer writes a Shared cannot be part of a multi-GPU group (each rank would store its own value)";
   if (g.nranks == 1 || n == 0) return "";
   if (root < 0 || root >= g.nranks) return "reduce: root out of range";
   if (!mix_dev) return "reduce: null mix buffer";
@@ -165,6 +166,8 @@ std::string group_render_host(Bank& b, Group& g, uint64_t n, const float* in, fl
   if (g.rank == root && !out_mix) return "render_reduced: the root needs an output buffer";
   CU(cudaSetDevice(b.device));
   if (n == 0) return "";
+  if (b.sh_writes()) return "#U render_reduced: a bank whose monitor / timer writes a Shared cannot be part of a multi-GPU group (each rank would store its own value)";
+  { std::string se = b.sh_pull(); if (!se.empty()) return se; }   // every rank reads the cells into its own voices' words
   const uint32_t chunk = (uint32_t)std::min<uint64_t>(16384, (n + 63) / 64 * 64);
   std::string e = b.ensure_staging(chunk);
   if (!e.empty()) return e;

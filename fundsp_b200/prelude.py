@@ -13,6 +13,7 @@ import math
 import numpy as np
 
 from .graph import (An, ArityError, _arity, M_BRANCH, M_BUS, M_CHAIN, M_REDUCE, M_STACK, OP_ADD, OP_MUL, f32, multi)
+from .shared import Shared, shared  # noqa: F401
 
 F = np.float32
 
@@ -616,8 +617,20 @@ def unit(x):   # src/audiounit.rs:430-484 Unit<I, O>: a boxed AudioUnit as a nod
     return x
 
 
-def monitor(shared=None, meter=None):   # src/dynamics.rs:441-520: the audio passes through; the Shared is host-side (use `meter` to read a level)
+def monitor(shared=None, meter=None):
+    """Monitor (src/dynamics.rs:441-520): the audio passes through. Given a `Shared`, the meter level is stored into it after every call
+    (meter: Meter.Sample, Meter.Peak(t) or Meter.Rms(t)); without one the node is a plain pass-through."""
+    if isinstance(shared, Shared):
+        m = Meter.Sample if meter is None else meter
+        return An("monitor_shared", (shared, int(m[0]), float(m[1])), (), 1, 1)
     return An("monitor", (), (), 1, 1)
+
+
+def timer(shared):
+    """Timer (src/shared.rs:203-250): stores the stream time in seconds into `shared` after every call; sets it to 0 now and on reset."""
+    if not isinstance(shared, Shared):
+        raise TypeError("timer: needs a Shared")
+    return An("timer", (shared,), (), 0, 0)
 
 
 def oversample(node):   # src/prelude.rs:996-1005: run `node` at twice the sample rate between halfband filters
@@ -791,8 +804,19 @@ def reverb3_stereo(time, diffusion, filt):
 
 
 def var(value):
-    """var(&shared): here the shared value is changed through Setting value (kind 4) / GpuBank.set."""
+    """var(&shared). Given a `Shared`, the voice reads the cell's value, taken once per call. Given a float, the value is a parameter
+    word changed through Setting value (kind 4) / GpuBank.set."""
+    if isinstance(value, Shared):
+        return An("var_shared", (value,), (), 0, 1)
     return An("var", (f32(value),), (), 0, 1)
+
+
+def var_fn(shared, closure, outputs=1, **captures):
+    """var_fn(&shared, f) (VarFn ID 70): `|x| ...` of the Shared's value, as closure text (the language of `map_`); a tuple value gives
+    several outputs. Evaluated once per call, with the value the call reads."""
+    if not isinstance(shared, Shared):
+        raise TypeError("var_fn: needs a Shared")
+    return _closure("var_fn", (shared, closure, int(outputs), _captures(captures)), 0, int(outputs))
 
 
 def feedback_unit(delay, node):

@@ -29,6 +29,7 @@ extern "C" {
 
 typedef struct fdsp_node fdsp_node;
 typedef struct fdsp_bank fdsp_bank;
+typedef struct fdsp_shared fdsp_shared;
 
 enum { FDSP_OK = 0, FDSP_ERR_ARG = 1, FDSP_ERR_CUDA = 2, FDSP_ERR_UNSUPPORTED = 3, FDSP_ERR_ARITY = 4, FDSP_ERR_STATE = 5 };
 /* Setting parameter kinds == src/setting.rs:14-31 */
@@ -125,6 +126,25 @@ fdsp_node* fdsp_nl_biquad(int fb, int mode, int shape, float p0, float p1, int i
 fdsp_node* fdsp_shaper_adaptive(double timescale, int inner_kind, float p0, float p1);
 fdsp_node* fdsp_nl_biquad_adaptive(int fb, int mode, double timescale, int inner_kind, float p0, float p1, int inputs, float center, float q, float gain);
 fdsp_node* fdsp_var(float value);                              /* Var ID 68 src/shared.rs:84: control value, changed with Setting::value (fdsp_node_set / fdsp_bank_set) */
+/* Shared src/shared.rs:47-81: a 32-bit cell set and read from any thread with relaxed atomics (an f32 bit pattern). Reference counted:
+   fdsp_shared_free drops the caller's reference; every node built on the cell, and every bank holding such a node, keeps one of its own
+   (clones share the cell, as an Arc clone does). fdsp_shared_wrap uses memory the caller owns — the AtomicU32 behind a Rust Shared,
+   `Shared::get_shared().as_ptr()`; `release(user)` (may be NULL) is called once when the last reference is dropped, which is when the
+   memory may go (the Rust binding passes `Arc::into_raw` of a clone and drops it there).
+   Banks read readers' cells once before each process / render call: a set between two calls holds for the whole next call. After a
+   call the bank stores into each written cell what its last writer in processing order stores (the last voice in bank order, within it
+   the last writer in evaluation order). A bank in which one cell is both read and written is refused with FDSP_ERR_UNSUPPORTED. */
+fdsp_shared* fdsp_shared_new(float value);
+fdsp_shared* fdsp_shared_wrap(uint32_t* cell, void (*release)(void* user), void* user);
+void fdsp_shared_free(fdsp_shared* s);
+void fdsp_shared_set(fdsp_shared* s, float value);
+float fdsp_shared_get(const fdsp_shared* s);
+fdsp_node* fdsp_var_shared(fdsp_shared* s);                                     /* Var ID 68: var(&shared) */
+fdsp_node* fdsp_monitor_shared(fdsp_shared* s, int kind, double timescale);     /* Monitor ID 56: monitor(&shared, meter), kind as fdsp_meter */
+/* VarFn ID 70 (`var_fn(&shared, f)`): the closure, as text in the language of fdsp_map with one parameter |x| (the cell's value), returning
+   `outputs` values; evaluated once per call with the value the call reads. NULL with the reason as for fdsp_map. */
+fdsp_node* fdsp_var_fn(fdsp_shared* s, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values);
+fdsp_node* fdsp_timer(fdsp_shared* s);                                          /* Timer ID 57: timer(&shared); sets the cell to 0 now, and on reset */
 fdsp_node* fdsp_dsf(int inputs, float harmonic_spacing, float roughness); /* Dsf<N> ID 55 src/oscillator.rs:114 (dsf_saw / dsf_square) */
 fdsp_node* fdsp_mls(int bits);                                 /* Mls           ID 19 src/noise.rs:100 */
 fdsp_node* fdsp_impulse(int n);                                /* Impulse<N>    ID 81 */

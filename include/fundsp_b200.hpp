@@ -259,6 +259,30 @@ inline An rotate(float angle, float gain) { return An(fdsp_rotate(angle, gain));
 inline An mixer(int inputs, int outputs, std::initializer_list<float> matrix) { return (int)matrix.size() == inputs * outputs ? An(fdsp_mixer(inputs, outputs, matrix.begin())) : An(nullptr); }
 struct Meter { int kind; double timescale; static Meter Sample() { return {0, 0.0}; } static Meter Peak(double t) { return {1, t}; } static Meter Rms(double t) { return {2, t}; } };
 inline An meter(Meter m) { return An(fdsp_meter(m.kind, m.timescale)); }
+// Shared (src/shared.rs:47-81): a float cell set from any thread; every node built on it shares the cell, as an Arc clone does. Banks read it once per call
+// (var) and store into it after each call (monitor, timer); see fdsp_shared_new in fundsp_b200.h.
+class Shared {
+ public:
+  explicit Shared(float value = 0.0f) : h_(fdsp_shared_new(value)) {}
+  Shared(const Shared& o) = delete;
+  Shared& operator=(const Shared&) = delete;
+  ~Shared() { fdsp_shared_free(h_); }
+  void set(float v) const { fdsp_shared_set(h_, v); }
+  void set_value(float v) const { set(v); }
+  float value() const { return fdsp_shared_get(h_); }
+  fdsp_shared* handle() const { return h_; }
+ private:
+  fdsp_shared* h_;
+};
+inline An var(const Shared& s) { return An(fdsp_var_shared(s.handle())); }                                   // var(&s)
+inline An monitor(const Shared& s, Meter m) { return An(fdsp_monitor_shared(s.handle(), m.kind, m.timescale)); }  // monitor(&s, meter)
+inline An timer(const Shared& s) { return An(fdsp_timer(s.handle())); }
+// var_fn(&s, f): the closure as text with one parameter |x|, e.g. var_fn(s, "|x| (x * g, -x)", 2, {{"g", 0.5f}})
+inline An var_fn(const Shared& s, const char* closure, int outputs = 1, std::initializer_list<std::pair<const char*, float>> captures = {}) {
+  std::vector<const char*> names; std::vector<float> values;
+  for (auto& c : captures) { names.push_back(c.first); values.push_back(c.second); }
+  return An(fdsp_var_fn(s.handle(), outputs, closure, (int)names.size(), names.data(), values.data()));
+}                                       // timer(&s)
 // playwave(&wave, channel, loop): `samples` = wave.channel(channel); loop_point < 0 = None
 inline An playwave(const std::vector<float>& samples, long long loop_point = -1) { return An(fdsp_playwave(samples.data(), samples.size(), 0, samples.size(), loop_point)); }
 inline An playwave_at(const std::vector<float>& samples, size_t start, size_t end, long long loop_point = -1) { return An(fdsp_playwave(samples.data(), samples.size(), start, end, loop_point)); }

@@ -32,6 +32,7 @@ use alloc::{string::String, vec::Vec};
 
 #[repr(C)] pub struct FdspNode { _p: [u8; 0] }
 #[repr(C)] pub struct FdspBank { _p: [u8; 0] }
+#[repr(C)] pub struct FdspShared { _p: [u8; 0] }
 #[repr(C)] pub struct FdspGroup { _p: [u8; 0] }
 
 pub const FDSP_OUT_VOICES: u32 = 1;
@@ -100,6 +101,12 @@ extern "C" {
     fn fdsp_reverb3(time: f64, diffusion: f64, filter: *mut FdspNode) -> *mut FdspNode;
     fn fdsp_panner() -> *mut FdspNode;
     fn fdsp_var(value: f32) -> *mut FdspNode;
+    fn fdsp_shared_wrap(cell: *mut u32, release: Option<unsafe extern "C" fn(*mut c_void)>, user: *mut c_void) -> *mut FdspShared;
+    fn fdsp_var_fn(s: *mut FdspShared, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
+    fn fdsp_shared_free(s: *mut FdspShared);
+    fn fdsp_var_shared(s: *mut FdspShared) -> *mut FdspNode;
+    fn fdsp_monitor_shared(s: *mut FdspShared, kind: c_int, timescale: f64) -> *mut FdspNode;
+    fn fdsp_timer(s: *mut FdspShared) -> *mut FdspNode;
     fn fdsp_net_new(inputs: c_int, outputs: c_int) -> *mut FdspNode;
     fn fdsp_net_push(net: *mut FdspNode, unit: *mut FdspNode) -> c_int;
     fn fdsp_net_connect(net: *mut FdspNode, source: c_int, source_port: c_int, target: c_int, target_port: c_int) -> c_int;
@@ -351,7 +358,26 @@ where N: Size<f32>, X: AudioNode<Inputs = N, Outputs = N> + Lower, Y: AudioNode<
 impl<F: AudioNode<Inputs = U1, Outputs = U1> + Lower> Lower for crate::reverb::Reverb<F> {
     unsafe fn lower(&self) -> *mut FdspNode { let (t, d, f) = self.time_diffusion_filter(); fdsp_reverb3(t, d, f.lower()) }               // reverb.rs:154 (reverb3_stereo)
 }
-impl Lower for crate::shared::Var { unsafe fn lower(&self) -> *mut FdspNode { fdsp_var(self.value()) } }                                 // shared.rs:85; later changes: Setting::value through AudioUnit::set
+/// Shared controls over the application's own cell: the AtomicU32 behind `Shared` (`Shared::get_shared`, the only public way to it in
+/// shared.rs) is wrapped, so `Shared::set` reaches the bank between calls and the bank's monitor / timer stores reach `Shared::value`.
+/// The reference keeps the Arc of Var, VarFn, Monitor and Timer private: these need one accessor each (`shared_arc()`). The wrapper
+/// holds an Arc clone of its own (leaked into `user`, dropped by `release_cell` when the library lets go of the cell's last reference),
+/// so the memory outlives every node and bank that uses it even when the application drops its Shared and graph first.
+unsafe extern "C" fn release_cell(user: *mut c_void) { drop(alloc::sync::Arc::from_raw(user as *const core::sync::atomic::AtomicU32)); }
+unsafe fn wrap_cell(a: &alloc::sync::Arc<core::sync::atomic::AtomicU32>) -> *mut FdspShared {
+    let keep = alloc::sync::Arc::into_raw(alloc::sync::Arc::clone(a)) as *mut c_void;
+    fdsp_shared_wrap(a.as_ptr(), Some(release_cell), keep)
+}
+impl Lower for crate::shared::Var {                                                                                                       // shared.rs:84-131, ID 68
+    unsafe fn lower(&self) -> *mut FdspNode { let s = wrap_cell(self.shared_arc()); let n = fdsp_var_shared(s); fdsp_shared_free(s); n }
+}
+impl Lower for crate::dynamics::Monitor {                                                                                                   // dynamics.rs:441-520, ID 56
+    unsafe fn lower(&self) -> *mut FdspNode {
+        let (kind, t) = match self.meter() { crate::dynamics::Meter::Sample => (0, 0.0), crate::dynamics::Meter::Peak(t) => (1, t), crate::dynamics::Meter::Rms(t) => (2, t) };
+        let s = wrap_cell(self.shared_arc()); let n = fdsp_monitor_shared(s, kind, t); fdsp_shared_free(s); n
+    }
+}
+impl Lower for crate::shared::Timer { unsafe fn lower(&self) -> *mut FdspNode { let s = wrap_cell(self.shared_arc()); let n = fdsp_timer(s); fdsp_shared_free(s); n } }   // shared.rs:203-250, ID 57
 /// The N-ary combinators hold their units in a Frame<X, N> (audionode.rs:2065-2673); kind codes are the nodes' IDs.
 macro_rules! lower_multi { ($t:ident, $kind:expr, $op:expr) => {
     impl<N: Size<f32> + Size<X>, X: AudioNode + Lower> Lower for $t<N, X> {
@@ -408,6 +434,17 @@ macro_rules! gpu_map {
         $crate::combinator::An($crate::gpu::GpuClosure {
             node: $crate::audionode::Map::<_, $i, $o>::new($($f)+, $crate::signal::Routing::Arbitrary(0.0)),
             kind: 0, interval: 0.0, text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
+        })
+    };
+}
+/// `gpu_var_fn!(&s, [g], |x: f32| (x * g, -x))`: `var_fn(&s, f)` (shared.rs:134-200, ID 70) that lowers to `fdsp_var_fn` over the
+/// Shared's own cell; the output count is the closure's return type.
+#[macro_export]
+macro_rules! gpu_var_fn {
+    ($s:expr, [$($c:ident),*], $($f:tt)+) => {
+        $crate::combinator::An($crate::gpu::GpuVarFn {
+            node: $crate::shared::VarFn::new($s, $($f)+), cell: ::alloc::sync::Arc::clone($s.get_shared()),
+            text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
         })
     };
 }
@@ -578,3 +615,31 @@ impl GpuGroup {
     }
 }
 impl Drop for GpuGroup { fn drop(&mut self) { if !self.h.is_null() { unsafe { fdsp_group_destroy(self.h) } } } }
+
+/// VarFn with its closure text (gpu_var_fn!): the reference's node runs on the CPU side, the text lowers to the device over the Shared's cell.
+pub struct GpuVarFn<X> { pub node: X, pub cell: alloc::sync::Arc<core::sync::atomic::AtomicU32>, pub text: &'static str, pub names: Vec<&'static str>, pub values: Vec<f32> }
+impl<X: Clone> Clone for GpuVarFn<X> {
+    fn clone(&self) -> Self { GpuVarFn { node: self.node.clone(), cell: self.cell.clone(), text: self.text, names: self.names.clone(), values: self.values.clone() } }
+}
+impl<X: AudioNode> AudioNode for GpuVarFn<X> {
+    const ID: u64 = X::ID;
+    type Inputs = X::Inputs;
+    type Outputs = X::Outputs;
+    fn reset(&mut self) { self.node.reset() }
+    fn set_sample_rate(&mut self, sample_rate: f64) { self.node.set_sample_rate(sample_rate) }
+    fn tick(&mut self, input: &Frame<f32, Self::Inputs>) -> Frame<f32, Self::Outputs> { self.node.tick(input) }
+    fn process(&mut self, size: usize, input: &BufferRef, output: &mut BufferMut) { self.node.process(size, input, output) }
+    fn set_hash(&mut self, hash: u64) { self.node.set_hash(hash) }
+    fn route(&mut self, input: &SignalFrame, frequency: f64) -> SignalFrame { self.node.route(input, frequency) }
+}
+impl<X: AudioNode> Lower for GpuVarFn<X> {
+    unsafe fn lower(&self) -> *mut FdspNode {
+        let text: Vec<u8> = self.text.bytes().chain(core::iter::once(0)).collect();
+        let names: Vec<Vec<u8>> = self.names.iter().map(|n| n.bytes().chain(core::iter::once(0)).collect()).collect();
+        let ptrs: Vec<*const c_char> = names.iter().map(|n| n.as_ptr() as *const c_char).collect();
+        let s = wrap_cell(&self.cell);
+        let n = fdsp_var_fn(s, X::Outputs::I32, text.as_ptr() as *const c_char, self.values.len() as c_int, ptrs.as_ptr(), self.values.as_ptr());
+        fdsp_shared_free(s);
+        n
+    }
+}
