@@ -1,7 +1,5 @@
-// ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). C ABI of the closure nodes of fo_closure.h, built as a library of its own
-// (oracle/_build/libfundsp_oracle_closure.so, by tests/oracle_closure.py). Its nodes are fo::Node objects like those of
-// libfundsp_oracle.so, compiled from the same headers with the same flags, so the combinators there take them as children
-// (they only call virtual functions of their children; the library stays loaded for the life of the process).
+// ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). C ABI of the closure nodes of fo_closure.h, linked into
+// oracle/_build/libfundsp_oracle.so with fundsp_oracle.cpp (oracle/Makefile); the combinators there take them as children.
 #include "fo_closure.h"
 
 using namespace fo;

@@ -1,5 +1,5 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). C ABI of the prelude64 nodes of fo_prelude64.h and of the oracle's f64 libm,
-// built as a library of its own (oracle/_build/libfundsp_oracle_prelude64.so, by tests/oracle_prelude64.py).
+// linked into oracle/_build/libfundsp_oracle.so with fundsp_oracle.cpp (oracle/Makefile); the combinators there take them as children.
 #include "fo_prelude64.h"
 
 using namespace fo;

@@ -1,7 +1,7 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). The prelude64 nodes (F = f64) that fundsp_b200 lowers: Sine<f64>
 // (src/oscillator.rs:18-102) and the Simper SVF in its fixed and audio-rate forms (src/svf.rs:17-221, 744-1031), restated
 // independently of the product's device code (csrc/dsp/nodes.cuh, libm64.cuh) with the oracle's own f64 libm (fo_libm64.h).
-// Built with fo_prelude64.cpp as a library of its own; these are fo::Node objects, so fo_nodes.h's combinators take them as children.
+// These are fo::Node objects, so fo_nodes.h's combinators take them as children.
 #pragma once
 #include "fo_nodes.h"
 #include "fo_libm64.h"

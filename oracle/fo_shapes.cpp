@@ -1,6 +1,5 @@
-// ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). C ABI of the shapes of fo_shapes.h, built as a library of its own
-// (oracle/_build/libfundsp_oracle_shapes.so, by tests/oracle_shapes.py). Its nodes are fo::Node objects like those of
-// libfundsp_oracle.so, compiled from the same headers with the same flags, so the combinators there take them as children.
+// ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). C ABI of the shapes of fo_shapes.h, linked into
+// oracle/_build/libfundsp_oracle.so with fundsp_oracle.cpp (oracle/Makefile); the combinators there take them as children.
 #include "fo_shapes.h"
 
 using namespace fo;

@@ -1,7 +1,6 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). The Atan and Adaptive waveshapes (src/shape.rs:88-104, :156-200) in Shaper
 // (ID 42) and in the nonlinear biquads (src/biquad.rs:494-920, IDs 88-91), restated independently of the product's device code
-// (csrc/dsp/nodes.cuh, libm.cuh, math.cuh). Built with fo_shapes.cpp as a library of its own; the other shape kinds are those of
-// fo_nodes.h's Shaper, reused as they are.
+// (csrc/dsp/nodes.cuh, libm.cuh, math.cuh). The other shape kinds are those of fo_nodes.h's Shaper, reused as they are.
 #pragma once
 #include "fo_nodes.h"
 

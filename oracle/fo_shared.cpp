@@ -1,6 +1,5 @@
-// ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). C ABI of the Shared nodes of fo_shared.h, built as a library of its own
-// (oracle/_build/libfundsp_oracle_shared.so, by tests/oracle_shared.py). Its nodes are fo::Node objects like those of libfundsp_oracle.so,
-// compiled from the same headers with the same flags, so the combinators there take them as children.
+// ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). C ABI of the Shared nodes of fo_shared.h, linked into
+// oracle/_build/libfundsp_oracle.so with fundsp_oracle.cpp (oracle/Makefile); the combinators there take them as children.
 #include "fo_shared.h"
 
 using namespace fo;

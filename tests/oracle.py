@@ -8,17 +8,24 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+import tempfile
+import weakref
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "oracle", "_build", "libfundsp_oracle.so")
+ODIR = os.path.join(ROOT, "oracle")
+SO = os.path.join(ODIR, "_build", "libfundsp_oracle.so")
 
 
-def build_oracle(force=False):
-    if force or not os.path.exists(SO):
-        subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle")], stdout=subprocess.DEVNULL)
-    return SO
+def build_oracle():
+    """The oracle library, built by oracle/Makefile when it is missing or older than any oracle source. A tree that cannot be
+    written and holds no up-to-date library gets one built in a per-user temporary directory instead."""
+    so = SO
+    if not os.access(ODIR, os.W_OK) and subprocess.call(["make", "-q", "-C", ODIR], stdout=subprocess.DEVNULL) != 0:
+        so = os.path.join(tempfile.gettempdir(), f"fdsp_oracle_{os.getuid()}", "libfundsp_oracle.so")
+    subprocess.check_call(["make", "-C", ODIR, "OUT=" + so], stdout=subprocess.DEVNULL)
+    return so
 
 
 _lib = None
@@ -27,10 +34,9 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build_oracle()
-        L = C.CDLL(os.environ.get("FDSP_ORACLE_SO") or SO)   # FDSP_ORACLE_SO: bench.py's -march=native build for the TIMED CPU arm only
+        L = C.CDLL(os.environ.get("FDSP_ORACLE_SO") or build_oracle())   # FDSP_ORACLE_SO: bench.py's -march=native build for the TIMED CPU arm only
         P, F, D, I, U64, I64 = C.c_void_p, C.c_float, C.c_double, C.c_int, C.c_uint64, C.c_int64
-        FP = C.POINTER(C.c_float)
+        FP, S = C.POINTER(C.c_float), C.c_char_p
         sig = {
             "fo_about": (C.c_char_p, []),
             "fo_rnd1": (D, [U64]), "fo_hash1": (U64, [U64]), "fo_attohash": (U64, [U64, U64]), "fo_hash32x": (C.c_uint32, [C.c_uint32]),
@@ -61,6 +67,21 @@ def lib():
             "fo_net_pass_through": (None, [P, I, I]), "fo_net_size": (I, [P]), "fo_net_has_cycle": (I, [P]), "fo_net_order": (I, [P, C.POINTER(I)]),
             "fo_net_combine": (P, [I, P, P]), "fo_net_crossfade": (None, [P, I, I, F, P]),
             "fo_bank_render": (None, [C.POINTER(P), I64, D, I64, FP, FP, FP, I]),
+            # fo_shapes.cpp: the Atan and Adaptive waveshapes
+            "fo_atanf": (F, [F]), "fo_wide_atanf": (F, [F]), "fo_shaper_x": (P, [I, F, F]), "fo_shaper_adaptive": (P, [D, I, F, F]),
+            "fo_nl_biquad_x": (P, [I, I, I, F, F, I, F, F, F]), "fo_nl_biquad_adaptive": (P, [I, I, D, I, F, F, I, F, F, F]),
+            # fo_closure.cpp: closures of the signal
+            "fo_map": (P, [I, I, S, I, C.POINTER(S), FP]), "fo_shape_fn": (P, [S, I, C.POINTER(S), FP]),
+            "fo_envelope_in": (P, [D, I, I, S, I, C.POINTER(S), FP]),
+            # fo_prelude64.cpp: the prelude64 nodes and the f64 libm
+            "fo64_sin": (D, [D]), "fo64_cos": (D, [D]), "fo64_tan": (D, [D]), "fo64_exp": (D, [D]),
+            "fo_sine_f64": (P, []), "fo_fixed_svf_f64": (P, [I, F, F, F]), "fo_svf_f64": (P, [I, F, F, F]),
+            "fo_biquad_f64": (P, [F, F, F, F, F]), "fo_butterpass_f64": (P, [F, I]), "fo_resonator_f64": (P, [F, F, I]),
+            "fo_onepole_f64": (P, [I, F, I]), "fo_sine_f64_phase_after": (D, [U64, D, F, I]),
+            # fo_shared.cpp: Shared cells and the nodes that read and write them
+            "fo_shared_new": (P, [F]), "fo_shared_free": (None, [P]), "fo_shared_set": (None, [P, F]), "fo_shared_get": (F, [P]),
+            "fo_var_shared": (P, [P]), "fo_monitor_shared": (P, [P, I, D]), "fo_timer": (P, [P]),
+            "fo_var_fn": (P, [P, I, S, I, C.POINTER(S), FP]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(L, name)
@@ -77,6 +98,18 @@ def _farr(v):
     if hasattr(v, "__array__"):   # a wave channel: no per-element conversion (data_as keeps the array alive)
         return np.ascontiguousarray(np.asarray(v, dtype=np.float32)).ctypes.data_as(C.POINTER(C.c_float))
     return (C.c_float * len(v))(*v)
+
+
+def _caps(caps):
+    """A closure's captures as the oracle takes them: count, names, values."""
+    names = [k.encode() for k, _ in caps]
+    return len(caps), (C.c_char_p * max(1, len(caps)))(*names), (C.c_float * max(1, len(caps)))(*[v for _, v in caps])
+
+
+def _node(h):
+    if not h:
+        raise ValueError("the oracle has no such node, or its closure interpreter could not parse the closure")
+    return h
 
 
 class OracleBackend:
@@ -113,7 +146,8 @@ class OracleBackend:
     def b_feedback_unit(self, delay, x): return self.L.fo_feedback_unit(delay, x)
     def b_convolve(self, response): return self.L.fo_convolve(_farr(response), len(response))
     def b_onepole(self, kind, param, nin): return self.L.fo_onepole(kind, param, nin)
-    def b_shaper(self, kind, p0, p1): return self.L.fo_shaper(kind, p0, p1)
+    def b_shaper(self, kind, p0, p1): return _node(self.L.fo_shaper_x(kind, p0, p1)) if kind == 6 else self.L.fo_shaper(kind, p0, p1)   # 6: Atan
+    def b_shaper_adaptive(self, timescale, kind, p0, p1): return _node(self.L.fo_shaper_adaptive(timescale, kind, p0, p1))
     def b_follow(self, asym, a, r): return self.L.fo_follow(asym, a, r)
     def b_morph(self, cutoff, q): return self.L.fo_morph(cutoff, q)
     def b_rez(self, bp, cutoff, q, nin): return self.L.fo_rez(bp, cutoff, q, nin)
@@ -146,7 +180,11 @@ class OracleBackend:
     def sequencer_new(self, i, o, mode, loop): return self.L.fo_sequencer(i, o, mode, loop)
     def sequencer_push(self, h, s, e, ease, fi, fo, unit, rel): return (self.L.fo_sequencer_push_relative if rel else self.L.fo_sequencer_push)(h, s, e, ease, fi, fo, unit)
     def sequencer_edit(self, h, eid, end, fo, rel): (self.L.fo_sequencer_edit_relative if rel else self.L.fo_sequencer_edit)(h, eid, end, fo)
-    def b_nl_biquad(self, fb, mode, shape, p0, p1, nin, ce, q, g): return self.L.fo_nl_biquad(fb, mode, shape, p0, p1, nin, ce, q, g)
+    def b_nl_biquad(self, fb, mode, shape, p0, p1, nin, ce, q, g):
+        return (_node(self.L.fo_nl_biquad_x(fb, mode, shape, p0, p1, nin, ce, q, g)) if shape == 6 else
+                self.L.fo_nl_biquad(fb, mode, shape, p0, p1, nin, ce, q, g))
+    def b_nl_biquad_adaptive(self, fb, mode, timescale, kind, p0, p1, nin, ce, q, g):
+        return _node(self.L.fo_nl_biquad_adaptive(fb, mode, timescale, kind, p0, p1, nin, ce, q, g))
     def b_var(self, value): return self.L.fo_var(value)
     def b_dsf(self, n, spacing, rough): return self.L.fo_dsf(n, spacing, rough)
     def b_mls(self, bits): return self.L.fo_mls(bits)
@@ -167,6 +205,23 @@ class OracleBackend:
     def b_feedback(self, had, x): return self.L.fo_feedback(x, had)
     def b_phase(self, p, x): self.L.fo_phase(x, p); return x
     def b_seed(self, s, x): self.L.fo_seed(x, s); return x
+    # closures of the signal (fo_closure.h)
+    def b_map(self, text, nin, nout, caps): return _node(self.L.fo_map(nin, nout, text.encode(), *_caps(caps)))
+    def b_shape_fn(self, text, caps): return _node(self.L.fo_shape_fn(text.encode(), *_caps(caps)))
+    def b_envelope_in(self, interval, text, nin, nout, caps): return _node(self.L.fo_envelope_in(interval, nin, nout, text.encode(), *_caps(caps)))
+    # prelude64 (fo_prelude64.h)
+    def b_sine_f64(self): return _node(self.L.fo_sine_f64())
+    def b_fixed_svf_f64(self, mode, f, q, g): return _node(self.L.fo_fixed_svf_f64(mode, f, q, g))
+    def b_svf_f64(self, mode, f, q, g): return _node(self.L.fo_svf_f64(mode, f, q, g))
+    def b_biquad_f64(self, a1, a2, b0, b1, b2): return _node(self.L.fo_biquad_f64(a1, a2, b0, b1, b2))
+    def b_butterpass_f64(self, f, nin): return _node(self.L.fo_butterpass_f64(f, nin))
+    def b_resonator_f64(self, f, q, nin): return _node(self.L.fo_resonator_f64(f, q, nin))
+    def b_onepole_f64(self, kind, p, nin): return _node(self.L.fo_onepole_f64(kind, p, nin))
+    # Shared controls (fo_shared.h), each on the oracle cell that mirrors the product's Shared
+    def b_var_shared(self, s): return _node(self.L.fo_var_shared(mirror(s).h))
+    def b_monitor_shared(self, s, kind, timescale): return _node(self.L.fo_monitor_shared(mirror(s).h, kind, timescale))
+    def b_timer(self, s): return _node(self.L.fo_timer(mirror(s).h))
+    def b_var_fn(self, s, text, nout, caps): return _node(self.L.fo_var_fn(mirror(s).h, nout, text.encode(), *_caps(caps)))
     # Net container (fundsp_b200/net.py)
     def net_new(self, i, o): return self.L.fo_net_new(i, o)
     def net_push(self, net, unit): return self.L.fo_net_push(net, unit)
@@ -245,6 +300,39 @@ class OracleUnit:
         fo = np.zeros(max(1, self.outputs()), np.float32)
         self.L.fo_tick(self.h, _fp(fi), _fp(fo))
         return fo[: self.outputs()].copy()
+
+
+class OracleShared:
+    """An oracle cell (std::shared_ptr<std::atomic<uint32_t>>)."""
+
+    def __init__(self, value=0.0):
+        self.h = lib().fo_shared_new(value)
+
+    def set(self, v): lib().fo_shared_set(self.h, v)
+    def value(self): return float(lib().fo_shared_get(self.h))
+
+    def __del__(self):
+        try:
+            lib().fo_shared_free(self.h)
+        except Exception:  # noqa: BLE001
+            pass
+
+
+_MIRRORS = weakref.WeakKeyDictionary()
+
+
+def mirror(s):
+    """The oracle cell that stands for the product Shared `s`: each product `Shared` gets one of its own, created with the product
+    cell's value on first use, so a test drives both sides with `set_both` and compares `s.value()` with `mirror(s).value()`."""
+    m = _MIRRORS.get(s)
+    if m is None:
+        m = _MIRRORS[s] = OracleShared(s.value())
+    return m
+
+
+def set_both(s, v):
+    s.set(v)
+    mirror(s).set(v)
 
 
 def oracle_bank_render(exprs, sr, n, inp=None, per_voice=True, mix=False, threads=1):

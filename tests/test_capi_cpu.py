@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from fundsp_b200 import capi, workloads
+from fundsp_b200 import prelude64 as p64
 from fundsp_b200.graph import ArityError
 from fundsp_b200.prelude import *  # noqa: F401,F403
 from oracle import OracleUnit, lib as olib
@@ -62,6 +63,13 @@ GRAPHS = [
     lambda: dc(1.5) >> resample(noise() | sine_hz(440.0)) | dc(0.5) >> resample(playwave(np.linspace(-1, 1, 50, dtype=np.float32)[None, :], 0, 0)) | noise() >> meter(Meter.Rms(0.1)),
     lambda: dc(220.0) >> dsf_saw_r(0.7) | (dc(110.0) | dc(0.4)) >> dsf_square() | dc(440.0) >> dsf_square_r(0.3).phase(0.25),
     lambda: noise() >> feedback2(delay(0.002) * 0.5, lowpass_hz(2000.0, 1.0)) | (noise() | dc(800.0)) >> butterpass() | (noise() | dc((900.0, 8.0))) >> resonator(),
+    # closures, the Atan and Adaptive shapes, prelude64 and Shared controls: leaves built by the oracle's fo_closure, fo_shapes,
+    # fo_prelude64 and fo_shared units, which its leaf-hash trace sees like those of fundsp_oracle.cpp
+    lambda: (noise() | sine_hz(110.0)) >> map_("|x| (x[0] * g, x[1] - x[0])", 2, 2, g=0.5) | noise() >> shape_fn("|x| x * 0.5") >> sine()
+            | (noise() | sine_hz(3.0) | dc(0.2)) >> envelope_in("|t, i| i[0] * 0.5 + i[1] * i[2] + sin_hz(2.0, t) * k", 3, k=0.1),
+    lambda: noise() >> shape(Atan(2.0)) >> sine() | noise() >> shape(Adaptive(0.01, Tanh(1.0))) | noise() >> fbell_hz(Atan(1.0), 500.0, 50.0, 0.5),
+    lambda: dc(440.0) >> p64.sine() | sine_hz(3.0) | noise() >> p64.lowpass_hz(1000.0, 0.7) | (noise() | dc(800.0)) >> p64.butterpass(),
+    lambda: var(shared(0.5)) * saw_hz(220.0) | var_fn(shared(0.25), "|x| (x, -x)", 2) | noise() >> monitor(shared(), Meter.Rms(0.1)) | timer(shared()),
 ]
 
 

@@ -14,7 +14,6 @@ from fundsp_b200.capi import FdspError
 from fundsp_b200.graph import ArityError
 from fundsp_b200.prelude import *  # noqa: F401,F403
 from oracle import OracleUnit, lib as olib
-import oracle_closure  # noqa: F401  (the oracle's closure nodes, registered on OracleBackend)
 from test_mock_bank_cpu import ROOT, mock_env  # noqa: F401  (the mock device build, shared with that file)
 
 import test_gpu_closures as G

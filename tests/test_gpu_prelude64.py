@@ -13,7 +13,6 @@ from fundsp_b200.net import Net
 from fundsp_b200.prelude64 import *  # noqa: F401,F403
 from fundsp_b200.sequencer import event
 from oracle import OracleUnit, lib as olib, oracle_bank_render
-import oracle_prelude64  # noqa: F401  (the oracle's prelude64 nodes, registered on OracleBackend)
 
 pytestmark = pytest.mark.gpu
 SR = 48000.0

@@ -10,7 +10,6 @@ from fundsp_b200.net import Net
 from fundsp_b200.prelude import *  # noqa: F401,F403
 from fundsp_b200.sequencer import event
 from oracle import OracleUnit, lib as olib, oracle_bank_render
-import oracle_shapes  # noqa: F401  (the oracle's Atan / Adaptive nodes, registered on OracleBackend)
 
 pytestmark = pytest.mark.gpu
 SR = 48000.0

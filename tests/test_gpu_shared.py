@@ -12,8 +12,7 @@ from fundsp_b200.capi import FdspError
 from fundsp_b200.net import Net
 from fundsp_b200.prelude import *  # noqa: F401,F403
 from fundsp_b200.sequencer import event, slot
-from oracle import OracleUnit, lib as olib
-from oracle_shared import mirror, set_both
+from oracle import OracleUnit, lib as olib, mirror, set_both
 from test_gpu_mix import MOCK, bank_classes, check_mix, launch_segments, mix_model
 
 pytestmark = pytest.mark.gpu

@@ -16,7 +16,6 @@ from fundsp_b200 import capi
 from fundsp_b200 import prelude as p32
 from fundsp_b200 import prelude64 as p64
 from oracle import OracleUnit, lib as olib
-import oracle_prelude64
 from test_mock_bank_cpu import ROOT, mock_env  # noqa: F401  (the mock device build, shared with that file)
 
 import test_gpu_prelude64 as G
@@ -50,7 +49,7 @@ def test_product_libm64_equals_oracle_and_quad(tmp_path):
 
 
 def test_oracle_libm64_known_values():
-    L = oracle_prelude64.lib()
+    L = olib()
     xs = np.concatenate([np.linspace(-10.0, 10.0, 2001), np.geomspace(1e-9, 1e5, 301)])
     for f, ref in ((L.fo64_sin, np.sin), (L.fo64_cos, np.cos), (L.fo64_tan, np.tan)):
         got = np.array([f(float(x)) for x in xs])
@@ -175,7 +174,7 @@ def test_sine_phase_starts_unrounded_and_advances_in_f64():
     ticks equals that f64 track exactly and differs from the track that starts from the f32-rounded phase; the product lowers the
     unrounded phase into its state word."""
     sr, f, n = 48000.0, 440.0, 1000
-    L = oracle_prelude64.lib()
+    L = olib()
     for hash_ in (1, 12345, 0xdeadbeefcafef00d):
         p0 = _rnd1(hash_)
         assert float(F32(p0)) != p0

@@ -13,7 +13,6 @@ from fundsp_b200 import capi
 from fundsp_b200.capi import FdspError
 from fundsp_b200.prelude import *  # noqa: F401,F403
 from oracle import OracleUnit, lib as olib
-import oracle_shapes
 from test_mock_bank_cpu import ROOT, mock_env  # noqa: F401  (the mock device build, shared with that file)
 
 import test_gpu_shapes as G
@@ -37,7 +36,7 @@ def test_product_atan_equals_oracle_and_float64(tmp_path):
 
 
 def test_oracle_atanf_against_numpy():
-    L = oracle_shapes.lib()
+    L = olib()
     x = np.concatenate([np.linspace(-30.0, 30.0, 20001), np.geomspace(1e-8, 1e12, 2001)]).astype(F32)
     got = np.array([L.fo_atanf(float(v)) for v in x], F32)
     exact = np.arctan(x.astype(np.float64))

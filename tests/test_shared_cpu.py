@@ -12,8 +12,7 @@ import pytest
 from fundsp_b200 import capi
 from fundsp_b200.graph import ArityError
 from fundsp_b200.prelude import *  # noqa: F401,F403
-from oracle import OracleUnit, lib as olib
-from oracle_shared import mirror
+from oracle import OracleUnit, lib as olib, mirror
 from test_mock_bank_cpu import ROOT, mock_env  # noqa: F401  (the mock device build, shared with that file)
 
 SR = 48000.0
@@ -92,13 +91,10 @@ def test_word_layouts_and_signatures():
 def test_ping_hashes_and_ids_match_the_oracle():
     a, b = shared(0.5), shared(0.0)
     g = (var(a) * saw_hz(220.0) >> monitor(b, Meter.Rms(0.1)) >> lowpass_hz(1000.0, 1.0)) | timer(shared()) | var(a) >> follow(0.01)
-    # (the oracle's Shared nodes live in a library of their own, whose leaves its leaf-hash trace does not see: compare the ping chains,
-    # and the hashes of the leaves the oracle traces, which follow the Shared leaves)
     for x in (g, var(a), monitor(b, Meter.Peak(0.1)), timer(b) | dc(1.0), var(a) * saw_hz(220.0), var_fn(a, "|x| (x, -x)", 2) | saw_hz(3.0)):
+        assert capi.NodeHandle(x).leaf_hashes() == OracleUnit(x).leaf_hashes()
         for probe in (True, False):
             assert capi.NodeHandle(x).ping(probe, 12345) == OracleUnit(x).ping(probe, 12345)
-    saw_leaf = lambda x: x.leaf_hashes()[-1]
-    assert saw_leaf(capi.NodeHandle(var(a) * saw_hz(220.0))) == saw_leaf(OracleUnit(var(a) * saw_hz(220.0)))
     assert capi.NodeHandle(var(a)).leaf_hashes() == capi.NodeHandle(var(0.5)).leaf_hashes()
     L = capi.lib()
     for node, want in ((var(a), 68), (var_fn(a, "|x| x"), 70), (monitor(b, Meter.Sample), 56), (timer(b), 57)):
