@@ -24,20 +24,19 @@ static uint32_t pipe_chunk() {
 }
 #define PIPE_CHUNK pipe_chunk()
 
-std::string cuerr(const char* what, cudaError_t e) { return std::string(what) + ": " + cudaGetErrorString(e); }
-#define CU(call)                                          \
-  do {                                                    \
-    cudaError_t e_ = (call);                              \
-    if (e_ != cudaSuccess) return cuerr(#call, e_);       \
-  } while (0)
+// the runtime's own calls (which return "" or the message) inside a function of the same convention
+#define TRY(call) do { std::string e_ = (call); if (!e_.empty()) return e_; } while (0)
 
-template <class T> std::string dev_alloc(T** p, size_t count) {
-  if (*p) { cudaFree(*p); *p = nullptr; }
-  if (count == 0) return "";
-  CU(cudaMalloc((void**)p, count * sizeof(T)));
-  return "";
+// the class (or the saved state of one, regroup) whose ascending `voices` hold `voice`, and the voice's column there; nullptr: none
+template <class C> C* locate(std::vector<C>& classes, uint32_t voice, uint32_t* col) {
+  for (auto& c : classes) {
+    auto it = std::lower_bound(c.voices.begin(), c.voices.end(), voice);
+    if (it != c.voices.end() && *it == voice) { *col = (uint32_t)(it - c.voices.begin()); return &c; }
+  }
+  return nullptr;
 }
 }  // namespace
+static_assert(!std::is_copy_constructible<VoiceClass>::value, "a copy of a class would free its buffers twice");
 
 // `Pipe<X, Convolver>` with a response long enough for 128-wide tiles goes to the tensor-core form (FDSP_TC_CONV=0: direct form only;
 // FDSP_TC_MINK: shortest response, default 32 taps). One output channel, and not on the CPU mock device.
@@ -62,24 +61,6 @@ Bank::~Bank() {
   cudaSetDevice(device);
   rt_stop();
   if (device >= 0 && device < 64) { std::lock_guard<std::mutex> lock(g_rt_mu); if (g_rt_owner[device] == this) g_rt_owner[device] = nullptr; }
-  if (rt_ctl) cudaFreeHost(rt_ctl);
-  if (sh_stage) cudaFreeHost(sh_stage);
-  if (sh_copied) cudaEventDestroy(sh_copied);
-  cudaFree(d_rt_relay); cudaFree(d_rt_partial);
-  for (auto& c : classes) {
-    cudaFree(c.d_params); cudaFree(c.d_state); cudaFree(c.d_state0); cudaFree(c.d_uniform); cudaFree(c.d_rowmap); cudaFree(c.d_dline); cudaFree(c.d_partial); cudaFree(c.d_ring); cudaFree(c.d_dry); cudaFree(c.d_dryrows); cudaFree(c.d_dry2); cudaFree(c.d_partial2); cudaFree(c.d_cx); cudaFree(c.d_cxl); cudaFree(c.d_th); cudaFree(c.d_tl); cudaFree(c.d_crows); for (int q = 0; q < 2; q++) { if (c.e_dry[q]) cudaEventDestroy(c.e_dry[q]); if (c.e_fdn[q]) cudaEventDestroy(c.e_fdn[q]); } if (c.cstream) cudaStreamDestroy(c.cstream); if (c.e_done) cudaEventDestroy(c.e_done);
-  }
-  for (float* p : d_wtdata) cudaFree(p);
-  cudaFree(d_wt); cudaFree(d_in); cudaFree(d_out); cudaFree(d_mix); cudaFree(d_rows); cudaFree(d_treepart);
-  if (h_in) cudaFreeHost(h_in);
-  if (h_out) cudaFreeHost(h_out);
-  for (cudaEvent_t e : dom_ev) cudaEventDestroy(e);
-  if (ev0) cudaEventDestroy(ev0);
-  if (ev1) cudaEventDestroy(ev1);
-  if (e_begin) cudaEventDestroy(e_begin);
-  cudaFree(d_ticket);
-  if (stream2) cudaStreamDestroy(stream2);
-  if (stream) cudaStreamDestroy(stream);
 }
 
 std::string Bank::init(std::vector<HNode*>& voices, int dev, uint32_t mode) {
@@ -94,21 +75,21 @@ std::string Bank::init(std::vector<HNode*>& voices, int dev, uint32_t mode) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= dev) return "no usable CUDA device: fundsp_b200 has no CPU fallback";
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; }   // (another bank's resident process() kernel would make the allocations below wait for its idle time-out)
+  TRY(rt_stop());   // (another bank's resident process() kernel would make the allocations below wait for its idle time-out)
   // `stream` carries the latency-bound voice programs (few CTAs, long serial chains) and gets the highest priority, so that in
   // the two-stage pipeline its CTAs are placed before the wide FDN kernel of the previous chunk (stream2) fills every SM.
   int prio_lo = 0, prio_hi = 0;
   CU(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-  CU(cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, prio_hi));
-  CU(cudaStreamCreateWithPriority(&stream2, cudaStreamNonBlocking, prio_lo));
-  CU(cudaEventCreate(&ev0)); CU(cudaEventCreate(&ev1)); CU(cudaEventCreateWithFlags(&e_begin, cudaEventDisableTiming));
-  CU(cudaMalloc((void**)&d_ticket, 4)); CU(cudaMemset(d_ticket, 0, 4));
+  CU(cudaStreamCreateWithPriority(stream.put(), cudaStreamNonBlocking, prio_hi));
+  CU(cudaStreamCreateWithPriority(stream2.put(), cudaStreamNonBlocking, prio_lo));
+  CU(cudaEventCreate(ev0.put())); CU(cudaEventCreate(ev1.put())); CU(cudaEventCreateWithFlags(e_begin.put(), cudaEventDisableTiming));
+  TRY(d_ticket.grow(1)); CU(cudaMemset(d_ticket, 0, 4));
   return lower_and_upload(true);
 }
 
 std::string Bank::lower_and_upload(bool upload_state) {
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; } process_streak = 0;
+  TRY(rt_end_streak());
   // a looping sequencer (ReplayMode::Loop): every event of the bank carries the sequencer's loop period
   {
     double la = 0.0; bool any = false; size_t events = 0;
@@ -196,7 +177,7 @@ std::string Bank::lower_and_upload(bool upload_state) {
   }
   sh_uses.assign(nodes.size(), {});
   for (size_t v = 0; v < nodes.size(); v++) sh_uses[v] = lows[v].l.shared;
-  { std::string se = sh_check(0, sh_uses[0]); if (!se.empty()) return se; }
+  TRY(sh_check(0, sh_uses[0]));
   if (fresh.size() > 1) {   // the tensor-core convolver form is for one-class banks (its mix-down is the voice-order fold of its own rows)
     for (auto& c : fresh) if (c.conv) {
       std::string jerr;
@@ -209,8 +190,7 @@ std::string Bank::lower_and_upload(bool upload_state) {
   const bool same_shape = classes.size() == fresh.size() && std::equal(classes.begin(), classes.end(), fresh.begin(), [](const VoiceClass& a, const VoiceClass& b) {
                             return a.sig == b.sig && a.voices == b.voices && a.uniform == b.uniform; });
   if (!same_shape) {
-    for (auto& c : classes) { cudaFree(c.d_params); cudaFree(c.d_state); cudaFree(c.d_state0); cudaFree(c.d_uniform); cudaFree(c.d_rowmap); cudaFree(c.d_dline); cudaFree(c.d_partial); cudaFree(c.d_ring); cudaFree(c.d_dry); cudaFree(c.d_dryrows); cudaFree(c.d_dry2); cudaFree(c.d_partial2); cudaFree(c.d_cx); cudaFree(c.d_cxl); cudaFree(c.d_th); cudaFree(c.d_tl); cudaFree(c.d_crows); for (int q = 0; q < 2; q++) { if (c.e_dry[q]) cudaEventDestroy(c.e_dry[q]); if (c.e_fdn[q]) cudaEventDestroy(c.e_fdn[q]); } if (c.cstream) cudaStreamDestroy(c.cstream); if (c.e_done) cudaEventDestroy(c.e_done); }
-    classes = std::move(fresh);
+    classes = std::move(fresh);   // (releases the old classes' buffers)
     upload_state = true;
   }
   for (auto& c : classes) {
@@ -226,34 +206,31 @@ std::string Bank::lower_and_upload(bool upload_state) {
     for (uint32_t i = 0; i < V; i++)   // the words whose reset value differs from their starting value (Lowering::resetS)
       for (auto& w : lows[c.voices[i]].l.resetS) if (w.first < (uint32_t)NS) c.state0[(size_t)w.first * V + i] = w.second;
     if (!same_shape) {
-      std::string e;
-      if (!(e = dev_alloc(&c.d_params, P.size())).empty()) return e;
-      if (!(e = dev_alloc(&c.d_state, S.size())).empty()) return e;
-      if (!(e = dev_alloc(&c.d_uniform, c.uniform.size())).empty()) return e;
-      if (!(e = dev_alloc(&c.d_rowmap, rows.size())).empty()) return e;
-      if (!(e = dev_alloc(&c.d_dline, (size_t)c.dl_floats * V)).empty()) return e;
+      TRY(c.d_params.grow(P.size()));
+      TRY(c.d_state.grow(S.size()));
+      TRY(c.d_uniform.grow(c.uniform.size()));
+      TRY(c.d_rowmap.grow(rows.size()));
+      TRY(c.d_dline.grow((size_t)c.dl_floats * V));
       if (c.fdn) {
-        if (!(e = dev_alloc(&c.d_ring, (size_t)c.ring_floats * V)).empty()) return e;
+        TRY(c.d_ring.grow((size_t)c.ring_floats * V));
         if (c.k) {
-          if (!(e = dev_alloc(&c.d_dry, (size_t)V * 2 * TIME_CHUNK)).empty()) return e;
-          if (!(e = dev_alloc(&c.d_dry2, (size_t)V * 2 * PIPE_CHUNK)).empty()) return e;
-          for (int q = 0; q < 2; q++) { CU(cudaEventCreateWithFlags(&c.e_dry[q], cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&c.e_fdn[q], cudaEventDisableTiming)); }
-          if (!(e = dev_alloc(&c.d_dryrows, V)).empty()) return e;
-          std::vector<uint32_t> id(V);
-          for (uint32_t i = 0; i < V; i++) id[i] = 2 * i;
-          CU(cudaMemcpy(c.d_dryrows, id.data(), V * 4, cudaMemcpyHostToDevice));
+          TRY(c.d_dry.grow((size_t)V * 2 * TIME_CHUNK));
+          TRY(c.d_dry2.grow((size_t)V * 2 * PIPE_CHUNK));
+          for (int q = 0; q < 2; q++) { CU(cudaEventCreateWithFlags(c.e_dry[q].put(), cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(c.e_fdn[q].put(), cudaEventDisableTiming)); }
         }
       }
       if (c.conv) {
-        if (!(e = dev_alloc(&c.d_cx, (size_t)V * c.conv_stride)).empty()) return e;
-        if (!(e = dev_alloc(&c.d_cxl, (size_t)V * c.conv_stride)).empty()) return e;
-        if (!(e = dev_alloc(&c.d_th, (size_t)128 * c.conv_J)).empty()) return e;
-        if (!(e = dev_alloc(&c.d_tl, (size_t)128 * c.conv_J)).empty()) return e;
-        if (!(e = dev_alloc(&c.d_dryrows, V)).empty()) return e;
-        std::vector<uint32_t> id(V);
-        for (uint32_t i = 0; i < V; i++) id[i] = i;
-        CU(cudaMemcpy(c.d_dryrows, id.data(), V * 4, cudaMemcpyHostToDevice));
+        TRY(c.d_cx.grow((size_t)V * c.conv_stride));
+        TRY(c.d_cxl.grow((size_t)V * c.conv_stride));
+        TRY(c.d_th.grow((size_t)128 * c.conv_J));
+        TRY(c.d_tl.grow((size_t)128 * c.conv_J));
         CU(conv_tc_make_maps(c.d_cx, c.d_cxl, V, c.conv_stride, c.d_th, c.d_tl, c.conv_J, &c.conv_maps));
+      }
+      if ((c.fdn && c.k) || c.conv) {   // the rows the dry stage writes (two per voice) or the convolver reads (one per voice)
+        TRY(c.d_dryrows.grow(V));
+        std::vector<uint32_t> id(V);
+        for (uint32_t i = 0; i < V; i++) id[i] = c.conv ? i : 2 * i;
+        CU(cudaMemcpy(c.d_dryrows, id.data(), V * 4, cudaMemcpyHostToDevice));
       }
       CU(cudaMemcpy(c.d_rowmap, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice));
       if (!c.uniform.empty()) CU(cudaMemcpy(c.d_uniform, c.uniform.data(), c.uniform.size() * 4, cudaMemcpyHostToDevice));
@@ -282,17 +259,12 @@ std::string Bank::lower_and_upload(bool upload_state) {
       const WaveTableHost& t = device_wavetable(kind);
       h_wt[kind].n = (int)t.pitch.size(); h_wt[kind].total = (int)t.data.size();
       for (size_t i = 0; i < t.pitch.size() && i < 48; i++) { h_wt[kind].pitch[i] = t.pitch[i]; h_wt[kind].off[i] = t.off[i]; h_wt[kind].len[i] = t.len[i]; }
-      std::string e = dev_alloc(&d_wtdata[kind], t.data.size());
-      if (!e.empty()) return e;
+      TRY(d_wtdata[kind].grow(t.data.size()));
       CU(cudaMemcpy(d_wtdata[kind], t.data.data(), t.data.size() * 4, cudaMemcpyHostToDevice));
       h_wt[kind].data = d_wtdata[kind];
       changed = true;
     }
-    if (!d_wt) {
-      std::string e = dev_alloc(&d_wt, 6);
-      if (!e.empty()) return e;
-      changed = true;
-    }
+    if (!d_wt) { TRY(d_wt.grow(6)); changed = true; }
     if (changed) CU(cudaMemcpy(d_wt, h_wt, sizeof(h_wt), cudaMemcpyHostToDevice));
   }
   if (upload_state) dirty = false;
@@ -301,10 +273,9 @@ std::string Bank::lower_and_upload(bool upload_state) {
 
 std::string Bank::set_sample_rate(double s) {  // AudioUnit::set_sample_rate
   sr = s;
-  const double unit_rate = net_rate ? (double)(float)s : s;
   for (auto& n : nodes) {   // the bank of a sequencer is re-rated like the sequencer: its events' units are reset (a unit pushed later is not)
-    const bool reset = event_rerate_resets(n.get(), unit_rate);
-    n->set_sample_rate(unit_rate);
+    const bool reset = event_rerate_resets(n.get(), unit_rate());
+    n->set_sample_rate(unit_rate());
     if (reset) n->reset();
   }
   // Parameters always follow the new rate. State is re-initialised only while nothing has been rendered
@@ -315,7 +286,7 @@ std::string Bank::set_sample_rate(double s) {  // AudioUnit::set_sample_rate
 std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (src/audiounit.rs:62, src/setting.rs) on a live bank
   if (voice >= V()) return "#A set: voice index out of range";
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; } process_streak = 0;
+  TRY(rt_end_streak());
   // the setting is tried on a COPY of the voice's host graph: a refused setting (one that would change a class-uniform word) leaves
   // both the host graph and the device untouched; the copy replaces the original only after the upload
   std::unique_ptr<HNode> trial(nodes[voice]->clone());
@@ -323,13 +294,13 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
   Lowering l;
   trial->lower(l);
   if (!l.ok) return "#U " + l.why;
-  for (auto& c : classes) {
-    auto it = std::lower_bound(c.voices.begin(), c.voices.end(), voice);
-    if (it == c.voices.end() || *it != voice) continue;
-    const uint32_t i = (uint32_t)(it - c.voices.begin()), Vc = c.V();
+  uint32_t i = 0;
+  if (VoiceClass* cp = locate(classes, voice, &i)) {
+    VoiceClass& c = *cp;
+    const uint32_t Vc = c.V();
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns)
       return "#U set: the setting changes a class-uniform word (a delay length); rebuild the bank instead";
-    { std::string se = sh_check(voice, l.shared); if (!se.empty()) return se; }
+    TRY(sh_check(voice, l.shared));
     // parameters take effect at once (one strided column of the [NP][V] block); running state is left alone, the
     // construction-time state (what reset() restores) follows the setting like the reference's stored phase/seed
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
@@ -346,15 +317,15 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
 
 double Bank::loop_point() const {
   if (!(loop_arg > 0.0)) return std::numeric_limits<double>::infinity();
-  const double unit_rate = net_rate ? (double)(float)sr : sr;
-  return std::max(64.0 * (1.0 / unit_rate), std::round(loop_arg * unit_rate) / unit_rate);
+  const double ur = unit_rate();
+  return std::max(64.0 * (1.0 / ur), std::round(loop_arg * ur) / ur);
 }
 void Bank::advance_clock(uint64_t n) {   // what every Event<X> voice does to its own clock (nodes.cuh Event::plan / at_sample)
-  const double unit_rate = net_rate ? (double)(float)sr : sr, sd = 1.0 / unit_rate, lp = loop_point();
+  const double ur = unit_rate(), sd = 1.0 / ur, lp = loop_point();
   for (uint64_t t0 = 0; t0 < n; t0 += 64) {
     const uint64_t size = std::min<uint64_t>(64, n - t0);
     if (!(loop_arg > 0.0)) { seq_time = seq_time + sd * (double)size; continue; }
-    const double x = std::round(std::max(0.0, lp - seq_time) * unit_rate);
+    const double x = std::round(std::max(0.0, lp - seq_time) * ur);
     const uint64_t loop_size = x > 0.0 ? (uint64_t)x : 0;
     seq_time = std::min(seq_time + sd * (double)size, lp);
     if (loop_size < size) seq_time = std::min(0.0 + sd * (double)(size - loop_size), lp);   // wrapped: the rest of the block counts from 0
@@ -363,7 +334,7 @@ void Bank::advance_clock(uint64_t n) {   // what every Event<X> voice does to it
 std::string Bank::state0_to_device(VoiceClass& c, const uint32_t** out) {
   *out = nullptr;
   if (!(loop_arg > 0.0) || c.state0.empty() || c.sig.compare(0, 6, "Event<") != 0) return "";
-  if (!c.d_state0) { std::string e = dev_alloc(&c.d_state0, c.state0.size()); if (!e.empty()) return e; c.state0_stale = true; }
+  if (!c.d_state0) { TRY(c.d_state0.grow(c.state0.size())); c.state0_stale = true; }
   if (c.state0_stale) { CU(cudaMemcpy(c.d_state0, c.state0.data(), c.state0.size() * 4, cudaMemcpyHostToDevice)); c.state0_stale = false; }
   *out = c.d_state0;
   return "";
@@ -371,15 +342,15 @@ std::string Bank::state0_to_device(VoiceClass& c, const uint32_t** out) {
 
 // `l`: the words to run with. `reset_state`: the construction-time state that reset() restores (defaults to l.S).
 std::string Bank::upload_voice(uint32_t voice, const Lowering& l, bool with_state, const std::vector<uint32_t>* reset_state) {
-  { std::string re = rt_stop(); if (!re.empty()) return re; } process_streak = 0;
-  for (auto& c : classes) {
-    auto it = std::lower_bound(c.voices.begin(), c.voices.end(), voice);
-    if (it == c.voices.end() || *it != voice) continue;
-    const uint32_t i = (uint32_t)(it - c.voices.begin()), Vc = c.V();
+  TRY(rt_end_streak());
+  uint32_t i = 0;
+  if (VoiceClass* cp = locate(classes, voice, &i)) {
+    VoiceClass& c = *cp;
+    const uint32_t Vc = c.V();
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns || (reset_state && reset_state->size() != c.ns))
       return "#U the voice does not fit its class: a class-uniform word (delay length, table, wave) or the word layout differs; rebuild the bank instead";
     if (with_state && c.fdn) return "#U voices of a two-stage (FDN reverb) class cannot be replaced in place";
-    { std::string se = sh_check(voice, l.shared); if (!se.empty()) return se; }
+    TRY(sh_check(voice, l.shared));
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
     const std::vector<uint32_t> S0 = reset_state ? *reset_state : l.reset_image();
     for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];
@@ -406,6 +377,16 @@ std::string Bank::edit_event(uint32_t voice, double end_time, double fade_out) {
   return upload_voice(voice, l, false);
 }
 
+void Bank::lower_entering(HNode* n, Lowering* l0, Lowering* l, bool fading) const {
+  n->set_sample_rate(unit_rate());
+  n->lower(*l0);                                          // (a crossfading vertex lowers as ARRIVED: a bank reset leaves it at its second unit)
+  const bool xf = fading && xfade_set_done(n, false);
+  const bool ev = event_set_clock(n, seq_time);          // an event put into a running sequencer counts from now
+  n->lower(*l);
+  if (ev) event_set_clock(n, 0.0);
+  if (xf) xfade_set_done(n, true);
+}
+
 std::string Bank::replace_voice(uint32_t voice, HNode* node) {
   std::unique_ptr<HNode> n(node);
   if (!n) return "#A replace: null node";
@@ -418,17 +399,11 @@ std::string Bank::replace_voice(uint32_t voice, HNode* node) {
   // the classes are regrouped around it, every other voice keeps its running state (the slow path, like add_voice)
   slot_latest.erase(voice); xfade_latest.erase(voice);   // (a parked update belongs to the unit that leaves)
   if (a != b) return regroup(n.release(), (int)voice, nullptr);
-  const double unit_rate = net_rate ? (double)(float)sr : sr;
-  n->set_sample_rate(unit_rate);
   Lowering l0, l;
-  n->lower(l0);                                        // what reset() restores: the event's clock at 0, like every other voice
-  const bool ev = event_set_clock(n.get(), seq_time);  // an event put into a running sequencer counts from now
-  n->lower(l);
-  if (ev) event_set_clock(n.get(), 0.0);
+  lower_entering(n.get(), &l0, &l, false);
   if (!l.ok) return "#U " + l.why;
   const std::vector<uint32_t> S0 = l0.reset_image();
-  std::string e = upload_voice(voice, l, true, &S0);
-  if (!e.empty()) return e;
+  TRY(upload_voice(voice, l, true, &S0));
   nodes[voice] = std::move(n);
   return "";
 }
@@ -458,16 +433,9 @@ std::string Bank::regroup(HNode* node, int at, uint32_t* voice, const Carry* car
   if (tree_mix && at < 0) return "#U add: a bank extracted from a Net mixes in the Net's order; rebuild it from the edited Net";
   for (auto& c : classes) if (c.fdn || c.conv) return std::string("#U ") + what + ": banks with a two-stage class (FDN reverb, tensor-core convolver) cannot be regrouped in place; rebuild the bank";
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; } process_streak = 0;
-  const double unit_rate = net_rate ? (double)(float)sr : sr;
-  n->set_sample_rate(unit_rate);
+  TRY(rt_end_streak());
   Lowering l0, l;
-  n->lower(l0);                                      // (a crossfading vertex lowers as ARRIVED: a bank reset leaves it at its second unit)
-  const bool xf = xfade_set_done(n.get(), false);   // ... and starts its life fading
-  const bool ev = event_set_clock(n.get(), seq_time);
-  n->lower(l);
-  if (ev) event_set_clock(n.get(), 0.0);
-  if (xf) xfade_set_done(n.get(), true);
+  lower_entering(n.get(), &l0, &l, true);
   if (!l.ok) return "#U " + l.why;
   { std::string sg, jerr; n->sig(sg); if (!get_program(sg, device, jerr)) return std::string("#U ") + what + ": no device program for `" + sg + "`: " + jerr; }
   // 1. read back what is running
@@ -499,31 +467,25 @@ std::string Bank::regroup(HNode* node, int at, uint32_t* voice, const Carry* car
     std::vector<float> D((size_t)c.dl_floats * Vc, 0.0f);
     for (uint32_t i = 0; i < Vc; i++) {
       const uint32_t v = c.voices[i];
+      uint32_t j = 0;
       if (v == nv) {   // the newcomer: live state (an event's clock = now); what reset() restores is its construction-time state
         const std::vector<uint32_t> S0 = l0.reset_image();
         for (uint32_t k = 0; k < c.ns && k < l.S.size(); k++) { S[(size_t)k * Vc + i] = l.S[k]; c.state0[(size_t)k * Vc + i] = S0[k]; }
         c.state0_stale = true;
-        if (carry) {   // a unit that keeps RUNNING inside the newcomer (the fading-out side of a crossfade): its words and delay lines move over
-          for (auto& sv : saved) {
-            auto it = std::lower_bound(sv.voices.begin(), sv.voices.end(), v);
-            if (it == sv.voices.end() || *it != v) continue;
-            const uint32_t j = (uint32_t)(it - sv.voices.begin()), Vo = (uint32_t)sv.voices.size();
-            if (carry->src_s + carry->ns > sv.ns || carry->dst_s + carry->ns > c.ns || carry->src_d + carry->nd > sv.dl || carry->dst_d + carry->nd > c.dl_floats) return "internal: crossfade carry out of range";
-            for (uint32_t k = 0; k < carry->ns; k++) S[(size_t)(carry->dst_s + k) * Vc + i] = sv.S[(size_t)(carry->src_s + k) * Vo + j];
-            for (uint64_t q = 0; q < carry->nd; q++) D[(size_t)(carry->dst_d + q) * Vc + i] = sv.D[(size_t)(carry->src_d + q) * Vo + j];
-            break;
-          }
+        // a unit that keeps RUNNING inside the newcomer (the fading-out side of a crossfade): its words and delay lines move over
+        if (const Saved* sv = carry ? locate(saved, v, &j) : nullptr) {
+          const uint32_t Vo = (uint32_t)sv->voices.size();
+          if (carry->src_s + carry->ns > sv->ns || carry->dst_s + carry->ns > c.ns || carry->src_d + carry->nd > sv->dl || carry->dst_d + carry->nd > c.dl_floats) return "internal: crossfade carry out of range";
+          for (uint32_t k = 0; k < carry->ns; k++) S[(size_t)(carry->dst_s + k) * Vc + i] = sv->S[(size_t)(carry->src_s + k) * Vo + j];
+          for (uint64_t q = 0; q < carry->nd; q++) D[(size_t)(carry->dst_d + q) * Vc + i] = sv->D[(size_t)(carry->src_d + q) * Vo + j];
         }
         continue;
       }
-      for (auto& sv : saved) {
-        auto it = std::lower_bound(sv.voices.begin(), sv.voices.end(), v);
-        if (it == sv.voices.end() || *it != v) continue;
-        if (sv.sig != c.sig || sv.ns != c.ns || sv.dl != c.dl_floats) return "internal: a voice changed class while the bank grew";
-        const uint32_t j = (uint32_t)(it - sv.voices.begin()), Vo = (uint32_t)sv.voices.size();
-        for (uint32_t k = 0; k < c.ns; k++) S[(size_t)k * Vc + i] = sv.S[(size_t)k * Vo + j];
-        for (uint64_t q = 0; q < c.dl_floats; q++) D[(size_t)q * Vc + i] = sv.D[(size_t)q * Vo + j];
-        break;
+      if (const Saved* sv = locate(saved, v, &j)) {
+        if (sv->sig != c.sig || sv->ns != c.ns || sv->dl != c.dl_floats) return "internal: a voice changed class while the bank grew";
+        const uint32_t Vo = (uint32_t)sv->voices.size();
+        for (uint32_t k = 0; k < c.ns; k++) S[(size_t)k * Vc + i] = sv->S[(size_t)k * Vo + j];
+        for (uint64_t q = 0; q < c.dl_floats; q++) D[(size_t)q * Vc + i] = sv->D[(size_t)q * Vo + j];
       }
     }
     if (!S.empty()) CU(cudaMemcpyAsync(c.d_state, S.data(), S.size() * 4, cudaMemcpyHostToDevice, stream));
@@ -546,25 +508,24 @@ std::string Bank::crossfade_voice(uint32_t voice, int ease, float fade_time, HNo
   if (!n || ease < 0 || ease > 1 || !(fade_time > 0.0f)) return "#A crossfade: needs a unit, fade 0 (Power) or 1 (Smooth) and a fade time > 0";
   if (n->inputs() != nin || n->outputs() != nout) return "#U crossfade: the unit's arity differs from the bank's";
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; } process_streak = 0;
+  TRY(rt_end_streak());
   const HNode* cur = nodes[voice].get();
   Carry carry{0, 0, 0, 0, 0, 0};
   auto count = [](const HNode* h, uint32_t* ns, uint64_t* nd) { Lowering q; h->lower(q); *ns = (uint32_t)q.S.size(); *nd = 0; for (uint32_t d : q.dlen) *nd += d; return q.ok; };
   std::unique_ptr<HNode> old;
   if (const HNode* y = xfade_unit(cur, 1)) {   // the vertex crossfaded before: it must have arrived at its second unit
-    for (auto& c : classes) {
-      auto it = std::lower_bound(c.voices.begin(), c.voices.end(), voice);
-      if (it == c.voices.end() || *it != voice) continue;
+    uint32_t i = 0;
+    if (const VoiceClass* c = locate(classes, voice, &i)) {
       CU(cudaStreamSynchronize(stream));
       uint32_t done = 0;
-      CU(cudaMemcpy(&done, c.d_state + (size_t)(it - c.voices.begin()), 4, cudaMemcpyDeviceToHost));   // state word 0 of Xfade: done
+      CU(cudaMemcpy(&done, c->d_state + i, 4, cudaMemcpyDeviceToHost));   // state word 0 of Xfade: done
       if (!done) {
         // Vertex::enqueue with `next` occupied: the edit waits as `latest`, a newer one replaces it (src/vertex.rs:203-218). Its program — the
         // class Xfade<second unit, new unit> the voice will move to — is compiled now, so that a unit without a device program is refused here
         std::unique_ptr<HNode> probe(mk_xfade(y->clone(), n->clone(), ease, fade_time));
         std::string sg, jerr;
         if (!probe) return "#A crossfade: the units do not fit one vertex";
-        probe->set_sample_rate(net_rate ? (double)(float)sr : sr);
+        probe->set_sample_rate(unit_rate());
         { Lowering q; probe->lower(q); if (!q.ok) return "#U " + q.why; }
         probe->sig(sg);
         if (!get_program(sg, device, jerr)) return "#U crossfade: no device program for `" + sg + "`: " + jerr;
@@ -601,11 +562,11 @@ std::string Bank::slot_set(uint32_t voice, int ease, double fade_time, HNode* un
 std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode* unit, bool force) {
   std::unique_ptr<HNode> n(unit);
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; } process_streak = 0;
-  for (auto& c : classes) {
-    auto it = std::lower_bound(c.voices.begin(), c.voices.end(), voice);
-    if (it == c.voices.end() || *it != voice) continue;
-    const uint32_t i = (uint32_t)(it - c.voices.begin()), Vc = c.V();
+  TRY(rt_end_streak());
+  uint32_t i = 0;
+  if (VoiceClass* cp = locate(classes, voice, &i)) {
+    VoiceClass& c = *cp;
+    const uint32_t Vc = c.V();
     if (c.fdn || c.ns < 4 || ((c.ns - 4) & 1u) || (c.dl_floats & 1u)) return "slot: unexpected class layout";
     CU(cudaStreamSynchronize(stream));
     uint32_t head[2] = {0, 0};   // which, has_next of this voice
@@ -620,7 +581,7 @@ std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode
     trial->lower(l);
     if (!l.ok) return "#U " + l.why;
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns) return "#U slot: the unit changes a class-uniform word (delay length, table, wave); rebuild the bank instead";
-    { std::string se = sh_check(voice, l.shared); if (!se.empty()) return se; }
+    TRY(sh_check(voice, l.shared));
     if (fading) {   // SlotBackend::handle_messages with `next` occupied: the update waits as `latest`, a newer one takes its place (:142-150)
       SlotLatest& w = slot_latest[voice];
       w.unit = std::move(parked); w.ease = ease; w.fade_time = fade_time;
@@ -651,50 +612,41 @@ std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode
 // phase_left, n_f, fade_phase += n_f / (fade_time sr)) from the voice's fade_phase word.
 std::string Bank::slot_service(uint64_t n, uint64_t* cut) {
   *cut = n;
-  auto locate = [&](uint32_t voice, VoiceClass** pc, uint32_t* pi) {
-    for (auto& c : classes) {
-      auto vi = std::lower_bound(c.voices.begin(), c.voices.end(), voice);
-      if (vi != c.voices.end() && *vi == voice) { *pc = &c; *pi = (uint32_t)(vi - c.voices.begin()); return true; }
-    }
-    return false;
-  };
   // 1. arm what is ready. Arming a vertex regroups the classes, so the scan starts over after every arm.
   for (bool again = true; again;) {
     again = false;
     CU(cudaStreamSynchronize(stream));
     for (auto it = slot_latest.begin(); it != slot_latest.end(); ++it) {
-      VoiceClass* c = nullptr; uint32_t i = 0;
-      if (!locate(it->first, &c, &i) || !is_slot(nodes[it->first].get())) { slot_latest.erase(it); again = true; break; }
+      uint32_t i = 0; const VoiceClass* c = locate(classes, it->first, &i);
+      if (!c || !is_slot(nodes[it->first].get())) { slot_latest.erase(it); again = true; break; }
       uint32_t has_next = 0;
       CU(cudaMemcpy(&has_next, c->d_state + (size_t)1 * c->V() + i, 4, cudaMemcpyDeviceToHost));
       if (has_next) continue;
       const uint32_t voice = it->first;
       SlotLatest w = std::move(it->second);
       slot_latest.erase(it);
-      std::string e = slot_arm_now(voice, w.ease, w.fade_time, w.unit.release(), false);
-      if (!e.empty()) return e;
+      TRY(slot_arm_now(voice, w.ease, w.fade_time, w.unit.release(), false));
       again = true; break;
     }
     if (again) continue;
     for (auto it = xfade_latest.begin(); it != xfade_latest.end(); ++it) {
-      VoiceClass* c = nullptr; uint32_t i = 0;
-      if (!locate(it->first, &c, &i) || !xfade_unit(nodes[it->first].get(), 1)) { xfade_latest.erase(it); again = true; break; }
+      uint32_t i = 0; const VoiceClass* c = locate(classes, it->first, &i);
+      if (!c || !xfade_unit(nodes[it->first].get(), 1)) { xfade_latest.erase(it); again = true; break; }
       uint32_t done = 0;
       CU(cudaMemcpy(&done, c->d_state + i, 4, cudaMemcpyDeviceToHost));
       if (!done) continue;
       const uint32_t voice = it->first;
       SlotLatest w = std::move(it->second);
       xfade_latest.erase(it);
-      std::string e = crossfade_voice(voice, w.ease, (float)w.fade_time, w.unit.release());
-      if (!e.empty()) return e;
+      TRY(crossfade_voice(voice, w.ease, (float)w.fade_time, w.unit.release()));
       again = true; break;
     }
   }
   // 2. where do the running fades with a parked unit end?
   auto consider = [&](uint64_t t_end) { if (t_end < *cut) *cut = t_end; };
   for (auto& kv : slot_latest) {
-    VoiceClass* c = nullptr; uint32_t i = 0;
-    if (!locate(kv.first, &c, &i)) continue;
+    uint32_t i = 0; const VoiceClass* c = locate(classes, kv.first, &i);
+    if (!c) continue;
     uint32_t w[2] = {0, 0};
     CU(cudaMemcpy2D(w, 4, c->d_state + (size_t)2 * c->V() + i, (size_t)c->V() * 4, 4, 2, cudaMemcpyDeviceToHost));   // fade_phase (f64)
     double fade_time = 0.0, rate = 0.0;
@@ -713,8 +665,8 @@ std::string Bank::slot_service(uint64_t n, uint64_t* cut) {
     }
   }
   for (auto& kv : xfade_latest) {
-    VoiceClass* c = nullptr; uint32_t i = 0;
-    if (!locate(kv.first, &c, &i)) continue;
+    uint32_t i = 0; const VoiceClass* c = locate(classes, kv.first, &i);
+    if (!c) continue;
     float phase = 0.0f;
     CU(cudaMemcpy(&phase, c->d_state + (size_t)1 * c->V() + i, 4, cudaMemcpyDeviceToHost));   // fade_phase (f32)
     float fade_time = 0.0f, rate = 0.0f;
@@ -739,14 +691,10 @@ std::string Bank::push_event(HNode* node, uint32_t* voice) {   // Sequencer::pus
   if (loop_arg > 0.0) return "#U push: a looping sequencer bank takes its events before the first render";
   if (n->inputs() != nin || n->outputs() != nout) return "#U push: the event's arity differs from the bank's";
   CU(cudaSetDevice(device));
-  const double unit_rate = net_rate ? (double)(float)sr : sr, sd = 1.0 / unit_rate;
-  n->set_sample_rate(unit_rate);
-  std::string want; n->sig(want);
+  const double sd = 1.0 / unit_rate();
   Lowering l0, l;
-  n->lower(l0);                             // what reset() restores: the event's clock at 0 (ReplayMode::All replays it from the top)
-  event_set_clock(n.get(), seq_time);       // the event counts from now; a start time in the past makes it sound from the next block on
-  n->lower(l);
-  event_set_clock(n.get(), 0.0);
+  lower_entering(n.get(), &l0, &l, false);   // (a start time in the past makes the event sound from the next block on)
+  std::string want; n->sig(want);
   if (!l.ok) return "#U " + l.why;
   for (auto& c : classes) {
     if (c.sig != want || c.uniform != l.U || c.fdn) continue;
@@ -754,8 +702,7 @@ std::string Bank::push_event(HNode* node, uint32_t* voice) {   // Sequencer::pus
       if (!event_times(nodes[v].get(), &s0, &e0)) break;
       if (!(e0 <= seq_time + 0.5 * sd)) continue;   // Event::plan's end-of-event test at the start of the next block: still sounding
       const std::vector<uint32_t> S0 = l0.reset_image();
-      std::string e = upload_voice(v, l, true, &S0);
-      if (!e.empty()) return e;
+      TRY(upload_voice(v, l, true, &S0));
       nodes[v] = std::move(n);
       if (voice) *voice = v;
       return "";
@@ -766,14 +713,13 @@ std::string Bank::push_event(HNode* node, uint32_t* voice) {   // Sequencer::pus
 
 std::string Bank::reset() {  // AudioUnit::reset: back to the construction-time state
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; } process_streak = 0;
+  TRY(rt_end_streak());
   while (!slot_latest.empty()) {   // SlotBackend::reset adopts the LATEST configuration (src/slot.rs:156-172): arm it (its words become the voice's reset image)
     auto it = slot_latest.begin();
     const uint32_t voice = it->first;
     SlotLatest w = std::move(it->second);
     slot_latest.erase(it);
-    std::string e = slot_arm_now(voice, w.ease, w.fade_time, w.unit.release(), true);
-    if (!e.empty()) return e;
+    TRY(slot_arm_now(voice, w.ease, w.fade_time, w.unit.release(), true));
   }
   for (auto& c : classes) {
     // everything goes back to its construction-time value EXCEPT what the reference's reset leaves alone (keep_s / keep_d)
@@ -818,12 +764,23 @@ static bool use_staged(const Program* k, uint32_t V, uint32_t len, uint32_t sms)
   const uint32_t maxv = m ? (uint32_t)atoi(m) : sms * 32u;
   return on != 0 && k && k->stages >= 2 && len >= 256u && V <= maxv;
 }
-// CTA shape of a stage-pipelined class: 32 voices per CTA while that still leaves SMs free, else 128 with the voices spread evenly
-// (FDSP_STAGED_W=128 forces the wide shape: lets the tests reach it with few voices)
-static uint32_t staged_grid(uint32_t V, uint32_t sms, uint32_t* vpc) {
+// CTAs (the rows of its partial mix), voices per CTA and kernel form of class c's voice program in a launch of len samples. Stage-pipelined:
+// 32 voices per CTA while that still leaves SMs free, else 128 spread evenly (FDSP_STAGED_W=128 forces the wide shape: lets the tests reach
+// it with few voices). Otherwise whole waves of CTAs with the voices spread evenly, but the dry stage of a two-stage class stays compact
+// (few CTAs) so that it leaves the other SMs to the FDN kernel it is pipelined with.
+struct ClassGrid { uint32_t ctas = 0, vpc = 0; bool staged = false; };
+static ClassGrid class_grid(const VoiceClass& c, uint32_t len, int device) {
+  ClassGrid g;
+  if (!c.k) return g;
+  const uint32_t V = c.V(), nsm = sm_count(device);
   const char* w = getenv("FDSP_STAGED_W");
-  if (V <= sms * 32u && !(w && atoi(w) == 128)) { *vpc = 32u; return (V + 31u) / 32u; }
-  return bank_grid(V, 128u, sms, vpc);
+  g.vpc = (uint32_t)c.k->threads;
+  g.staged = use_staged(c.k.get(), V, len, nsm);
+  if (g.staged && V <= nsm * 32u && !(w && atoi(w) == 128)) { g.vpc = 32u; g.ctas = (V + 31u) / 32u; }
+  else if (g.staged) g.ctas = bank_grid(V, 128u, nsm, &g.vpc);
+  else if (c.fdn || getenv("FDSP_NO_SPREAD")) g.ctas = (V + g.vpc - 1) / g.vpc;
+  else g.ctas = bank_grid(V, g.vpc, nsm, &g.vpc);
+  return g;
 }
 
 // ---- resident process() kernel
@@ -834,7 +791,7 @@ static uint32_t staged_grid(uint32_t V, uint32_t sms, uint32_t* vpc) {
 std::string Bank::rt_stop() {
   Bank* other = nullptr;
   if (device >= 0 && device < 64) { std::lock_guard<std::mutex> lock(g_rt_mu); other = g_rt_owner[device]; if (other == this || (other && !other->rt_running)) other = nullptr; }
-  if (other) { std::string e = other->rt_stop(); if (!e.empty()) return e; }
+  if (other) TRY(other->rt_stop());
   if (!rt_running) return "";
   rt_ctl->doorbell = RT_QUIT;
   __sync_synchronize();
@@ -862,13 +819,9 @@ std::string Bank::rt_process(uint32_t size, const float* in, float* out, bool* s
   const uint32_t grid = bank_grid(c.V(), (uint32_t)c.k->threads, sm_count(device), &vpc);
   if (grid > sm_count(device)) return "";           // every CTA must be resident at once
   if (++process_streak < 3u && !rt_running) return "";   // a bank that is driven block by block: the third process() call in a row starts the kernel
-  if (!rt_running) { std::string re = rt_stop(); if (!re.empty()) return re; }   // (another bank of this device may own the resident slot)
-  if (!rt_ctl) {
-    CU(cudaHostAlloc((void**)&rt_ctl, sizeof(RtCtl), cudaHostAllocMapped));
-    CU(cudaHostGetDevicePointer((void**)&rt_ctl_dev, rt_ctl, 0));
-    CU(cudaMalloc((void**)&d_rt_relay, 16));
-  }
-  if (rt_partial_cap < (size_t)grid * nout * 64) { cudaFree(d_rt_partial); d_rt_partial = nullptr; CU(cudaMalloc((void**)&d_rt_partial, (size_t)grid * nout * 64 * 4)); rt_partial_cap = (size_t)grid * nout * 64; }
+  if (!rt_running) TRY(rt_stop());   // (another bank of this device may own the resident slot)
+  TRY(rt_ctl.grow(1)); TRY(d_rt_relay.grow(4));
+  TRY(d_rt_partial.grow((size_t)grid * nout * 64));
   if (!rt_running) {
     const uint32_t first = ++rt_seq; if (rt_seq >= 0xfffffff0u) rt_seq = 1;
     memset((void*)rt_ctl, 0, sizeof(RtCtl));
@@ -877,11 +830,9 @@ std::string Bank::rt_process(uint32_t size, const float* in, float* out, bool* s
     CU(cudaMemcpyAsync(d_rt_relay, relay, 16, cudaMemcpyHostToDevice, stream));
     CU(cudaMemsetAsync(d_ticket, 0, 4, stream));
     BankArgs a;
-    { std::string se = state0_to_device(c, &a.state0); if (!se.empty()) return se; } a.dl_floats = (uint32_t)c.dl_floats;
-    a.params = c.d_params; a.state = c.d_state; a.uniform = c.d_uniform; a.dline = c.d_dline; a.wt = d_wt; a.in = nullptr; a.out = nullptr; a.partial = d_rt_partial;
-    a.V = c.V(); a.n = 64; a.vpc = vpc; a.in_stride = 0; a.in_offset = 0; a.out_stride = 0; a.out_offset = 0; a.row_map = c.d_rowmap;
-    a.sr = (float)sr; a.sd64 = (float)(1.0 / sr); a.sd32 = 1.0f / (float)sr; a.ticket = d_ticket; a.mix = nullptr; a.mix_stride = 0; a.mix_offset = 0; a.mix_accumulate = 0;
-    RtArgs rt{rt_ctl_dev, d_rt_relay, first};
+    TRY(voice_args(c, 64, vpc, &a));
+    a.partial = d_rt_partial; a.ticket = d_ticket;
+    RtArgs rt{rt_ctl.dev(), d_rt_relay, first};
     CU(cudaStreamSynchronize(stream));   // the relay words are in place (pageable source)
     CU(c.k->launch_rt(a, rt, table_bytes_of(c, 64), stream));
     launches++;
@@ -920,7 +871,7 @@ std::string Bank::rt_process(uint32_t size, const float* in, float* out, bool* s
 std::string Bank::dom_mark(cudaStream_t st) {   // called in pairs: begin, end
   static const bool off = getenv("FDSP_NO_DOM") != nullptr;   // A/B: what the event records themselves cost
   if (!timing || off) return "";
-  if (dom_n == dom_ev.size()) { cudaEvent_t e; CU(cudaEventCreate(&e)); dom_ev.push_back(e); }
+  if (dom_n == dom_ev.size()) { Event e; CU(cudaEventCreate(e.put())); dom_ev.push_back(std::move(e)); }
   CU(cudaEventRecord(dom_ev[dom_n++], st));
   return "";
 }
@@ -930,24 +881,33 @@ std::string Bank::render_device(uint64_t n, const float* in_dev, uint64_t in_str
   if (!has_parked()) return render_device_run(n, in_dev, in_stride, out_dev, out_stride, mix_dev, mix_stride);
   // parked Slot updates: the launch is cut behind the block in which a running fade ends, the parked unit is armed, the rest follows
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; }
+  TRY(rt_stop());
   uint64_t done = 0;
   do {
     uint64_t cut = n - done;
-    std::string e = slot_service(n - done, &cut);
-    if (!e.empty()) return e;
+    TRY(slot_service(n - done, &cut));
     if (cut == 0) break;
-    e = render_device_run(cut, in_dev ? in_dev + done : nullptr, in_stride, out_dev ? out_dev + done : nullptr, out_stride, mix_dev ? mix_dev + done : nullptr, mix_stride);
-    if (!e.empty()) return e;
+    TRY(render_device_run(cut, in_dev ? in_dev + done : nullptr, in_stride, out_dev ? out_dev + done : nullptr, out_stride, mix_dev ? mix_dev + done : nullptr, mix_stride));
     done += cut;
   } while (done < n);
+  return "";
+}
+
+// The window (input, output rows, partial and fused mix) is the caller's: it is left empty here. state0 / dl_floats are the reset image of
+// an Event class of a looping sequencer, null for every other class (state0_to_device); the kernels read dl_floats only with that image.
+std::string Bank::voice_args(VoiceClass& c, uint32_t len, uint32_t vpc, BankArgs* a) {
+  *a = BankArgs{};
+  TRY(state0_to_device(c, &a->state0)); a->dl_floats = (uint32_t)c.dl_floats;
+  a->params = c.d_params; a->state = c.d_state; a->uniform = c.d_uniform; a->dline = c.d_dline; a->wt = d_wt; a->row_map = c.d_rowmap;
+  a->V = c.V(); a->n = len; a->vpc = vpc;
+  a->sr = (float)sr; a->sd64 = (float)(1.0 / sr); a->sd32 = 1.0f / (float)sr;
   return "";
 }
 
 std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in_stride, float* out_dev, uint64_t out_stride, float* mix_dev,
                                     uint64_t mix_stride) {
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; }
+  TRY(rt_stop());
   if (!in_process) process_streak = 0;
   if (nin > 0 && !in_dev) return "#A bank has inputs but no input buffer was given";
   const bool want_v = (out_mode & 1u) && out_dev, want_m = (out_mode & 2u) && mix_dev;
@@ -979,12 +939,9 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
   bool joined = true;
   // FDSP_PIPE_TRACE=1: print the device timeline of the two pipeline stages (diagnostic; synchronises)
   const bool trace = pipelined && getenv("FDSP_PIPE_TRACE") != nullptr;
-  std::vector<cudaEvent_t> tev;   // per chunk: dry start, dry end, fdn start, fdn end
-  auto tmark = [&](cudaStream_t st) { if (trace) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); tev.push_back(e); } };
-  if (tree && !want_v) {
-    const size_t need = (size_t)V() * nout * CH;
-    if (rows_cap < need) { std::string e = dev_alloc(&d_rows, need); if (!e.empty()) return e; rows_cap = need; }
-  }
+  std::vector<Event> tev;   // per chunk: dry start, dry end, fdn start, fdn end
+  auto tmark = [&](cudaStream_t st) { if (trace) { tev.emplace_back(); cudaEventCreate(tev.back().put()); cudaEventRecord(tev.back(), st); } };
+  if (tree && !want_v) TRY(d_rows.grow((size_t)V() * nout * CH));
   const bool save_want_v = want_v, save_want_m = want_m;
   // pipelined banks accumulate into a zeroed mix: cleared once for the whole call, so that nothing sits between the dry-stage launches of
   // consecutive chunks on `stream` (a gap there lets the wide FDN kernel of the previous chunk take every SM first)
@@ -1018,67 +975,59 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
       const uint32_t V = c.V();
       cudaStream_t ks = stream;
       if (concurrent) {
-        if (!c.cstream) { CU(cudaStreamCreateWithFlags(&c.cstream, cudaStreamNonBlocking)); CU(cudaEventCreateWithFlags(&c.e_done, cudaEventDisableTiming)); }
+        if (!c.cstream) { CU(cudaStreamCreateWithFlags(c.cstream.put(), cudaStreamNonBlocking)); CU(cudaEventCreateWithFlags(c.e_done.put(), cudaEventDisableTiming)); }
         ks = c.cstream;
         CU(cudaStreamWaitEvent(ks, e_begin, 0));
       }
-      const uint32_t nsm = sm_count(device);
-      const bool staged = use_staged(c.k.get(), V, len, nsm);
+      const ClassGrid g = class_grid(c, len, device);
       int fdn_warps = 1;   // voices (= warps) per CTA of the FDN kernel
       if (c.fdn) {
         const int cap = fdn_max_warps();
         // pipelined: leave SMs free for the CTAs of the dry stage of the next chunk (their shared-memory tables cannot share an SM
         // with an FDN CTA), otherwise the two stages serialise on SM residency
+        const uint32_t nsm = sm_count(device);
         uint32_t sms = nsm;
-        if (pipelined && c.k) { uint32_t dv = 0; const uint32_t dry_ctas = staged ? staged_grid(V, nsm, &dv) : (V + (uint32_t)c.k->threads - 1) / (uint32_t)c.k->threads; sms = dry_ctas < nsm / 2 ? nsm - dry_ctas : nsm / 2; }
+        if (pipelined && c.k) sms = g.ctas < nsm / 2 ? nsm - g.ctas : nsm / 2;
         fdn_warps = (int)((V + sms - 1) / sms); if (fdn_warps > cap) fdn_warps = cap; if (fdn_warps < 1) fdn_warps = 1;
       }
-      // voice programs: whole waves of CTAs with the voices spread evenly; the dry stage of a two-stage class stays compact
-      // (few CTAs) so that it leaves the other SMs to the FDN kernel it is pipelined with
-      uint32_t vpc = c.k ? (uint32_t)c.k->threads : 0u;
-      const uint32_t vgrid = !c.k ? 0u : (staged ? staged_grid(V, nsm, &vpc) : (c.fdn || getenv("FDSP_NO_SPREAD") ? (V + vpc - 1) / vpc : bank_grid(V, (uint32_t)c.k->threads, nsm, &vpc)));
-      auto launch_voice = [&](const BankArgs& args, int md, cudaStream_t st) { return staged ? c.k->launch_staged(args, md, table_bytes_of(c, len), st) : c.k->launch(args, md, table_bytes_of(c, len), st); };
-      const uint32_t grid = c.fdn ? V : vgrid;   // rows of the partial-mix buffer: one per CTA of a voice program, one per VOICE of the FDN kernel (its warps never meet)
+      auto launch_voice = [&](const BankArgs& args, int md, cudaStream_t st) { return g.staged ? c.k->launch_staged(args, md, table_bytes_of(c, len), st) : c.k->launch(args, md, table_bytes_of(c, len), st); };
+      const uint32_t grid = c.fdn ? V : g.ctas;   // rows of the partial-mix buffer: one per CTA of a voice program, one per VOICE of the FDN kernel (its warps never meet)
+      BankArgs a;
+      TRY(voice_args(c, len, g.vpc, &a));
+      a.in = in_dev; a.in_stride = (uint32_t)in_stride; a.in_offset = (uint32_t)t0;
       if (c.conv) {
         // stage 1: the program in front of the convolver writes its rows behind the history columns; then x_lo, the Toeplitz GEMM tiles
         // (rows straight into the caller's buffer, or an internal one), the history shift, and the voice-order fold of the rows
-        BankArgs d{};
-        d.params = c.d_params; d.state = c.d_state; d.uniform = c.d_uniform; d.dline = c.d_dline; d.wt = d_wt; d.in = in_dev; d.partial = nullptr;
-        d.out = c.d_cx; d.V = V; d.n = len; d.vpc = vpc; d.in_stride = (uint32_t)in_stride; d.in_offset = (uint32_t)t0; d.out_stride = c.conv_stride; d.out_offset = c.conv_H;
-        d.row_map = c.d_dryrows; d.sr = (float)sr; d.sd64 = (float)(1.0 / sr); d.sd32 = 1.0f / (float)sr; d.ticket = nullptr; d.mix = nullptr; d.mix_stride = 0; d.mix_offset = 0; d.mix_accumulate = 0;
+        BankArgs d = a;
+        d.out = c.d_cx; d.out_stride = c.conv_stride; d.out_offset = c.conv_H; d.row_map = c.d_dryrows;
         CU(launch_voice(d, 1, stream));
         CU(launch_conv_split(c.d_cx, c.d_cxl, V, c.conv_stride, c.conv_H, len, stream));
         float* y = want_v ? out_dev_c : nullptr; uint32_t ys = (uint32_t)out_stride_c, yo = (uint32_t)out_t0;
         if (!y) {
-          if (c.crows_cap < (size_t)V * TIME_CHUNK) { std::string e = dev_alloc(&c.d_crows, (size_t)V * TIME_CHUNK); if (!e.empty()) return e; c.crows_cap = (size_t)V * TIME_CHUNK; }
+          TRY(c.d_crows.grow((size_t)V * TIME_CHUNK));
           y = c.d_crows; ys = TIME_CHUNK; yo = 0;
         }
-        { std::string de = dom_mark(stream); if (!de.empty()) return de; }
+        TRY(dom_mark(stream));
         CU(launch_conv_tc(c.conv_maps, y, ys, yo, c.d_dryrows, V, len, c.conv_K, c.conv_H, stream));
-        { std::string de = dom_mark(stream); if (!de.empty()) return de; }
+        TRY(dom_mark(stream));
         CU(launch_conv_history(c.d_cx, c.d_cxl, V, c.conv_stride, c.conv_H, len, stream));
         launches += 4;
         if (want_m) { CU(launch_tree_mix(y, V, 1u, ys, yo, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, 0, stream)); launches++; }
         first = false;
         continue;
       }
-      if (want_m) {
+      if (want_m) {   // (sized for the longest launch: TIME_CHUNK, or PIPE_CHUNK for the second buffer of a pipelined class)
         const size_t need = (size_t)grid * nout * len;
-        if (c.partial_floats < need) { std::string e = dev_alloc(&c.d_partial, (size_t)grid * nout * TIME_CHUNK); if (!e.empty()) return e; c.partial_floats = (size_t)grid * nout * TIME_CHUNK; }
-        if (pipelined && c.fdn && c.k && c.partial2_floats < need) { std::string e = dev_alloc(&c.d_partial2, (size_t)grid * nout * PIPE_CHUNK); if (!e.empty()) return e; c.partial2_floats = (size_t)grid * nout * PIPE_CHUNK; }
+        if (c.d_partial.size() < need) TRY(c.d_partial.grow((size_t)grid * nout * TIME_CHUNK));
+        if (pipelined && c.fdn && c.k && c.d_partial2.size() < need) TRY(c.d_partial2.grow((size_t)grid * nout * PIPE_CHUNK));
       }
-      BankArgs a;
-      { std::string se = state0_to_device(c, &a.state0); if (!se.empty()) return se; } a.dl_floats = (uint32_t)c.dl_floats;
-      a.params = c.d_params; a.state = c.d_state; a.uniform = c.d_uniform; a.dline = c.d_dline; a.wt = d_wt;
-      a.in = in_dev; a.out = want_v ? out_dev_c : nullptr; a.partial = want_m ? c.d_partial : nullptr;
-      a.V = V; a.n = len; a.vpc = vpc;
-      a.in_stride = (uint32_t)in_stride; a.in_offset = (uint32_t)t0;
+      a.out = want_v ? out_dev_c : nullptr;
+      if (want_m) a.partial = c.d_partial;
       a.out_stride = (uint32_t)out_stride_c; a.out_offset = (uint32_t)out_t0;
-      a.row_map = c.d_rowmap;
-      a.sr = (float)sr; a.sd64 = (float)(1.0 / sr); a.sd32 = 1.0f / (float)sr;
       // process()-sized launches of plain voice programs finish their mix-down inside the kernel (one launch instead of two)
       const bool fused_mix = want_m && !c.fdn && len <= 64;
-      a.ticket = fused_mix ? d_ticket : nullptr; a.mix = mix_dev; a.mix_stride = (uint32_t)mix_stride; a.mix_offset = (uint32_t)t0; a.mix_accumulate = first ? 0 : 1;
+      if (fused_mix) a.ticket = d_ticket;
+      a.mix = mix_dev; a.mix_stride = (uint32_t)mix_stride; a.mix_offset = (uint32_t)t0; a.mix_accumulate = first ? 0 : 1;
       if (t0 > 0xffffffffull - TIME_CHUNK) return "#A render too long for one call";
       if (c.fdn && len > TIME_CHUNK) return "internal: chunk";
       // long launches of wavetable programs stage the table set in shared memory (TMA bulk copy, ~160 KB per CTA);
@@ -1086,6 +1035,9 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
       if (c.fdn) {
         FdnArgs f;
         f.params = c.d_params; f.state = c.d_state; f.uniform = c.d_uniform; f.p0 = c.p0; f.s0 = c.s0; f.u0 = c.u0; f.scalar_row = c.scalar_row;
+        f.out = want_v ? out_dev_c : nullptr; f.row_map = c.d_rowmap; f.out_stride = (uint32_t)out_stride_c; f.out_offset = (uint32_t)out_t0;
+        f.partial = a.partial;
+        f.ring = c.d_ring; f.ring_voice_stride = c.ring_floats; f.V = V; f.n = len;
         if (c.k && pipelined) {
           // stage 1 of chunk k on `stream`, stage 2 on `stream2`; buffers alternate, chunk k-1's partial mix is reduced after
           // stage 1 of chunk k has been queued so that the two stages of neighbouring chunks run side by side
@@ -1103,16 +1055,14 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
           // holds its SMs before the wide FDN kernel of chunk k floods the rest — and reduces on stream2 behind the FDN kernel. With other
           // classes in the bank every reduction stays on `stream` (they accumulate into the same mix region), one chunk late.
           const bool solo = classes.size() == 1;
-          if (!solo) { std::string pe = flush_pending(&c); if (!pe.empty()) return pe; }   // reduce chunk k-1 of this class (waits for its FDN)
+          if (!solo) TRY(flush_pending(&c));   // reduce chunk k-1 of this class (waits for its FDN)
           f.dry = dry; f.dry_voice_stride = 2ull * PIPE_CHUNK; f.dry_ch_stride = PIPE_CHUNK; f.dry_offset = 0;
-          f.out = want_v ? out_dev_c : nullptr; f.row_map = c.d_rowmap; f.out_stride = (uint32_t)out_stride_c; f.out_offset = (uint32_t)out_t0;
-          f.partial = want_m ? (buf ? c.d_partial2 : c.d_partial) : nullptr;
-          f.ring = c.d_ring; f.ring_voice_stride = c.ring_floats; f.V = V; f.n = len;
+          if (want_m && buf) f.partial = c.d_partial2;
           CU(cudaStreamWaitEvent(stream2, c.e_dry[buf], 0));
           tmark(stream2);
-          { std::string de = dom_mark(stream2); if (!de.empty()) return de; }
+          TRY(dom_mark(stream2));
           CU(launch_fdn(f, fdn_warps, stream2));
-          { std::string de = dom_mark(stream2); if (!de.empty()) return de; }
+          TRY(dom_mark(stream2));
           launches++;
           tmark(stream2);
           CU(cudaEventRecord(c.e_fdn[buf], stream2));
@@ -1132,16 +1082,13 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
         } else {    // reverb applied straight to the bank's stereo input
           f.dry = in_dev; f.dry_voice_stride = 0; f.dry_ch_stride = (uint32_t)in_stride; f.dry_offset = (uint32_t)t0;
         }
-        f.out = want_v ? out_dev_c : nullptr; f.row_map = c.d_rowmap; f.out_stride = (uint32_t)out_stride_c; f.out_offset = (uint32_t)out_t0;
-        f.partial = want_m ? c.d_partial : nullptr;
-        f.ring = c.d_ring; f.ring_voice_stride = c.ring_floats; f.V = V; f.n = len;
-        { std::string de = dom_mark(stream); if (!de.empty()) return de; }
+        TRY(dom_mark(stream));
         CU(launch_fdn(f, fdn_warps, stream));
-        { std::string de = dom_mark(stream); if (!de.empty()) return de; }
+        TRY(dom_mark(stream));
       } else {
-        { std::string de = dom_mark(ks); if (!de.empty()) return de; }
+        TRY(dom_mark(ks));
         CU(launch_voice(a, mode, ks));
-        { std::string de = dom_mark(ks); if (!de.empty()) return de; }
+        TRY(dom_mark(ks));
       }
       launches++;
       if (concurrent) { CU(cudaEventRecord(c.e_done, ks)); continue; }   // reduced below, after every class has been launched
@@ -1155,10 +1102,7 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
       for (auto& c : classes) {
         CU(cudaStreamWaitEvent(stream, c.e_done, 0));
         if (want_m) {
-          uint32_t vpc = (uint32_t)c.k->threads;
-          const uint32_t nsm = sm_count(device);
-          const uint32_t grid = use_staged(c.k.get(), c.V(), len, nsm) ? staged_grid(c.V(), nsm, &vpc) : (getenv("FDSP_NO_SPREAD") ? (c.V() + vpc - 1) / vpc : bank_grid(c.V(), (uint32_t)c.k->threads, nsm, &vpc));
-          CU(launch_mix_reduce(c.d_partial, grid, (uint32_t)nout, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, first ? 0 : 1, stream));
+          CU(launch_mix_reduce(c.d_partial, class_grid(c, len, device).ctas, (uint32_t)nout, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, first ? 0 : 1, stream));
           launches++;
         }
         first = false;
@@ -1166,12 +1110,12 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
     }
     if (tree) {
       const size_t sc = tree_mix == 1 ? tree_mix_scratch_floats(V(), (uint32_t)nout, CH) : 0;   // balanced tree of a big bank: subtree sums first
-      if (sc > treepart_cap) { std::string e = dev_alloc(&d_treepart, sc); if (!e.empty()) return e; treepart_cap = sc; }
-      CU(launch_tree_mix(out_dev_c, V(), (uint32_t)nout, (uint32_t)out_stride_c, (uint32_t)out_t0, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, tree_mix == 1 ? 1 : 0, stream, sc ? d_treepart : nullptr));
+      TRY(d_treepart.grow(sc));
+      CU(launch_tree_mix(out_dev_c, V(), (uint32_t)nout, (uint32_t)out_stride_c, (uint32_t)out_t0, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, tree_mix == 1 ? 1 : 0, stream, sc ? d_treepart.get() : nullptr));
       launches += sc ? 2 : 1;
     }
   }
-  { std::string pe = flush_pending(nullptr); if (!pe.empty()) return pe; }   // also joins stream2 back into `stream`
+  TRY(flush_pending(nullptr));   // also joins stream2 back into `stream`
   if (!joined) { CU(cudaEventRecord(e_begin, stream2)); CU(cudaStreamWaitEvent(stream, e_begin, 0)); }   // solo two-stage class: its reductions ran on stream2
   if (timing) CU(cudaEventRecord(ev1, stream));
   if (trace) {
@@ -1181,28 +1125,24 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
       for (int w = 0; w < 4; w++) cudaEventElapsedTime(&t[w], ev0, tev[q + w]);
       fprintf(stderr, "[pipe] chunk %zu: dry %.3f..%.3f ms   fdn %.3f..%.3f ms\n", q / 4, t[0], t[1], t[2], t[3]);
     }
-    for (auto e : tev) cudaEventDestroy(e);
   }
   dirty = true; advance_clock(n);
   return "";
 }
 
 std::string Bank::ensure_staging(uint32_t chunk) {
-  { std::string re = rt_stop(); if (!re.empty()) return re; }   // allocations synchronise with the device: no resident kernel may be waiting on its doorbell
-  const size_t rows = (size_t)V() * nout;
-  std::string e;
-  if (nin > 0 && in_cap < (size_t)nin * chunk) { if (!(e = dev_alloc(&d_in, (size_t)nin * chunk)).empty()) return e; in_cap = (size_t)nin * chunk; }
-  if ((out_mode & 1u) && out_cap < rows * chunk) { if (!(e = dev_alloc(&d_out, rows * chunk)).empty()) return e; out_cap = rows * chunk; }
-  if ((out_mode & 2u) && mix_cap < (size_t)nout * chunk) { if (!(e = dev_alloc(&d_mix, (size_t)nout * chunk)).empty()) return e; mix_cap = (size_t)nout * chunk; }
-  stage_chunk = std::max(stage_chunk, chunk);
+  TRY(rt_stop());   // allocations synchronise with the device: no resident kernel may be waiting on its doorbell
+  if (nin > 0) TRY(d_in.grow((size_t)nin * chunk));
+  if (out_mode & 1u) TRY(d_out.grow((size_t)V() * nout * chunk));
+  if (out_mode & 2u) TRY(d_mix.grow((size_t)nout * chunk));
   return "";
 }
 
 std::string Bank::render_host(uint64_t n, const float* in, float* out_voices, float* out_mix) {
   CU(cudaSetDevice(device));
-  { std::string re = rt_stop(); if (!re.empty()) return re; }
+  TRY(rt_stop());
   if (n == 0) return "";
-  { std::string se = sh_pull(); if (!se.empty()) return se; }
+  TRY(sh_pull());
   const size_t rows = (size_t)V() * nout;
   // chunk so that the per-voice staging buffer stays below ~512 MB
   uint32_t chunk = TIME_CHUNK;
@@ -1211,16 +1151,14 @@ std::string Bank::render_host(uint64_t n, const float* in, float* out_voices, fl
     chunk = (uint32_t)std::max<uint64_t>(64, std::min<uint64_t>(TIME_CHUNK, cap / 64 * 64));
   }
   chunk = (uint32_t)std::min<uint64_t>(chunk, (n + 63) / 64 * 64);
-  std::string e = ensure_staging(chunk);
-  if (!e.empty()) return e;
+  TRY(ensure_staging(chunk));
   for (uint64_t t0 = 0; t0 < n; t0 += chunk) {
     const uint32_t len = (uint32_t)std::min<uint64_t>(chunk, n - t0);
     if (nin > 0) {
       if (!in) return "#A bank has inputs but no input buffer was given";
       CU(cudaMemcpy2DAsync(d_in, (size_t)chunk * 4, in + t0, (size_t)n * 4, (size_t)len * 4, nin, cudaMemcpyHostToDevice, stream));
     }
-    e = render_device(len, d_in, chunk, (out_voices ? d_out : nullptr), chunk, (out_mix ? d_mix : nullptr), chunk);
-    if (!e.empty()) return e;
+    TRY(render_device(len, d_in, chunk, (out_voices ? d_out.get() : nullptr), chunk, (out_mix ? d_mix.get() : nullptr), chunk));
     if (out_voices && (out_mode & 1u)) CU(cudaMemcpy2DAsync(out_voices + t0, (size_t)n * 4, d_out, (size_t)chunk * 4, (size_t)len * 4, rows, cudaMemcpyDeviceToHost, stream));
     if (out_mix && (out_mode & 2u)) CU(cudaMemcpy2DAsync(out_mix + t0, (size_t)n * 4, d_mix, (size_t)chunk * 4, (size_t)len * 4, nout, cudaMemcpyDeviceToHost, stream));
   }
@@ -1241,39 +1179,30 @@ std::string Bank::process(uint32_t size, const float* in, float* out) {  // Audi
     if (!re.empty()) return re;
     process_streak = keep;
   }
-  std::string e = ensure_staging(64);
-  if (!e.empty()) return e;
+  TRY(ensure_staging(64));
   const bool mix = (out_mode & 2u) != 0;  // mix mode wins for the AudioUnit surface; voices mode returns V*c channels
   const size_t rows = mix ? (size_t)nout : (size_t)V() * nout;
-  if (h_in_cap < (size_t)std::max(1, nin) * 64) { if (h_in) cudaFreeHost(h_in); CU(cudaMallocHost((void**)&h_in, (size_t)std::max(1, nin) * 64 * 4)); h_in_cap = (size_t)std::max(1, nin) * 64; }
-  if (h_out_cap < rows * 64) {
-    if (h_out) cudaFreeHost(h_out);
-    CU(cudaHostAlloc((void**)&h_out, rows * 64 * 4, cudaHostAllocMapped));   // mapped: the mix is written straight into it by the GPU
-    CU(cudaHostGetDevicePointer((void**)&d_hout, h_out, 0));
-    h_out_cap = rows * 64;
-  }
+  TRY(h_in.grow((size_t)std::max(1, nin) * 64));
+  TRY(h_out.grow(rows * 64));   // mapped: the mix is written straight into it by the GPU
   if (nin > 0) {
     if (!in) return "#A bank has inputs but no input buffer was given";
     memcpy(h_in, in, (size_t)nin * 64 * 4);
     CU(cudaMemcpyAsync(d_in, h_in, (size_t)nin * 64 * 4, cudaMemcpyHostToDevice, stream));
   }
-  { std::string se = sh_pull(); if (!se.empty()) return se; }
+  TRY(sh_pull());
   struct NoTiming { bool& t; explicit NoTiming(bool& x) : t(x) { t = false; } ~NoTiming() { t = true; } } no_timing(timing);  // no event records on this path
   struct InProcess { bool& f; explicit InProcess(bool& x) : f(x) { f = true; } ~InProcess() { f = false; } } in_proc(in_process);
   bool two_stage = false;   // pipelined classes clear / accumulate the mix region on the device: keep that in device memory
   for (auto& c : classes) two_stage = two_stage || (c.fdn && c.k);
   if (mix && two_stage) {
-    e = render_device(size, d_in, 64, nullptr, 64, d_mix, 64);
-    if (!e.empty()) return e;
+    TRY(render_device(size, d_in, 64, nullptr, 64, d_mix, 64));
     CU(cudaMemcpyAsync(h_out, d_mix, rows * 64 * 4, cudaMemcpyDeviceToHost, stream));
   } else if (mix) {
     // one block of mix is a few hundred bytes: mix_reduce_kernel stores it over PCIe into the mapped host buffer, which saves
     // the separate device-to-host copy of the latency-critical process() path
-    e = render_device(size, d_in, 64, nullptr, 64, d_hout, 64);
-    if (!e.empty()) return e;
+    TRY(render_device(size, d_in, 64, nullptr, 64, h_out.dev(), 64));
   } else {
-    e = render_device(size, d_in, 64, d_out, 64, nullptr, 64);
-    if (!e.empty()) return e;
+    TRY(render_device(size, d_in, 64, d_out, 64, nullptr, 64));
     CU(cudaMemcpyAsync(h_out, d_out, rows * 64 * 4, cudaMemcpyDeviceToHost, stream));
   }
   CU(cudaStreamSynchronize(stream));
@@ -1282,14 +1211,13 @@ std::string Bank::process(uint32_t size, const float* in, float* out) {  // Audi
 }
 
 std::string Bank::clone_into(Bank& dst) const {
-  { std::string re = const_cast<Bank*>(this)->rt_stop(); if (!re.empty()) return re; }
+  TRY(const_cast<Bank*>(this)->rt_stop());
   std::vector<HNode*> copies;
   for (auto& n : nodes) copies.push_back(n->clone());
   dst.sr = sr; dst.tree_mix = tree_mix; dst.net_rate = net_rate; dst.vertex_of_voice = vertex_of_voice;
-  std::string e = dst.init(copies, device, out_mode);
-  if (!e.empty()) return e;
+  TRY(dst.init(copies, device, out_mode));
   for (auto& n : dst.nodes) n->set_sample_rate(sr);
-  if (!(e = dst.lower_and_upload(true)).empty()) return e;
+  TRY(dst.lower_and_upload(true));
   CU(cudaSetDevice(device));
   CU(cudaStreamSynchronize(stream));
   for (size_t i = 0; i < classes.size(); i++) {
@@ -1348,14 +1276,9 @@ std::string Bank::sh_rebuild() {
     CU(cudaStreamSynchronize(stream));
     for (size_t r = 0; r < c.sh_rows.size(); r++) CU(cudaMemcpy(c.sh_img.data() + r * Vc, c.d_params + (size_t)c.sh_rows[r] * Vc, (size_t)Vc * 4, cudaMemcpyDeviceToHost));
   }
-  if (stage > sh_stage_cap) {
-    if (sh_pending) { CU(cudaEventSynchronize(sh_copied)); sh_pending = false; }
-    if (sh_stage) cudaFreeHost(sh_stage);
-    sh_stage = nullptr; sh_stage_cap = 0;
-    CU(cudaMallocHost((void**)&sh_stage, stage * 4));
-    sh_stage_cap = stage;
-  }
-  if (stage && !sh_copied) CU(cudaEventCreateWithFlags(&sh_copied, cudaEventDisableTiming));
+  if (stage > sh_stage.size() && sh_pending) { CU(cudaEventSynchronize(sh_copied)); sh_pending = false; }   // (grow frees the staging)
+  TRY(sh_stage.grow(stage));
+  if (stage && !sh_copied) CU(cudaEventCreateWithFlags(sh_copied.put(), cudaEventDisableTiming));
   return "";
 }
 
@@ -1376,7 +1299,7 @@ std::string Bank::sh_pull() {
         if (k >= 0 && c.sh_img[r * Vc + i] != now[k]) { c.sh_img[r * Vc + i] = now[k]; changed = true; }
       }
       if (!changed) continue;
-      if (at + Vc > sh_stage_cap) return "internal: Shared staging too small";
+      if (at + Vc > sh_stage.size()) return "internal: Shared staging too small";
       memcpy(sh_stage + at, c.sh_img.data() + r * Vc, (size_t)Vc * 4);
       CU(cudaMemcpyAsync(c.d_params + (size_t)c.sh_rows[r] * Vc, sh_stage + at, (size_t)Vc * 4, cudaMemcpyHostToDevice, stream));
       sh_pending = true;

@@ -8,6 +8,7 @@
 #include <string>
 #include <vector>
 
+#include "cuda_owned.h"
 #include "graph.h"
 #include "registry.h"
 #include "../dsp/rt_args.h"
@@ -27,18 +28,18 @@ struct VoiceClass {
   uint32_t np = 0, ns = 0, nu = 0;  // words per voice (whole graph)
   // reverb_stereo tail handled by the warp-per-voice FDN kernel (dsp/fdn_kernel.cuh); `k` is then the dry-stage program (may be null)
   bool fdn = false; int scalar_row = -1; uint32_t p0 = 0, s0 = 0, u0 = 0; uint64_t ring_floats = 0;
-  float* d_ring = nullptr; float* d_dry = nullptr; uint32_t* d_dryrows = nullptr;
+  Array<float> d_ring, d_dry; Array<uint32_t> d_dryrows;
   // `... >> convolve(h)` tail on tensor cores (dsp/conv_tc_kernel.cuh): `k` is then the program in front of the Convolver; its output rows
   // live in d_cx [V][conv_H + chunk] (history columns in front), d_cxl = their TF32 remainders, d_th / d_tl = Toeplitz(h) hi / lo
   bool conv = false; uint32_t conv_K = 0, conv_H = 0, conv_J = 0, conv_stride = 0, conv_off = 0;
-  float *d_cx = nullptr, *d_cxl = nullptr, *d_th = nullptr, *d_tl = nullptr, *d_crows = nullptr; size_t crows_cap = 0;
+  Array<float> d_cx, d_cxl, d_th, d_tl, d_crows;
   ConvTcMaps conv_maps;
   // two-stage classes are software-pipelined over sub-chunks: dry stage of chunk k+1 (stream) runs beside the FDN of chunk k (stream2)
-  float* d_dry2 = nullptr; float* d_partial2 = nullptr; size_t partial2_floats = 0;
-  cudaEvent_t e_dry[2] = {nullptr, nullptr}, e_fdn[2] = {nullptr, nullptr};
+  Array<float> d_dry2, d_partial2;
+  Event e_dry[2], e_fdn[2];
   // banks with several plain classes run the class kernels side by side, each on its own stream (one class alone leaves most
   // warp schedulers with a single warp)
-  cudaStream_t cstream = nullptr; cudaEvent_t e_done = nullptr;
+  Stream cstream; Event e_done;
   std::vector<uint32_t> state0;     // initial state, SoA [NS][V]
   // what AudioUnit::reset leaves alone (Lowering::keepS / keepD): state word ranges and delay-line float ranges (per voice), ascending
   std::vector<std::pair<uint64_t, uint64_t>> keep_s, keep_d;
@@ -46,9 +47,9 @@ struct VoiceClass {
   // voice's word there is no reader) and the host image of those rows, [row][V]
   std::vector<uint32_t> sh_rows; std::vector<int32_t> sh_cell; std::vector<uint32_t> sh_img;
   // looping sequencer banks: the reset image also lives on the device (Event<X> resets its unit from it when the event ends, src/sequencer.rs:631-633)
-  uint32_t* d_state0 = nullptr; bool state0_stale = true;
-  uint32_t* d_params = nullptr; uint32_t* d_state = nullptr; uint32_t* d_uniform = nullptr; uint32_t* d_rowmap = nullptr;
-  float* d_dline = nullptr; float* d_partial = nullptr; size_t partial_floats = 0;
+  Array<uint32_t> d_state0; bool state0_stale = true;
+  Array<uint32_t> d_params, d_state, d_uniform, d_rowmap;
+  Array<float> d_dline, d_partial;
   uint32_t V() const { return (uint32_t)voices.size(); }
 };
 
@@ -57,31 +58,33 @@ struct Bank {
   double sr = DEFAULT_SR; bool dirty = false;
   // voices extracted from a Net: mix in the Net's own association order (0 none, 1 pairwise tree, 2 left fold) and hand the
   // units the Net's f32-rounded sample rate (src/net.rs:132,1323-1328)
-  int tree_mix = 0; bool net_rate = false; float* d_rows = nullptr; size_t rows_cap = 0; float* d_treepart = nullptr; size_t treepart_cap = 0;
+  int tree_mix = 0; bool net_rate = false; Array<float> d_rows, d_treepart;
   std::vector<std::unique_ptr<HNode>> nodes;
   std::vector<int> vertex_of_voice;   // banks made from a Net: the Net vertex (NodeId) behind each voice
   std::vector<VoiceClass> classes;
-  cudaStream_t stream = nullptr, stream2 = nullptr; cudaEvent_t ev0 = nullptr, ev1 = nullptr, e_begin = nullptr;
-  WaveTableDev* d_wt = nullptr; float* d_wtdata[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}; WaveTableDev h_wt[6] = {};   // h_wt: host copy of the table directory
+  Stream stream, stream2; Event ev0, ev1, e_begin;
+  Array<WaveTableDev> d_wt; Array<float> d_wtdata[6]; WaveTableDev h_wt[6] = {};   // h_wt: host copy of the table directory
   // staging for host-buffer entry points
-  float *d_in = nullptr, *d_out = nullptr, *d_mix = nullptr; size_t in_cap = 0, out_cap = 0, mix_cap = 0; uint32_t stage_chunk = 0;
-  float *h_in = nullptr, *h_out = nullptr, *d_hout = nullptr; size_t h_in_cap = 0, h_out_cap = 0;  // pinned (h_out also device-mapped), process() path
+  Array<float> d_in, d_out, d_mix;
+  PinnedArray<float> h_in; MappedArray<float> h_out;   // process() path
   uint64_t launches = 0; float last_ms = 0.0f;
-  uint32_t* d_ticket = nullptr;   // arrival counter of the fused mix-down (short launches)
+  Array<uint32_t> d_ticket;       // arrival counter of the fused mix-down (short launches)
   bool timing = true;             // record ev0/ev1 around render_device (off on the process() path)
   // event pairs around the DOMINANT kernel of every chunk (the voice program; the FDN kernel of a two-stage class; the tensor-core tiles of
   // a convolver class), on the stream it is launched on: bench.py's roofline divides by this, not by the whole render
-  std::vector<cudaEvent_t> dom_ev; size_t dom_n = 0; float last_dom_ms = 0.0f;
+  std::vector<Event> dom_ev; size_t dom_n = 0; float last_dom_ms = 0.0f;
   std::string dom_mark(cudaStream_t st);
 
   // resident process() kernel (dsp/bank_kernel_rt.cuh): a single-class bank that is driven block by block keeps one kernel on the GPU
   // and rings a doorbell per block; every other call on the bank stops it first (state words are saved on the way out)
-  RtCtl* rt_ctl = nullptr; RtCtl* rt_ctl_dev = nullptr; uint32_t* d_rt_relay = nullptr; float* d_rt_partial = nullptr; size_t rt_partial_cap = 0;
+  MappedArray<RtCtl> rt_ctl; Array<uint32_t> d_rt_relay; Array<float> d_rt_partial;   // (the kernel reads rt_ctl until it exits: ~Bank stops it first)
   bool rt_running = false, in_process = false; uint32_t rt_seq = 1; uint32_t process_streak = 0;
   std::string rt_stop();
+  std::string rt_end_streak() { std::string e = rt_stop(); if (e.empty()) process_streak = 0; return e; }   // the next process() calls start a new streak
   std::string rt_process(uint32_t size, const float* in, float* out, bool* served);
   ~Bank();
   uint32_t V() const { return (uint32_t)nodes.size(); }
+  double unit_rate() const { return net_rate ? (double)(float)sr : sr; }   // the sample rate the voices' units are given
   std::string init(std::vector<HNode*>& voices, int device, uint32_t out_mode);  // returns "" or error text
   std::string lower_and_upload(bool upload_state);
   std::string set_sample_rate(double sr);
@@ -98,6 +101,8 @@ struct Bank {
   std::string replace_voice(uint32_t voice, HNode* node);                     // a new unit in the slot of a voice of the same class; consumes node
   struct Carry { uint32_t src_s, dst_s, ns; uint64_t src_d, dst_d, nd; };    // state words / delay-line floats of the OLD voice that move into the new one
   std::string regroup(HNode* unit, int at, uint32_t* voice, const Carry* carry = nullptr);   // classes rebuilt around one new / replaced voice, running state of the others kept
+  // a unit entering the running bank: `l0` as constructed (what reset() restores), `l` as it runs from now (at the sequencer's clock; `fading`: fading in)
+  void lower_entering(HNode* n, Lowering* l0, Lowering* l, bool fading) const;
   std::string crossfade_voice(uint32_t voice, int ease, float fade_time, HNode* unit);   // Net::crossfade: fade the voice to a unit of any class; consumes unit
   std::string remove_voice(uint32_t voice);                                   // Net::remove: the voice carries silence from now on
   std::string add_voice(HNode* unit, uint32_t* voice);                        // grow by one voice, running state of the others preserved; consumes unit
@@ -112,6 +117,7 @@ struct Bank {
   bool has_parked() const { return !slot_latest.empty() || !xfade_latest.empty(); }
   std::string slot_arm_now(uint32_t voice, int ease, double fade_time, HNode* unit, bool force);   // consumes unit; force: also while a fade is running (reset adopts `latest`)
   std::string slot_service(uint64_t n, uint64_t* cut);   // arms parked units whose fade is over; *cut = samples (<= n) after which the first running fade with a parked unit ends
+  std::string voice_args(VoiceClass& c, uint32_t len, uint32_t vpc, BankArgs* a);   // class c's part of a launch's arguments; the window starts empty
   std::string render_device_run(uint64_t n, const float* in_dev, uint64_t in_stride, float* out_dev, uint64_t out_stride, float* mix_dev, uint64_t mix_stride);
   std::string push_event(HNode* event, uint32_t* voice);                      // Sequencer::push on a running bank: takes the slot of a finished event of the same class; consumes event
   std::string set(uint32_t voice, const Setting& s);  // AudioUnit::set on one voice of a live bank (parameters only; state continues)
@@ -129,8 +135,8 @@ struct Bank {
   std::vector<uint32_t> sh_last;                 // the cells' values at the last sh_pull (empty: compare every reader word)
   struct ShWriter { int cls = -1; uint32_t word = 0, col = 0, voice = 0; };
   std::vector<ShWriter> sh_last_writer;          // per cell: the write-back word stored after a call (cls < 0: the cell is read)
-  uint32_t* sh_stage = nullptr; size_t sh_stage_cap = 0;   // pinned staging of the reader rows sh_pull copies ([row][V] of every class in turn)
-  cudaEvent_t sh_copied = nullptr; bool sh_pending = false; // recorded behind those copies: the staging is rewritten only after they have landed
+  PinnedArray<uint32_t> sh_stage;   // staging of the reader rows sh_pull copies ([row][V] of every class in turn)
+  Event sh_copied; bool sh_pending = false; // recorded behind those copies: the staging is rewritten only after they have landed
   std::string sh_check(uint32_t voice, const std::vector<SharedUse>& uses) const;   // "" or the refusal when `voice` would use `uses`
   std::string sh_rebuild();
   std::string sh_pull();

@@ -51,7 +51,6 @@ Nccl& nccl() {
 }
 std::string nerr(const char* what, int rc) { return std::string(what) + ": " + (nccl().GetErrorString ? nccl().GetErrorString(rc) : "NCCL error"); }
 #define NC(call) do { int rc_ = (call); if (rc_ != 0) return nerr(#call, rc_); } while (0)
-#define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return std::string(#call) + ": " + cudaGetErrorString(e_); } while (0)
 
 #ifndef FDSP_HOST_EMUL
 // root: mix[c][t] = ((p_0 + p_1) + p_2) + ... in rank order; the root's own partial is read from `mix` itself
@@ -70,8 +69,7 @@ __global__ void rank_fold_kernel(float* mix, uint32_t mix_stride, const float* g
 }  // namespace
 
 Group::~Group() {
-  cudaSetDevice(device);
-  if (d_gather) cudaFree(d_gather);
+  cudaSetDevice(device);   // (also for d_gather, released after this body)
   if (comm && nccl().ok) nccl().CommDestroy((ncclComm_t)comm);
 }
 
@@ -135,10 +133,10 @@ std::string group_reduce_device(Bank& b, Group& g, uint64_t n, float* mix_dev, u
     return "";
   }
   const size_t plane = (size_t)ch * n;
-  if (g.rank == root && g.gather_cap < plane * g.nranks) {
-    if (g.d_gather) { CU(cudaStreamSynchronize(b.stream)); cudaFree(g.d_gather); g.d_gather = nullptr; }
-    CU(cudaMalloc((void**)&g.d_gather, plane * g.nranks * sizeof(float)));
-    g.gather_cap = plane * g.nranks;
+  if (g.rank == root && g.d_gather.size() < plane * g.nranks) {
+    if (g.d_gather) CU(cudaStreamSynchronize(b.stream));   // (earlier receives may still be landing in it)
+    std::string e = g.d_gather.grow(plane * g.nranks);
+    if (!e.empty()) return e;
   }
   GroupScope gs(N);
   NC(gs.start());

@@ -19,7 +19,7 @@ namespace host {
 struct Group {
   int nranks = 1, rank = 0, device = 0;
   void* comm = nullptr;            // ncclComm_t
-  float* d_gather = nullptr; size_t gather_cap = 0;   // root: [nranks][channels][chunk]
+  Array<float> d_gather;           // root: [nranks][channels][chunk]
   bool nccl_reduce = false;
   ~Group();
 };

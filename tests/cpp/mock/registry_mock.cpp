@@ -147,3 +147,6 @@ std::string jit_precompile(const std::string&, int, int, int) { return "mock reg
 
 }  // namespace host
 }  // namespace fdsp
+
+// live mock allocations, streams and events (tests/test_bank_resources_cpu.py)
+extern "C" long fdsp_mock_live_resources() { return mock_live(); }
