@@ -148,6 +148,9 @@ API fdsp_node* fdsp_shape_fn(const char* closure, int ncaptures, const char* con
 API fdsp_node* fdsp_envelope_in(double interval, int inputs, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values) {
   return closure_node(CL_ENVELOPE_IN, inputs, outputs, interval, closure, ncaptures, names, values);
 }
+API fdsp_node* fdsp_envelope_text(double interval, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values) {
+  return closure_node(CL_ENVELOPE, 0, outputs, interval, closure, ncaptures, names, values);
+}
 API fdsp_node* fdsp_shaper_adaptive(double timescale, int inner_kind, float p0, float p1) {
   std::string e;
   HNode* n = mk_shaper_adaptive(timescale, inner_kind, p0, p1, e);

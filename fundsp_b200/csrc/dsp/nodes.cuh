@@ -2349,6 +2349,58 @@ template <int NI, int NO, int NC, class E> struct EnvelopeInFn {
   static FDSP_DEV void end_simd(R&) {}
 };
 
+// Envelope<f32, E, R> (src/envelope.rs:14-183, ID 14) with the closure E of time in the type. It samples at the same jittered points as
+// EnvelopeTab, from the same hash, but evaluates E there instead of reading a table, so nothing holds past a horizon. The host lowers
+// reset's t = t_0 = t_1 = 0; E(0), which reset() stores as value_0 = value_1, is evaluated by the first next_segment (t_1 > 0 after it).
+// The block path follows process (:139-163): a run ending a segment moves to the next one at once, as the reference does.
+template <int NO, int NC, class E> struct EnvelopeFn {
+  FDSP_NODE(0, NO, NC + 1, 8 + 4 * NO, 0);
+  typedef typename EnvelopeInFn<0, NO, NC, E>::R R;
+  static FDSP_DEV void load(R& r, Loader& l) { EnvelopeInFn<0, NO, NC, E>::load(r, l); }
+  static FDSP_DEV void save(const R& r, Saver& s) { EnvelopeInFn<0, NO, NC, E>::save(r, s); }
+  static FDSP_DEV void call(const R& r, float time, float* out) { const Ex::Root s{nullptr, r.c, time}; Ex::Emit<E>::out(s, out); }
+  template <class C> static FDSP_DEV void next_segment(R& r, const C& c) {   // :80-101
+    if (r.t0 == 0.0f && r.t1 == 0.0f) call(r, 0.0f, r.v1);                 // reset :114-122
+    r.t0 = r.t1;
+#pragma unroll
+    for (int k = 0; k < NO; k++) r.v0[k] = r.v1[k];
+    const float next_interval = lerpf(0.75f, 1.25f, (float)rnd1(r.t_hash)) * r.interval;
+    r.t1 = r.t0 + next_interval;
+    call(r, r.t1, r.v1);
+    r.t_hash = r.t_hash * 6364136223846793005ull + 1ull;
+    const float u = delerpf(r.t0, r.t1, r.t);
+    const float samples = next_interval / c.sd64;
+#pragma unroll
+    for (int k = 0; k < NO; k++) { r.value[k] = lerpf(r.v0[k], r.v1[k], u); r.delta[k] = (r.v1[k] - r.v0[k]) / samples; }
+  }
+  template <class C> static FDSP_DEV void plan(R& r, const C& c) {   // the while-loop of :144-162 from block index c.i
+    for (;;) {
+      const unsigned long long left = (unsigned long long)(long long)ceilf((r.t1 - r.t) / c.sd64);
+      const unsigned long long room = (unsigned long long)(c.n - c.i);
+      const unsigned long long loop = left < room ? left : room;
+      if (loop == 0ull) { next_segment(r, c); continue; }
+      r.run = (uint32_t)loop; r.run_len = r.run; r.seg_end = (loop == left) ? 1u : 0u;
+      return;
+    }
+  }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<0>&, Fr<NO>& o) {
+    if (T) {   // tick :129-137
+      if (r.t >= r.t1) next_segment(r, c);
+#pragma unroll
+      for (int k = 0; k < NO; k++) { o.v[k] = r.value[k]; r.value[k] += r.delta[k]; }
+      r.t += c.sd64;
+      return;
+    }
+    if (c.i == 0) { if (r.t >= r.t1) next_segment(r, c); plan(r, c); }
+    else if (r.run == 0u) plan(r, c);
+#pragma unroll
+    for (int k = 0; k < NO; k++) { o.v[k] = r.value[k]; r.value[k] += r.delta[k]; }
+    r.run -= 1u;
+    if (r.run == 0u) { r.t += (float)r.run_len * c.sd64; if (r.seg_end) next_segment(r, c); }
+  }
+  static FDSP_DEV void end_simd(R&) {}
+};
+
 
 // ---------------------------------------------------------------- Dag: a whole Net as ONE fused node (src/net.rs:118-146, 1224-1286)
 // The reference's Net is a dynamic DAG of boxed units processed vertex by vertex in dependency order, each vertex reading the
@@ -2491,6 +2543,7 @@ template <int NI, int NO, int NC, class E> struct Cost<Map<NI, NO, NC, E>> { sta
 template <int NC, class E> struct Cost<ShaperFn<NC, E>> { static constexpr int value = 2 + E::cost; };
 template <int NO, int NC, class E> struct Cost<VarFn<NO, NC, E>> { static constexpr int value = NO; };
 template <int NI, int NO, int NC, class E> struct Cost<EnvelopeInFn<NI, NO, NC, E>> { static constexpr int value = 120; };
+template <int NO, int NC, class E> struct Cost<EnvelopeFn<NO, NC, E>> { static constexpr int value = 120; };
 template <> struct Cost<Delay> { static constexpr int value = 12; };
 template <int N> struct Cost<Panner<N>> { static constexpr int value = N == 1 ? 2 : 80; };
 template <int K, class X, class Y> struct Cost<Binop<K, X, Y>> { static constexpr int value = Cost<X>::value + Cost<Y>::value + 1; };

@@ -389,6 +389,9 @@ std::string parse_closure(const char* text, ClosureKind kind, int inputs, int ou
     } else if (kind == CL_SHAPE_FN || kind == CL_VAR_FN) {
       if (np != 1) return arity(kind == CL_VAR_FN ? "var_fn takes one parameter |x|" : "shape_fn takes one parameter |x|");
       ps.params.push_back({names[0], PK_SCALAR, 0});
+    } else if (kind == CL_ENVELOPE) {
+      if (np != 1) return arity("envelope takes one time parameter |t|");
+      ps.params.push_back({names[0], PK_TIME, 0});
     } else {
       if (np == 2 && inputs != 1) { ps.params.push_back({names[0], PK_TIME, 0}); ps.params.push_back({names[1], PK_FRAME, 0}); }
       else if (np == 2 && inputs == 1) { ps.params.push_back({names[0], PK_TIME, 0}); ps.params.push_back({names[1], PK_FRAME_OR_SCALAR, 0}); }

@@ -1,4 +1,4 @@
-// fundsp_b200 closure parser: the text of a closure of the signal (map, shape_fn, envelope_in) -> the type expression the device
+// fundsp_b200 closure parser: the text of a closure of the signal or of time (map, shape_fn, envelope_in, envelope) -> the type expression the device
 // compiles (the Ex:: templates of csrc/dsp/nodes.cuh). The text is a subset of Rust closure syntax (DESIGN.md §2); user text never
 // reaches NVRTC, only the type expression generated from the parsed tree.
 #pragma once
@@ -8,7 +8,8 @@
 namespace fdsp {
 namespace host {
 
-enum ClosureKind { CL_MAP = 0, CL_SHAPE_FN = 1, CL_ENVELOPE_IN = 2, CL_VAR_FN = 3 };   // CL_VAR_FN: var_fn's |x| of the Shared's value
+// CL_VAR_FN: var_fn's |x| of the Shared's value; CL_ENVELOPE: envelope / lfo's |t| of time alone
+enum ClosureKind { CL_MAP = 0, CL_SHAPE_FN = 1, CL_ENVELOPE_IN = 2, CL_VAR_FN = 3, CL_ENVELOPE = 4 };
 constexpr int CLOSURE_MAX_TEXT = 4096;   // bytes
 constexpr int CLOSURE_MAX_OPS = 256;     // operators, calls and literals: bounds the template depth NVRTC sees
 

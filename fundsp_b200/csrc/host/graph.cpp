@@ -967,25 +967,29 @@ struct AdsrLive : HNode {
 
 // ---------------------------------------------------------------- closures of the signal (csrc/host/closure.cpp parses the text)
 // The parsed closure is part of the signature; the captured values are per-voice parameter words in Cap<k> order.
+// CL_ENVELOPE is Envelope<f32> (src/envelope.rs:14-183) with its closure of time compiled into the voice program: unlike EnvelopeN above
+// it stores no sampled values, so it has no horizon and its words do not grow with the length of the render.
 struct ClosureN : HNode {
   ClosureKind kind; int nin, nout; std::string expr; std::vector<float> caps;
-  float interval = 0.0f; uint64_t hash = 0;   // EnvelopeIn only
+  float interval = 0.0f; uint64_t hash = 0;   // the envelopes only
   ClosureN(ClosureKind k, int i, int o, std::string e, std::vector<float> c) : kind(k), nin(i), nout(o), expr(std::move(e)), caps(std::move(c)) {}
+  bool envelope() const { return kind == CL_ENVELOPE_IN || kind == CL_ENVELOPE; }
   int inputs() const override { return nin; } int outputs() const override { return nout; }
-  uint64_t id() const override { return kind == CL_MAP ? 5 : (kind == CL_SHAPE_FN ? 42 : 53); }
-  void set(const Setting& s) override { if (kind == CL_ENVELOPE_IN && s.kind == P_INTERVAL) interval = s.v[0]; }   // src/envelope.rs:344-348; map and shape_fn have no parameter
-  void set_hash(uint64_t h) override { if (kind == CL_ENVELOPE_IN) hash = h; }                                       // envelope.rs:350-353
+  uint64_t id() const override { return kind == CL_MAP ? 5 : (kind == CL_SHAPE_FN ? 42 : (kind == CL_ENVELOPE ? 14 : 53)); }
+  void set(const Setting& s) override { if (envelope() && s.kind == P_INTERVAL) interval = s.v[0]; }   // src/envelope.rs:165-170, :344-348; map and shape_fn have no parameter
+  void set_hash(uint64_t h) override { if (envelope()) hash = h; }                                     // envelope.rs:172-175, :350-353
   void sig(std::string& o) const override {
     const std::string nc = I((int)caps.size());
     if (kind == CL_MAP) o += "Map<" + I(nin) + "," + I(nout) + "," + nc + "," + expr + ">";
     else if (kind == CL_SHAPE_FN) o += "ShaperFn<" + nc + "," + expr + ">";
+    else if (kind == CL_ENVELOPE) o += "EnvelopeFn<" + I(nout) + "," + nc + "," + expr + ">";
     else o += "EnvelopeInFn<" + I(nin) + "," + I(nout) + "," + nc + "," + expr + ">";
   }
   void lower(Lowering& l) const override {
     for (float c : caps) l.p(c);
-    if (kind != CL_ENVELOPE_IN) return;
+    if (!envelope()) return;
     l.p(interval);
-    l.s(0.0f); l.s(0.0f); l.s(0.0f);                      // t, t_0, t_1 (EnvelopeIn::reset)
+    l.s(0.0f); l.s(0.0f); l.s(0.0f);                      // t, t_0, t_1 (reset; the device evaluates E(0) at the first segment)
     l.su((uint32_t)hash); l.su((uint32_t)(hash >> 32));   // t_hash
     for (int k = 0; k < nout; k++) { l.s(0.0f); l.s(0.0f); l.s(0.0f); l.s(0.0f); }   // value_0, value_1, value, value_d
     l.su(0u); l.su(0u); l.su(0u);                         // run, run_len, seg_end
@@ -1445,11 +1449,11 @@ HNode* mk_panner() { return new Panner(0.0f, 2); }
 HNode* mk_adsr_live(float a, float d, float s, float r) { return new AdsrLive(a, d, s, r); }
 static HNode* mk_closure_of(SharedCell* cell, int kind, int inputs, int outputs, double interval, const char* text, int ncaptures,
                             const char* const* names, const float* values, std::string& err) {
-  const char* what = kind == CL_MAP ? "map" : (kind == CL_SHAPE_FN ? "shape_fn" : (kind == CL_VAR_FN ? "var_fn" : "envelope_in"));
+  const char* what = kind == CL_MAP ? "map" : (kind == CL_SHAPE_FN ? "shape_fn" : (kind == CL_VAR_FN ? "var_fn" : (kind == CL_ENVELOPE ? "envelope" : "envelope_in")));
   auto bad = [&](const std::string& w) -> HNode* { err = std::string(what) + ": " + w; return nullptr; };
-  if (kind < CL_MAP || kind > CL_VAR_FN || (kind == CL_VAR_FN) != (cell != nullptr)) { err = "closure: bad kind"; return nullptr; }
-  if (inputs < 0 || inputs > 8 || outputs < 1 || outputs > 8) return bad("arity mismatch: 0-8 inputs and 1-8 outputs");
-  if (kind == CL_ENVELOPE_IN && !(interval > 0.0)) return bad("the interval must be positive");   // EnvelopeIn::new asserts it (src/envelope.rs:230)
+  if (kind < CL_MAP || kind > CL_ENVELOPE || (kind == CL_VAR_FN) != (cell != nullptr)) { err = "closure: bad kind"; return nullptr; }
+  if (inputs < 0 || inputs > 8 || outputs < 1 || outputs > 8 || (kind == CL_ENVELOPE && inputs != 0)) return bad("arity mismatch: 0-8 inputs and 1-8 outputs");
+  if ((kind == CL_ENVELOPE_IN || kind == CL_ENVELOPE) && !(interval > 0.0)) return bad("the interval must be positive");   // Envelope::new / EnvelopeIn::new assert it (src/envelope.rs:59, :230)
   if (ncaptures < 0 || (ncaptures > 0 && (!names || !values))) return bad("bad capture arrays");
   Closure c;
   const std::string e = parse_closure(text, (ClosureKind)kind, inputs, outputs, c);
@@ -1470,7 +1474,7 @@ static HNode* mk_closure_of(SharedCell* cell, int kind, int inputs, int outputs,
   }
   if (kind == CL_VAR_FN) return new VarFnN(cell, outputs, c.expr, std::move(v));
   ClosureN* n = new ClosureN((ClosureKind)kind, kind == CL_SHAPE_FN ? 1 : inputs, kind == CL_SHAPE_FN ? 1 : outputs, c.expr, std::move(v));
-  n->interval = (float)interval;   // EnvelopeIn<f32>: F::from_f32 / the f32 interval of prelude32 (src/prelude32.rs:716-724)
+  n->interval = (float)interval;   // Envelope<f32> / EnvelopeIn<f32>: F::from_f32 / the f32 interval of prelude32 (src/prelude32.rs:581-724)
   return n;
 }
 HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char* text, int ncaptures, const char* const* names, const float* values,

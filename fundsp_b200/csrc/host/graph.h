@@ -217,7 +217,8 @@ HNode* mk_feedback2(HNode* x, HNode* y, int hadamard);
 HNode* mk_pan(float value);
 HNode* mk_panner();
 HNode* mk_adsr_live(float a, float d, float s, float r);
-// closures of the signal, parsed from text (closure.h): kind 0 Map ID 5, 1 Shaper<ShapeFn> ID 42, 2 EnvelopeIn<f32> ID 53 (`interval` seconds);
+// closures of the signal or of time, parsed from text (closure.h): kind 0 Map ID 5, 1 Shaper<ShapeFn> ID 42, 2 EnvelopeIn<f32> ID 53, 4 Envelope<f32>
+// ID 14 (`interval` seconds for both envelopes; no horizon: the device evaluates the closure at every sample point);
 // captures are (name, value) pairs. On failure returns null with the reason in `err` (arity mismatches start with "<what>: arity mismatch").
 HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char* text, int ncaptures, const char* const* names, const float* values,
                   std::string& err);

@@ -2,9 +2,9 @@
 
 Every function returns an `An` expression and cites the reference constructor it mirrors
 (file:line relative to the reference crate (SamiPerttu/fundsp v0.23.0)).  Names, argument order and argument meaning follow the
-reference; `pass` is spelled `pass_` (Python keyword).  Anything that needs a Rust closure
-(`envelope(|t| ..)`, `map`, `shape_fn`) cannot cross a C ABI and is intentionally absent;
-`adsr_live` is a closed-form opcode (src/adsr.rs:21-70).
+reference; `pass` is spelled `pass_` (Python keyword).  A Rust closure cannot cross a C ABI, so the closure nodes (`map_`, `shape_fn`,
+`envelope_in`, and `envelope` / `lfo` given text) take the closure as text in a subset of Rust closure syntax, compiled for the GPU;
+`envelope` / `lfo` also take a Python callable, sampled on the host. `adsr_live` is a closed-form opcode (src/adsr.rs:21-70).
 """
 from __future__ import annotations
 
@@ -536,18 +536,29 @@ def mixer(matrix):
 
 
 # ---- src/prelude.rs:580-612 envelope / lfo: control signals from a closure of time, sampled every ~2 ms and interpolated.
-# `f(t)` returns a float or a tuple (one value per output); `outputs` defaults to what f(0.0) returns. The closure runs on the HOST when
-# the graph is lowered, at the sample points the reference would use, up to `horizon` seconds (then the last value holds).
-# time64=True is `F = f64` (prelude64 / hacker); the default is the f32 time of hacker32.
-def envelope(f, outputs=None, horizon=10.0, time64=False, interval=0.002):
+# Given TEXT, `f` is a closure `|t| ...` in the closure language below, with its captured values as keyword arguments:
+#   lfo("|t| 1000.0 + 500.0 * sin_hz(rate, t)", rate=0.5)
+# It is compiled into the voice program and evaluated on the GPU at the reference's sample points, so it has no horizon and keeps no table;
+# `outputs` (default 1) must match the arity of its value, and `horizon` does not apply. The closure computes in f32 (F = f32).
+# Given a Python callable, `f(t)` returns a float or a tuple (one value per output); `outputs` defaults to what f(0.0) returns. The callable
+# runs on the HOST when the graph is lowered, at the same sample points, up to `horizon` seconds (then the last value holds).
+# time64=True is `F = f64` (prelude64 / hacker), for callables only; the default is the f32 time of hacker32.
+def envelope(f, outputs=None, horizon=10.0, time64=False, interval=0.002, **captures):
+    if isinstance(f, str):
+        if time64:
+            raise NotImplementedError("envelope: a text closure computes in f32; an F = f64 envelope takes a Python callable")
+        nout = 1 if outputs is None else int(outputs)
+        return _closure("envelope_text", (f32(interval), f, nout, _captures(captures)), 0, nout)
+    if captures:
+        raise TypeError("envelope: captured values are for a text closure; a Python callable captures its own")
     if outputs is None:
         v = f(0.0)
         outputs = len(v) if isinstance(v, (tuple, list)) else 1
     return An("envelope", (float(interval) if time64 else f32(interval), int(outputs), 1 if time64 else 0, f, float(horizon)), (), 0, int(outputs))
 
 
-def lfo(f, outputs=None, horizon=10.0, time64=False):
-    return envelope(f, outputs, horizon, time64)
+def lfo(f, outputs=None, horizon=10.0, time64=False, **captures):
+    return envelope(f, outputs, horizon, time64, **captures)
 
 
 # ---- closures of the signal, run per sample on the GPU (prelude32: src/prelude32.rs:625-740, 1126-1183). The closure is text in a
@@ -602,14 +613,31 @@ def lfo3(closure, outputs=1, **captures):
     return envelope_in(closure, 2, outputs, **captures)
 
 
-# ---- src/prelude.rs:2719-2753 flanger / phaser: the delay (phase) closure is a closure of time, so it lowers like `lfo`
-def flanger(feedback_amount, minimum_delay, maximum_delay, delay_f, horizon=10.0):
-    return pass_() & feedback2((pass_() | lfo(lambda t: f32(delay_f(t)), 1, horizon)) >> tap(minimum_delay, maximum_delay), shape(Tanh(feedback_amount)))
+# ---- src/prelude.rs:2719-2753 flanger / phaser: the delay (phase) closure is a closure of time, so it lowers like `lfo`: given text
+# `|t| ...` (captures as keyword arguments) it runs on the GPU without a horizon, given a Python callable it is sampled on the host.
+def flanger(feedback_amount, minimum_delay, maximum_delay, delay_f, horizon=10.0, **captures):
+    f = delay_f if isinstance(delay_f, str) else (lambda t: f32(delay_f(t)))
+    return pass_() & feedback2((pass_() | lfo(f, 1, horizon, **captures)) >> tap(minimum_delay, maximum_delay), shape(Tanh(feedback_amount)))
 
 
-def phaser(feedback_amount, phase_f, horizon=10.0):
-    c01 = lambda x: min(1.0, max(0.0, f32(x)))
-    return pass_() & feedback((pass_() | lfo(lambda t: lerp(2.0, 20.0, c01(phase_f(t))), 1, horizon))
+def _phaser_text(phase_f):
+    """`move |t| lerp(2.0, 20.0, clamp01(phase_f(t)))` for a text `phase_f`: its body, in a block, becomes clamp01's argument."""
+    s = phase_f.strip()
+    if s.startswith("move") and s[4:5] in " \t\n|":
+        s = s[4:].lstrip()
+    if s.startswith("||") or not s.startswith("|") or "|" not in s[1:]:
+        return phase_f   # not of the form |t| ..: the closure parser reports it
+    end = s.index("|", 1)
+    return s[:end + 1] + " lerp(2.0, 20.0, clamp01({ " + s[end + 1:] + "\n}))"
+
+
+def phaser(feedback_amount, phase_f, horizon=10.0, **captures):
+    if isinstance(phase_f, str):
+        f = _phaser_text(phase_f)
+    else:
+        c01 = lambda x: min(1.0, max(0.0, f32(x)))
+        f = lambda t: lerp(2.0, 20.0, c01(phase_f(t)))
+    return pass_() & feedback((pass_() | lfo(f, 1, horizon, **captures))
                               >> pipei(10, lambda i: add((0.0, 0.1)) >> ~allpole()) >> (mul(feedback_amount) | sink()))
 
 

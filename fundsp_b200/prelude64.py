@@ -139,10 +139,14 @@ def brown():
 
 # ---- src/prelude64.rs:581-612: Envelope<f64, E, R>
 def envelope(f, outputs=None, horizon=10.0, interval=0.002):
+    if isinstance(f, str):   # the closure language computes in f32, and Envelope<f64> computes its closure in f64
+        raise NotImplementedError("prelude64.envelope: a text closure computes in f32; an F = f64 envelope takes a Python callable")
     return _p32.envelope(f, outputs, horizon, True, interval)
 
 
 def lfo(f, outputs=None, horizon=10.0):
+    if isinstance(f, str):
+        raise NotImplementedError("prelude64.lfo: a text closure computes in f32; an F = f64 envelope takes a Python callable")
     return _p32.envelope(f, outputs, horizon, True)
 
 

@@ -159,10 +159,14 @@ fdsp_node* fdsp_adsr_live(float attack, float decay, float sustain, float releas
    class. Map has 0-8 inputs and 1-8 outputs; a tuple value is a multi-output closure. On failure these return NULL with the reason and
    its column in fdsp_last_error(): reasons that begin "<node>: arity mismatch" are arity errors (the reference rejects them at compile
    time); every other refusal (syntax, an unsupported function, a capture that does not occur in the text, an identifier without a
-   value) is an argument error. No closure has a settable parameter; fdsp_envelope_in takes Setting::interval. */
+   value) is an argument error. Only the envelopes have a settable parameter: fdsp_envelope_in and fdsp_envelope_text take Setting::interval. */
 fdsp_node* fdsp_map(int inputs, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values);        /* Map ID 5 src/audionode.rs:1328 (`map`): |x| with x[0..inputs) */
 fdsp_node* fdsp_shape_fn(const char* closure, int ncaptures, const char* const* names, const float* values);                          /* Shaper<ShapeFn> ID 42 src/shape.rs:33 (`shape_fn`): |x| with a scalar x */
 fdsp_node* fdsp_envelope_in(double interval, int inputs, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values); /* EnvelopeIn<f32> ID 53 src/envelope.rs:185 (`envelope_in`, `envelope2`, `envelope3`, `lfo_*`; interval 0.002): |t, i| with a frame i[0..inputs), or |t, x1, .., xN| with one scalar per input */
+/* Envelope<f32, E, R> ID 14 src/envelope.rs:14 (`envelope`, `lfo`; interval 0.002) with the closure E as TEXT |t| of time alone, 1-8
+   outputs: the device evaluates it at the reference's jittered sample points (the same points as fdsp_envelope's callback), so it has no
+   horizon and stores no table of values. The closure computes in f32; for F = f64 time use fdsp_envelope's callback. */
+fdsp_node* fdsp_envelope_text(double interval, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values);
 /* combinators (src/combinator.rs:289-488; src/audionode.rs) */
 fdsp_node* fdsp_pipe(fdsp_node* x, fdsp_node* y);              /* x >> y  Pipe   ID 6  */
 fdsp_node* fdsp_stack(fdsp_node* x, fdsp_node* y);             /* x | y   Stack  ID 7  */

@@ -292,10 +292,20 @@ inline An limiter_stereo(float attack_time, float release_time) { return An(fdsp
 // the closure runs on the host when the graph is lowered, at the reference's sample points, up to `horizon` seconds
 inline An envelope(fdsp_envelope_fn f, int outputs = 1, void* user = nullptr, double horizon = 10.0, bool time64 = false) { return An(fdsp_envelope(0.002, outputs, time64 ? 1 : 0, f, user, horizon)); }
 inline An lfo(fdsp_envelope_fn f, int outputs = 1, void* user = nullptr, double horizon = 10.0, bool time64 = false) { return envelope(f, outputs, user, horizon, time64); }
+// envelope("|t| ...") / lfo("|t| ...") with the closure as text (F = f32): the GPU evaluates it at the same sample points, with no horizon,
+// e.g. lfo("|t| 1000.0 + 500.0 * sin_hz(rate, t)", 1, {{"rate", 0.5f}})
+inline An envelope(const char* closure, int outputs = 1, Captures captures = {}) {
+  detail::CaptureArrays c(captures);
+  return detail::closure_node(fdsp_envelope_text(0.002, outputs, closure, (int)c.names.size(), c.names.data(), c.values.data()));
+}
+inline An lfo(const char* closure, int outputs = 1, Captures captures = {}) { return envelope(closure, outputs, captures); }
 // flanger / phaser (src/prelude.rs:2719-2753): the delay (phase) closure is a closure of time and lowers like `lfo`. phaser's closure
 // returns the allpole delay itself here: lerp(2, 20, clamp01(phase_f(t))) of the reference is the caller's to apply.
 inline An flanger(float feedback_amount, float minimum_delay, float maximum_delay, fdsp_envelope_fn delay_f, void* user = nullptr, double horizon = 10.0) {
   return pass() & feedback2((pass() | lfo(delay_f, 1, user, horizon)) >> tap(minimum_delay, maximum_delay), shape(Tanh{feedback_amount}));
+}
+inline An flanger(float feedback_amount, float minimum_delay, float maximum_delay, const char* delay_f, Captures captures = {}) {
+  return pass() & feedback2((pass() | lfo(delay_f, 1, captures)) >> tap(minimum_delay, maximum_delay), shape(Tanh{feedback_amount}));
 }
 enum class Fade { Power = 0, Smooth = 1 };                                                 // src/sequencer.rs:35-52
 inline An slot(An unit) { return An(fdsp_slot(unit.release())); }                             // Slot::new: replaceable with a crossfade (Bank::slot_set)

@@ -59,6 +59,7 @@ extern "C" {
     fn fdsp_map(inputs: c_int, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_shape_fn(closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_envelope_in(interval: f64, inputs: c_int, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
+    fn fdsp_envelope_text(interval: f64, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_convolve(response: *const f32, n: c_int) -> *mut FdspNode;
     fn fdsp_shaper(kind: c_int, p0: f32, p1: f32) -> *mut FdspNode;
     fn fdsp_shaper_adaptive(timescale: f64, inner_kind: c_int, p0: f32, p1: f32) -> *mut FdspNode;
@@ -394,8 +395,8 @@ pub struct AdsrLive { pub attack: f32, pub decay: f32, pub sustain: f32, pub rel
 impl Lower for AdsrLive { unsafe fn lower(&self) -> *mut FdspNode { fdsp_adsr_live(self.attack, self.decay, self.sustain, self.release) } }
 
 /// A closure of the signal that can also run on the GPU: the reference's node `X` (what runs on the CPU) plus the closure's text and
-/// captured values, which `Lower` hands to `fdsp_map` / `fdsp_shape_fn` / `fdsp_envelope_in`. Made by `gpu_map!`, `gpu_shape_fn!` and
-/// `gpu_envelope_in!`, which take the closure ONCE: it is compiled by rustc for the CPU node and `stringify!`-ed for the GPU node, so
+/// captured values, which `Lower` hands to `fdsp_map` / `fdsp_shape_fn` / `fdsp_envelope_in` / `fdsp_envelope_text`. Made by `gpu_map!`,
+/// `gpu_shape_fn!`, `gpu_envelope_in!`, `gpu_envelope!` and `gpu_lfo!`, which take the closure ONCE: it is compiled by rustc for the CPU node and `stringify!`-ed for the GPU node, so
 /// the two cannot drift apart. The text must stay inside the closure language of DESIGN.md §2 (f32 literals, the listed functions);
 /// `fdsp_*` refuses anything else with the token and its column, and `GpuBank::new` returns that error.
 #[derive(Clone)]
@@ -422,6 +423,7 @@ impl<X: AudioNode> Lower for GpuClosure<X> {
         match self.kind {
             0 => fdsp_map(i, o, t, nc, ptrs.as_ptr(), self.values.as_ptr()),
             1 => fdsp_shape_fn(t, nc, ptrs.as_ptr(), self.values.as_ptr()),
+            4 => fdsp_envelope_text(self.interval, o, t, nc, ptrs.as_ptr(), self.values.as_ptr()),
             _ => fdsp_envelope_in(self.interval, i, o, t, nc, ptrs.as_ptr(), self.values.as_ptr()),
         }
     }
@@ -469,6 +471,23 @@ macro_rules! gpu_envelope_in {
             kind: 2, interval: 0.002f32 as f64, text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
         })
     };
+}
+/// `gpu_envelope!([rate], |t: f32| 1000.0 + 500.0 * sin_hz(rate, t))`: `envelope(..)` (prelude32.rs:581, Envelope<f32> ID 14, interval
+/// 2 ms) that lowers to `fdsp_envelope_text`: the GPU evaluates the closure at every sample point, with no horizon. The output count is
+/// the closure's return type.
+#[macro_export]
+macro_rules! gpu_envelope {
+    ([$($c:ident),*], $($f:tt)+) => {
+        $crate::combinator::An($crate::gpu::GpuClosure {
+            node: $crate::envelope::Envelope::<f32, _, _>::new(0.002, $($f)+),
+            kind: 4, interval: 0.002f32 as f64, text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
+        })
+    };
+}
+/// `gpu_lfo!(..)`: `lfo(..)` is `envelope(..)` (prelude32.rs:604).
+#[macro_export]
+macro_rules! gpu_lfo {
+    ($($t:tt)+) => { $crate::gpu_envelope!($($t)+) };
 }
 
 /// V voices of typed graphs evaluated in lockstep on one GPU; to the host ONE `AudioUnit` (audiounit.rs:21-95).

@@ -70,6 +70,10 @@ def jobs():
     add(sg(envelope2("|t, x| x * x * a + t", a=1.0)), (1,))
     for g in (saw_hz(50.0) >> map_("|x| tanh(x[0] * drive)", 1, 1, drive=1.0), saw_hz(50.0) >> shape(Tanh(1.0))):
         add(sg(g), (1, 2, 3))
+    # text envelopes (tests/test_gpu_envelope_text.py: rows, rows + mix)
+    import test_gpu_envelope_text as ET
+    for mk in ET.CASES.values():
+        add(sg(mk(0)), (1, 2, 3))
     # the Atan and Adaptive waveshapes (tests/test_gpu_shapes.py: rows, rows + mix, the resident process() kernel of its ragged cases;
     # tools/bench_shapes.py: mix)
     import test_gpu_shapes as SH
