@@ -74,6 +74,11 @@ FDSP_DEV float clamp11f(float x) { return fminf(fmaxf(x, -1.0f), 1.0f); }       
 FDSP_DEV float wide_roundf(float x) { return rintf(x); }
 FDSP_DEV float wide_floorf(float x) { return rintf(x - 0.4999999f); }
 
+// f32 -> i32 with the semantics of x86's cvttss2si / cvttps2dq, which `wide` and the host run: truncation toward zero in range, and
+// INT32_MIN (0x80000000) for NaN and for |y| >= 2^31. A plain (int) cast is undefined there; PTX's cvt.rzi.s32.f32 saturates to
+// 0x7fffffff and gives 0 for NaN.
+FDSP_DEV int32_t cvtt_i32(float y) { return (y >= -2147483648.0f && y < 2147483648.0f) ? (int32_t)y : (int32_t)0x80000000u; }
+
 // `wide` f32x8::sin as called by the block path of Sine (src/oscillator.rs:82): Cephes/VCL sincos, lane-wise.
 FDSP_DEV float wide_sinf(float v) {
   const float DP1F = 0.78515625f * 2.0f;
@@ -84,7 +89,7 @@ FDSP_DEV float wide_sinf(float v) {
   const float TWO_OVER_PI = 2.0f / 3.14159274101257324f;
   float xa = fabsf(v);
   float y = rintf(xa * TWO_OVER_PI);
-  int q = (int)y;
+  int q = cvtt_i32(y);
   float x = ((xa - y * DP1F) - y * DP2F) - y * DP3F;
   float x2 = x * x;
   float x4 = x2 * x2;

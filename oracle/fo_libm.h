@@ -7,7 +7,8 @@
 //   expm1f, tanhf  : s_expm1f.c / s_tanhf.c
 // PARITY UNPINNED at the ulp level against the real crate (no Rust toolchain here); tests pin these against
 // glibc to <= 1 ulp over dense sweeps (tests/test_oracle.py::test_restated_libm_*), which would expose any
-// mis-remembered constant. |x| >= 2^28*pi/2 falls back to the platform libm (never reached by audio graphs).
+// mis-remembered constant. |x| >= 2^28*pi/2 takes rem_pio2f's large path (k_rem_pio2.c, Payne-Hanek), restated below: no f32 path
+// calls the platform's sin/cos/tan.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -59,6 +60,107 @@ inline int rem_pio2f_medium(float x, double* y) {
   *y = x64 - fn * PIO2_1 - fn * PIO2_1T;
   return (int)(int32_t)fn;
 }
+// k_rem_pio2.c __rem_pio2_large(x, y, e0, nx, prec) for prec 0 (one double out), as rem_pio2f.c calls it with nx = 1.
+static const int32_t IPIO2[] = {   // 2/pi in 24-bit digits
+  0xA2F983, 0x6E4E44, 0x1529FC, 0x2757D1, 0xF534DD, 0xC0DB62, 0x95993C, 0x439041, 0xFE5163, 0xABDEBB, 0xC561B7, 0x246E3A,
+  0x424DD2, 0xE00649, 0x2EEA09, 0xD1921C, 0xFE1DEB, 0x1CB129, 0xA73EE8, 0x8235F5, 0x2EBB44, 0x84E99C, 0x7026B4, 0x5F7E41,
+  0x3991D6, 0x398353, 0x39F49C, 0x845F8B, 0xBDF928, 0x3B1FF8, 0x97FFDE, 0x05980F};
+static const double PIO2_PIECES[] = {1.57079625129699707031e+00, 7.54978941586159635335e-08, 5.39030252995776476554e-15,
+                                     3.28200341580791294123e-22, 1.27065575308067607349e-29, 1.22933308981111328932e-36,
+                                     2.73370053816464559624e-44, 2.16741683877804819444e-51};
+inline double scalbn_exact(double x, int n) {   // x * 2^n for the small |n| used here (never leaves the normal range)
+  uint64_t u = (uint64_t)(0x3ff + n) << 52; double p; memcpy(&p, &u, 8); return x * p;
+}
+inline int rem_pio2_large(const double* x, double* y, int e0, int nx) {
+  const int jk = 3, jp = jk;   // init_jk[prec = 0]
+  int32_t jz, jx, jv, carry, n, iq[20], i, j, k, m, q0, ih;
+  double z, fw, f[20], fq[20], q[20];
+  jx = nx - 1;
+  jv = (e0 - 3) / 24; if (jv < 0) jv = 0;
+  q0 = e0 - 24 * (jv + 1);
+  j = jv - jx; m = jx + jk;
+  for (i = 0; i <= m; i++, j++) f[i] = j < 0 ? 0.0 : (double)IPIO2[j];
+  for (i = 0; i <= jk; i++) { for (j = 0, fw = 0.0; j <= jx; j++) fw += x[j] * f[jx + i - j]; q[i] = fw; }
+  jz = jk;
+recompute:
+  for (i = 0, j = jz, z = q[jz]; j > 0; i++, j--) {
+    fw = (double)(int32_t)(0x1p-24 * z);
+    iq[i] = (int32_t)(z - 0x1p24 * fw);
+    z = q[j - 1] + fw;
+  }
+  z = scalbn_exact(z, q0);
+  z -= 8.0 * std::floor(z * 0.125);
+  n = (int32_t)z;
+  z -= (double)n;
+  ih = 0;
+  if (q0 > 0) {
+    i = iq[jz - 1] >> (24 - q0); n += i;
+    iq[jz - 1] -= i << (24 - q0);
+    ih = iq[jz - 1] >> (23 - q0);
+  } else if (q0 == 0) ih = iq[jz - 1] >> 23;
+  else if (z >= 0.5) ih = 2;
+  if (ih > 0) {
+    n += 1; carry = 0;
+    for (i = 0; i < jz; i++) {
+      j = iq[i];
+      if (carry == 0) {
+        if (j != 0) { carry = 1; iq[i] = 0x1000000 - j; }
+      } else iq[i] = 0xffffff - j;
+    }
+    if (q0 > 0) {
+      switch (q0) { case 1: iq[jz - 1] &= 0x7fffff; break; case 2: iq[jz - 1] &= 0x3fffff; break; }
+    }
+    if (ih == 2) { z = 1.0 - z; if (carry != 0) z -= scalbn_exact(1.0, q0); }
+  }
+  if (z == 0) {
+    j = 0;
+    for (i = jz - 1; i >= jk; i--) j |= iq[i];
+    if (j == 0) {
+      for (k = 1; iq[jk - k] == 0; k++) {}
+      for (i = jz + 1; i <= jz + k; i++) {
+        f[jx + i] = (double)IPIO2[jv + i];
+        for (j = 0, fw = 0.0; j <= jx; j++) fw += x[j] * f[jx + i - j];
+        q[i] = fw;
+      }
+      jz += k;
+      goto recompute;
+    }
+  }
+  if (z == 0.0) {
+    jz -= 1; q0 -= 24;
+    while (iq[jz] == 0) { jz--; q0 -= 24; }
+  } else {
+    z = scalbn_exact(z, -q0);
+    if (z >= 0x1p24) {
+      fw = (double)(int32_t)(0x1p-24 * z);
+      iq[jz] = (int32_t)(z - 0x1p24 * fw);
+      jz += 1; q0 += 24;
+      iq[jz] = (int32_t)fw;
+    } else iq[jz] = (int32_t)z;
+  }
+  fw = scalbn_exact(1.0, q0);
+  for (i = jz; i >= 0; i--) { q[i] = fw * (double)iq[i]; fw *= 0x1p-24; }
+  for (i = jz; i >= 0; i--) {
+    for (fw = 0.0, k = 0; k <= jp && k <= jz - i; k++) fw += PIO2_PIECES[k] * q[i + k];
+    fq[jz - i] = fw;
+  }
+  fw = 0.0;
+  for (i = jz; i >= 0; i--) fw += fq[i];
+  y[0] = ih == 0 ? fw : -fw;
+  return n & 7;
+}
+// rem_pio2f.c: the medium path below 2^28 * pi/2, else x scaled into [2^23, 2^24) and handed to rem_pio2_large (x finite)
+inline int rem_pio2f_(float x, double* y) {
+  const uint32_t hx = fbits(x), ix = hx & 0x7fffffffu;
+  if (ix < 0x4dc90fdbu) return rem_pio2f_medium(x, y);
+  const int32_t e0 = (int32_t)(ix >> 23) - (0x7f + 23);
+  double tx[1], ty[1];
+  tx[0] = (double)fromb(ix - ((uint32_t)e0 << 23));
+  const int n = rem_pio2_large(tx, ty, e0, 1);
+  if (hx >> 31) { *y = -ty[0]; return -n; }
+  *y = ty[0];
+  return n;
+}
 const double S1PIO2 = 1.0 * 1.57079632679489661923, S2PIO2 = 2.0 * 1.57079632679489661923, S3PIO2 = 3.0 * 1.57079632679489661923,
              S4PIO2 = 4.0 * 1.57079632679489661923;
 
@@ -74,8 +176,7 @@ inline float sinf_(float x) {  // sinf.c
     return k_sindf(sign ? (double)x + S4PIO2 : (double)x - S4PIO2);
   }
   if (ix >= 0x7f800000u) return x - x;
-  if (ix >= 0x4dc90fdbu) return ::sinf(x);
-  double y; int n = rem_pio2f_medium(x, &y);
+  double y; int n = rem_pio2f_(x, &y);
   switch (n & 3) { case 0: return k_sindf(y); case 1: return k_cosdf(y); case 2: return k_sindf(-y); default: return -k_cosdf(y); }
 }
 inline float cosf_(float x) {  // cosf.c
@@ -90,8 +191,7 @@ inline float cosf_(float x) {  // cosf.c
     return sign ? k_sindf(-(double)x - S3PIO2) : k_sindf((double)x - S3PIO2);
   }
   if (ix >= 0x7f800000u) return x - x;
-  if (ix >= 0x4dc90fdbu) return ::cosf(x);
-  double y; int n = rem_pio2f_medium(x, &y);
+  double y; int n = rem_pio2f_(x, &y);
   switch (n & 3) { case 0: return k_cosdf(y); case 1: return k_sindf(-y); case 2: return -k_cosdf(y); default: return k_sindf(y); }
 }
 inline float tanf_(float x) {  // tanf.c
@@ -106,8 +206,7 @@ inline float tanf_(float x) {  // tanf.c
     return k_tandf(sign ? (double)x + S4PIO2 : (double)x - S4PIO2, 0);
   }
   if (ix >= 0x7f800000u) return x - x;
-  if (ix >= 0x4dc90fdbu) return ::tanf(x);
-  double y; int n = rem_pio2f_medium(x, &y);
+  double y; int n = rem_pio2f_(x, &y);
   return k_tandf(y, n & 1);
 }
 

@@ -9,7 +9,7 @@
 // are pinned bit-for-bit by the golden vectors in tests/golden/. Transcendentals are NOT pinned at
 // the ulp level: the reference calls the Rust `libm 0.2.15` crate (musl port) for scalars and
 // `wide 1.1.1` for the f32x8 block path; neither source is in the reference crate and no Rust
-// toolchain exists here. Scalars use glibc (<= 1 ulp from musl's, both are < 1 ulp functions);
+// toolchain exists here. Scalars are musl's algorithms restated in fo_libm.h (no platform libm on an f32 trig path);
 // `wide::f32x8::sin` is restated from its published algorithm (Agner Fog VCL sincos, Cephes
 // coefficients) below. "parity unpinned" at ulp level for sin/tan/tanh/exp and wavetable entries.
 #pragma once
@@ -106,7 +106,8 @@ inline float wide_sinf(float v) {
   const float TWO_OVER_PI = 2.0f / 3.14159274101257324f;
   float xa = fabsf(v);
   float y = wide_roundf(xa * TWO_OVER_PI);
-  int32_t q = (int32_t)y;
+  // cvttps2dq: truncation in range, 0x80000000 for NaN and |y| >= 2^31 (finite |v| >~ 3.4e9); a plain cast would be undefined there
+  int32_t q = (y >= -2147483648.0f && y < 2147483648.0f) ? (int32_t)y : INT32_MIN;
   float x = ((xa - y * DP1F) - y * DP2F) - y * DP3F;
   float x2 = x * x;
   float x4 = x2 * x2;

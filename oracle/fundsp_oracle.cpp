@@ -7,6 +7,7 @@
 //   fir3     src/prelude.rs:863-867      reverb_stereo src/prelude.rs:1732-1762
 //   moog_q   src/prelude.rs:559-561      Wave::render src/wave.rs:441-466, Wave::filter :518-565
 #include "fo_nodes.h"
+#include "fo_shapes.h"   // atanf_ and wide_atanf, for fo_libm_eval
 #include <thread>
 
 using namespace fo;
@@ -80,7 +81,8 @@ API Node* fo_pan(float value) { return new Panner(value, 1); }
 API Node* fo_panner() { return new Panner(0.0f, 2); }
 API Node* fo_adsr_live(float a, float d, float s, float r) { return new AdsrLive(a, d, s, r); }
 API Node* fo_phase_osc(int kind) { return new PhaseOsc(kind); }   // 0 ramp, 1 poly_saw, 2 poly_square, 3 poly_pulse
-// restated libm entry points, for the accuracy tests (fn: 0 sinf 1 cosf 2 tanf 3 tanhf 4 expm1f 5 expf 6 powf(x, y))
+// restated libm entry points, for the accuracy and sweep tests
+// (fn: 0 sinf 1 cosf 2 tanf 3 tanhf 4 expm1f 5 expf 6 powf(x, y) 7 atanf 8 wide_sinf 9 wide_atanf)
 API void fo_libm_eval(int fn, const float* x, const float* y, float* out, int64_t n) {
   for (int64_t i = 0; i < n; i++) {
     switch (fn) {
@@ -90,6 +92,9 @@ API void fo_libm_eval(int fn, const float* x, const float* y, float* out, int64_
       case 3: out[i] = m::tanhf_(x[i]); break;
       case 4: out[i] = m::expm1f_(x[i]); break;
       case 5: out[i] = m::expf_(x[i]); break;
+      case 7: out[i] = m::atanf_(x[i]); break;
+      case 8: out[i] = wide_sinf(x[i]); break;
+      case 9: out[i] = wide_atanf(x[i]); break;
       default: out[i] = m::powf_(x[i], y[i]); break;
     }
   }
