@@ -17,12 +17,8 @@ namespace host {
 
 namespace {
 constexpr uint32_t TIME_CHUNK = 16384;  // samples per launch (multiple of 64): bounds the partial-mix buffer
-// sub-chunk of two-stage (dry program -> FDN reverb) classes: stage 1 of chunk k+1 overlaps stage 2 of chunk k (FDSP_PIPE_CHUNK: tuning)
-static uint32_t pipe_chunk() {
-  static const uint32_t v = [] { const char* e = getenv("FDSP_PIPE_CHUNK"); uint32_t x = e ? (uint32_t)atoi(e) : 2048u; x = x / 64u * 64u; return x < 256u ? 256u : (x > TIME_CHUNK ? TIME_CHUNK : x); }();
-  return v;
-}
-#define PIPE_CHUNK pipe_chunk()
+// sub-chunk of two-stage (dry program -> FDN reverb) classes: stage 1 of chunk k+1 overlaps stage 2 of chunk k
+constexpr uint32_t PIPE_CHUNK = 2048;
 
 // the runtime's own calls (which return "" or the message) inside a function of the same convention
 #define TRY(call) do { std::string e_ = (call); if (!e_.empty()) return e_; } while (0)
@@ -38,20 +34,54 @@ template <class C> C* locate(std::vector<C>& classes, uint32_t voice, uint32_t* 
 }  // namespace
 static_assert(!std::is_copy_constructible<VoiceClass>::value, "a copy of a class would free its buffers twice");
 
-// `Pipe<X, Convolver>` with a response long enough for 128-wide tiles goes to the tensor-core form (FDSP_TC_CONV=0: direct form only;
-// FDSP_TC_MINK: shortest response, default 32 taps). One output channel, and not on the CPU mock device.
-static bool tc_conv_wanted(const std::string& sig, const Lowering& l, int nout) {
-#ifdef FDSP_HOST_EMUL
-  (void)sig; (void)l; (void)nout; return false;
-#else
-  static const std::string CT = ",Convolver>";
-  const char* e = getenv("FDSP_TC_CONV"); const char* m = getenv("FDSP_TC_MINK");
-  if (e && atoi(e) == 0) return false;
-  const uint32_t mink = m ? (uint32_t)atoi(m) : 32u;
-  return nout == 1 && sig.compare(0, 5, "Pipe<") == 0 && sig.size() > 5 + CT.size() && sig.compare(sig.size() - CT.size(), CT.size(), CT) == 0 && l.conv_K >= mink &&
-         l.conv_off + 2u + l.conv_K == l.U.size();
-#endif
+// `sig` is `Pipe<X,tail>`: *front = X
+static bool pipe_into(const std::string& sig, const std::string& tail, std::string* front) {
+  const std::string t = "," + tail + ">";
+  if (sig.size() <= 5 + t.size() || sig.compare(0, 5, "Pipe<") != 0 || sig.compare(sig.size() - t.size(), t.size(), t) != 0) return false;
+  *front = sig.substr(5, sig.size() - 5 - t.size());
+  return true;
 }
+
+// The form of class c (see Form), from the lowering `l` of one of its voices, and the signature of its program (empty: an FDN class
+// without a dry stage). `wet`: the FDN tail adds the reverb to the dry signal on a stereo bus.
+static Form choose_form(const VoiceClass& c, const Lowering& l, int nin, int nout, bool one_class, std::string* prog, bool* wet) {
+  static const std::string REV = "Pipe<Pipe<MultiSplit<2,16>,Feedback<1,Multi<30,0,32,Pipe<Delay,Fir<3>>>>>,Binop<2,Multi<31,0,32,Panner<1>>,Constant<2>>>";
+  static const std::string BUS = "Bus<MultiPass<2>,Unop<3," + REV + ">>";   // dry + g * reverb on a stereo bus
+  *prog = c.sig; *wet = false;
+  if (!getenv("FDSP_DISABLE_FDN")) {   // A/B switch: run reverbs in the generic thread-per-voice form
+    std::string front;
+    bool fdn = true;
+    if ((c.sig == REV || c.sig == BUS) && nin == 2) *wet = c.sig == BUS;
+    else if (pipe_into(c.sig, BUS, &front)) *wet = true;
+    else if (!pipe_into(c.sig, REV, &front)) fdn = false;
+    // the kernel's prefetch distance needs every delay >= 192 samples
+    for (size_t k = c.nu - 32; fdn && k < c.nu; k++) fdn = c.uniform[k] >= FDN_MIN_RING;
+    if (fdn) { *prog = front; return Form::fdn; }
+    *wet = false;
+  }
+#ifndef FDSP_HOST_EMUL   // (not on the CPU mock device)
+  // `X >> convolve(h)` with a response long enough for 128-wide tiles goes to tensor cores (FDSP_TC_CONV=0: direct form only; FDSP_TC_MINK:
+  // shortest response, default 32 taps). One output channel, and one class: its mix-down is the voice-order fold of its own rows.
+  const char* e = getenv("FDSP_TC_CONV"); const char* m = getenv("FDSP_TC_MINK");
+  std::string front;
+  if (one_class && nout == 1 && !(e && atoi(e) == 0) && pipe_into(c.sig, "Convolver", &front) && l.conv_K >= (m ? (uint32_t)atoi(m) : 32u) &&
+      l.conv_off + 2u + l.conv_K == c.nu) {
+    *prog = front;
+    return Form::conv;
+  }
+#endif
+  return Form::plain;
+}
+
+// Per form: the words of a class's lowering that its tail holds rather than its program (FDN: the reverb's, plus the gain of a wet bus;
+// conv: the Convolver's state word, its ring index, and two uniform words, which stay in the class's layout unused like its history
+// ring), the program's output channels (0: the bank's), and the wording of the errors about the program.
+struct FormRule { uint32_t tail_p, tail_s, tail_u; int out; const char *name, *name_end, *layout, *layout_end; };
+static const FormRule FORM_RULES[] = {
+    /* plain */ {0, 0, 0, 0, "graph class `", "`", "host lowering of `", "` disagrees with the device word layout"},
+    /* fdn */ {162, 160, 32, 2, "the dry stage `", "`", "dry-stage layout of `", "` disagrees with the host lowering"},
+    /* conv */ {0, 1, 2, 1, "`", "` (in front of the convolver)", "layout of `", "` in front of the convolver disagrees with the host lowering"},
+};
 
 namespace {
 std::mutex g_rt_mu;          // registry of the bank that owns each device's resident process() kernel (see rt_stop)
@@ -87,6 +117,16 @@ std::string Bank::init(std::vector<HNode*>& voices, int dev, uint32_t mode) {
   return lower_and_upload(true);
 }
 
+// the FDN rings and the convolver's history columns (with the rows behind them)
+std::string VoiceClass::clear_history(cudaStream_t st) {
+  if (ring_floats) CU(cudaMemsetAsync(d_ring, 0, (size_t)ring_floats * V() * sizeof(float), st));
+  if (form == Form::conv) {
+    CU(cudaMemsetAsync(d_cx, 0, (size_t)V() * conv_stride * sizeof(float), st));
+    CU(cudaMemsetAsync(d_cxl, 0, (size_t)V() * conv_stride * sizeof(float), st));
+  }
+  return "";
+}
+
 std::string Bank::lower_and_upload(bool upload_state) {
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
@@ -115,77 +155,46 @@ std::string Bank::lower_and_upload(bool upload_state) {
       ci = (int)fresh.size(); index[lo.key] = ci;
       VoiceClass c; c.sig = lo.sig; c.uniform = lo.l.U;
       c.np = (uint32_t)lo.l.P.size(); c.ns = (uint32_t)lo.l.S.size(); c.nu = (uint32_t)lo.l.U.size();
-      const uint32_t nu_static = c.nu - lo.l.extraU;   // what the device templates count (NU); the rest is variable-length uniform data
-      std::string jerr, prog_sig = lo.sig;
-      // reverb_stereo tail -> warp-per-voice FDN kernel; the part in front of it (if any) stays a fused per-voice program
-      static const std::string REV = "Pipe<Pipe<MultiSplit<2,16>,Feedback<1,Multi<30,0,32,Pipe<Delay,Fir<3>>>>>,Binop<2,Multi<31,0,32,Panner<1>>,Constant<2>>>";
-      const std::string wet_tail = ",Bus<MultiPass<2>,Unop<3," + REV + ">>>", pipe_tail = "," + REV + ">";
-      auto ends_with = [](const std::string& s, const std::string& t) { return s.size() >= t.size() && s.compare(s.size() - t.size(), t.size(), t) == 0; };
-      bool wet = false;
-      const bool fdn_off = getenv("FDSP_DISABLE_FDN") != nullptr;  // A/B switch: run reverbs in the generic thread-per-voice form
-      if (fdn_off) {}
-      else if (lo.sig == REV && nin == 2) { c.fdn = true; prog_sig.clear(); }
-      else if (lo.sig == "Bus<MultiPass<2>,Unop<3," + REV + ">>" && nin == 2) { c.fdn = true; wet = true; prog_sig.clear(); }   // dry + g * reverb on a stereo bus
-      else if (lo.sig.compare(0, 5, "Pipe<") == 0 && ends_with(lo.sig, wet_tail)) { c.fdn = true; wet = true; prog_sig = lo.sig.substr(5, lo.sig.size() - 5 - wet_tail.size()); }
-      else if (lo.sig.compare(0, 5, "Pipe<") == 0 && ends_with(lo.sig, pipe_tail)) { c.fdn = true; prog_sig = lo.sig.substr(5, lo.sig.size() - 5 - pipe_tail.size()); }
-      if (c.fdn) {
-        for (size_t k = lo.l.U.size() - 32; k < lo.l.U.size(); k++) if (lo.l.U[k] < FDN_MIN_RING) c.fdn = false;  // the kernel's prefetch distance needs every delay >= 192 samples
-        if (!c.fdn) prog_sig = lo.sig;
-      }
-      if (c.fdn) {
-        c.p0 = c.np - 162; c.s0 = c.ns - 160; c.u0 = c.nu - 32;
-        c.scalar_row = wet ? (int)c.p0 - 1 : -1;
-        for (size_t k = 0; k < lo.l.dlen.size(); k++) { if (k + 32 >= lo.l.dlen.size()) c.ring_floats += fdn_ring_phys(lo.l.dlen[k]); else c.dl_floats += lo.l.dlen[k]; }
-        if (!prog_sig.empty()) {
-          c.k = get_program(prog_sig, device, jerr);
-          if (!c.k) return "#U no device program for the dry stage `" + prog_sig + "`: " + jerr;
-          if ((uint32_t)c.k->NP != c.p0 - (wet ? 1u : 0u) - lo.l.extraP || (uint32_t)c.k->NS != c.s0 || (uint32_t)c.k->NU != c.u0 - lo.l.extraU || c.k->IN != nin || c.k->OUT != 2)
-            return "internal: dry-stage layout of `" + prog_sig + "` disagrees with the host lowering";
-        }
-      } else if (tc_conv_wanted(lo.sig, lo.l, nout)) {
-        // `X >> convolve(h)`: X stays a fused per-voice program that writes its rows, the tap contraction runs on tensor cores. The
-        // Convolver's own words (ring index, history ring) stay in the layout and are simply not used by this form.
-        static const std::string CT = ",Convolver>";
-        const std::string xsig = lo.sig.substr(5, lo.sig.size() - 5 - CT.size());
-        for (uint32_t d : lo.l.dlen) c.dl_floats += d;
-        c.k = get_program(xsig, device, jerr);
-        if (!c.k) return "#U no device program for `" + xsig + "` (in front of the convolver): " + jerr;
-        if ((uint32_t)c.k->NP != c.np - lo.l.extraP || (uint32_t)c.k->NS + 1u != c.ns || (uint32_t)c.k->NU + 2u != nu_static || c.k->IN != nin || c.k->OUT != 1)
-          return "internal: layout of `" + xsig + "` in front of the convolver disagrees with the host lowering";
-        c.conv = true; c.conv_K = lo.l.conv_K; c.conv_off = lo.l.conv_off;
-        c.conv_H = (c.conv_K - 1u + 31u) / 32u * 32u; if (c.conv_H == 0) c.conv_H = 32;
-        c.conv_J = conv_tc_toeplitz_cols(c.conv_K); c.conv_stride = c.conv_H + TIME_CHUNK;
-      } else {
-        for (uint32_t d : lo.l.dlen) c.dl_floats += d;
-        c.k = get_program(lo.sig, device, jerr);
-        if (!c.k) return "#U no device program for graph class `" + lo.sig + "`: " + jerr;
-        if ((uint32_t)c.k->NP != c.np - lo.l.extraP || (uint32_t)c.k->NS != c.ns || (uint32_t)c.k->NU != nu_static || c.k->IN != nin || c.k->OUT != nout)
-          return "internal: host lowering of `" + lo.sig + "` disagrees with the device word layout";
-      }
-      {   // reset exemptions of this graph class, in the class's own word / delay-line coordinates
-        for (auto& r : lo.l.keepS) if (r.second > r.first) c.keep_s.emplace_back(r.first, r.second);
-        std::vector<uint64_t> doff(lo.l.dlen.size() + 1, 0);
-        const size_t nd_lines = c.fdn ? lo.l.dlen.size() - 32 : lo.l.dlen.size();   // the last 32 lines of an FDN class live in its rings
-        for (size_t k = 0; k < lo.l.dlen.size(); k++) doff[k + 1] = doff[k] + (k < nd_lines ? lo.l.dlen[k] : 0u);
-        for (auto& r : lo.l.keepD) if (r.second > r.first && r.second <= nd_lines) c.keep_d.emplace_back(doff[r.first], doff[r.second]);
-        std::sort(c.keep_s.begin(), c.keep_s.end()); std::sort(c.keep_d.begin(), c.keep_d.end());
-      }
       fresh.push_back(std::move(c));
     } else ci = it->second;
     fresh[ci].voices.push_back((uint32_t)v);
     std::string().swap(lo.key); std::vector<uint32_t>().swap(lo.l.U);   // the class keeps the uniform words (a sampler voice's may be a whole wave)
   }
+  // then the form of each class, its program and the layout that program must have (the class's first voice gives its layout)
+  for (auto& c : fresh) {
+    const Lowering& l = lows[c.voices[0]].l;
+    std::string prog; bool wet = false;
+    c.form = choose_form(c, l, nin, nout, fresh.size() == 1, &prog, &wet);
+    const size_t nd_lines = c.form == Form::fdn ? l.dlen.size() - 32 : l.dlen.size();   // the last 32 lines of an FDN class live in its rings
+    for (size_t k = 0; k < l.dlen.size(); k++) { if (k < nd_lines) c.dl_floats += l.dlen[k]; else c.ring_floats += fdn_ring_phys(l.dlen[k]); }
+    if (c.form == Form::fdn) {
+      c.p0 = c.np - 162; c.s0 = c.ns - 160; c.u0 = c.nu - 32;
+      c.scalar_row = wet ? (int)c.p0 - 1 : -1;
+    } else if (c.form == Form::conv) {
+      c.conv_K = l.conv_K; c.conv_off = l.conv_off;
+      c.conv_H = (c.conv_K - 1u + 31u) / 32u * 32u; if (c.conv_H == 0) c.conv_H = 32;
+      c.conv_J = conv_tc_toeplitz_cols(c.conv_K); c.conv_stride = c.conv_H + TIME_CHUNK;
+    }
+    if (!prog.empty()) {
+      const FormRule& r = FORM_RULES[(int)c.form];
+      std::string jerr;
+      c.k = get_program(prog, device, jerr);
+      if (!c.k) return std::string("#U no device program for ") + r.name + prog + r.name_end + ": " + jerr;
+      // extraP / extraU: variable-length data behind the words the device templates count
+      if ((uint32_t)c.k->NP != c.np - l.extraP - r.tail_p - (wet ? 1u : 0u) || (uint32_t)c.k->NS != c.ns - r.tail_s ||
+          (uint32_t)c.k->NU != c.nu - l.extraU - r.tail_u || c.k->IN != nin || c.k->OUT != (r.out ? r.out : nout))
+        return std::string("internal: ") + r.layout + prog + r.layout_end;
+    }
+    // reset exemptions of this graph class, in the class's own word / delay-line coordinates
+    for (auto& q : l.keepS) if (q.second > q.first) c.keep_s.emplace_back(q.first, q.second);
+    std::vector<uint64_t> doff(l.dlen.size() + 1, 0);
+    for (size_t k = 0; k < l.dlen.size(); k++) doff[k + 1] = doff[k] + (k < nd_lines ? l.dlen[k] : 0u);
+    for (auto& q : l.keepD) if (q.second > q.first && q.second <= nd_lines) c.keep_d.emplace_back(doff[q.first], doff[q.second]);
+    std::sort(c.keep_s.begin(), c.keep_s.end()); std::sort(c.keep_d.begin(), c.keep_d.end());
+  }
   sh_uses.assign(nodes.size(), {});
   for (size_t v = 0; v < nodes.size(); v++) sh_uses[v] = lows[v].l.shared;
   TRY(sh_check(0, sh_uses[0]));
-  if (fresh.size() > 1) {   // the tensor-core convolver form is for one-class banks (its mix-down is the voice-order fold of its own rows)
-    for (auto& c : fresh) if (c.conv) {
-      std::string jerr;
-      c.conv = false;
-      c.k = get_program(c.sig, device, jerr);
-      if (!c.k) return "#U no device program for graph class `" + c.sig + "`: " + jerr;
-    }
-  }
   // 2. keep device buffers of classes that survive unchanged (same key order / sizes), else rebuild
   const bool same_shape = classes.size() == fresh.size() && std::equal(classes.begin(), classes.end(), fresh.begin(), [](const VoiceClass& a, const VoiceClass& b) {
                             return a.sig == b.sig && a.voices == b.voices && a.uniform == b.uniform; });
@@ -211,25 +220,23 @@ std::string Bank::lower_and_upload(bool upload_state) {
       TRY(c.d_uniform.grow(c.uniform.size()));
       TRY(c.d_rowmap.grow(rows.size()));
       TRY(c.d_dline.grow((size_t)c.dl_floats * V));
-      if (c.fdn) {
-        TRY(c.d_ring.grow((size_t)c.ring_floats * V));
-        if (c.k) {
-          TRY(c.d_dry.grow((size_t)V * 2 * TIME_CHUNK));
-          TRY(c.d_dry2.grow((size_t)V * 2 * PIPE_CHUNK));
-          for (int q = 0; q < 2; q++) { CU(cudaEventCreateWithFlags(c.e_dry[q].put(), cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(c.e_fdn[q].put(), cudaEventDisableTiming)); }
-        }
+      if (c.form == Form::fdn) TRY(c.d_ring.grow((size_t)c.ring_floats * V));
+      if (c.fdn_with_dry()) {
+        TRY(c.d_dry.grow((size_t)V * 2 * TIME_CHUNK));
+        TRY(c.d_dry2.grow((size_t)V * 2 * PIPE_CHUNK));
+        for (int q = 0; q < 2; q++) { CU(cudaEventCreateWithFlags(c.e_dry[q].put(), cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(c.e_fdn[q].put(), cudaEventDisableTiming)); }
       }
-      if (c.conv) {
+      if (c.form == Form::conv) {
         TRY(c.d_cx.grow((size_t)V * c.conv_stride));
         TRY(c.d_cxl.grow((size_t)V * c.conv_stride));
         TRY(c.d_th.grow((size_t)128 * c.conv_J));
         TRY(c.d_tl.grow((size_t)128 * c.conv_J));
         CU(conv_tc_make_maps(c.d_cx, c.d_cxl, V, c.conv_stride, c.d_th, c.d_tl, c.conv_J, &c.conv_maps));
       }
-      if ((c.fdn && c.k) || c.conv) {   // the rows the dry stage writes (two per voice) or the convolver reads (one per voice)
+      if (c.fdn_with_dry() || c.form == Form::conv) {   // the rows the dry stage writes (two per voice) or the convolver reads (one per voice)
         TRY(c.d_dryrows.grow(V));
         std::vector<uint32_t> id(V);
-        for (uint32_t i = 0; i < V; i++) id[i] = c.conv ? i : 2 * i;
+        for (uint32_t i = 0; i < V; i++) id[i] = c.form == Form::conv ? i : 2 * i;
         CU(cudaMemcpy(c.d_dryrows, id.data(), V * 4, cudaMemcpyHostToDevice));
       }
       CU(cudaMemcpy(c.d_rowmap, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice));
@@ -239,9 +246,8 @@ std::string Bank::lower_and_upload(bool upload_state) {
     if (upload_state) {
       if (!S.empty()) CU(cudaMemcpy(c.d_state, S.data(), S.size() * 4, cudaMemcpyHostToDevice));
       if (c.dl_floats) CU(cudaMemset(c.d_dline, 0, (size_t)c.dl_floats * V * sizeof(float)));
-      if (c.ring_floats) CU(cudaMemset(c.d_ring, 0, (size_t)c.ring_floats * V * sizeof(float)));
-      if (c.conv) {
-        CU(cudaMemset(c.d_cx, 0, (size_t)V * c.conv_stride * sizeof(float))); CU(cudaMemset(c.d_cxl, 0, (size_t)V * c.conv_stride * sizeof(float)));
+      TRY(c.clear_history(0));   // (on the default stream, like the cudaMemset above)
+      if (c.form == Form::conv) {
         CU(launch_conv_toeplitz(reinterpret_cast<const float*>(c.d_uniform + c.conv_off + 2), c.conv_K, c.d_th, c.d_tl, c.conv_J, stream));
         CU(cudaStreamSynchronize(stream));
       }
@@ -349,7 +355,7 @@ std::string Bank::upload_voice(uint32_t voice, const Lowering& l, bool with_stat
     const uint32_t Vc = c.V();
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns || (reset_state && reset_state->size() != c.ns))
       return "#U the voice does not fit its class: a class-uniform word (delay length, table, wave) or the word layout differs; rebuild the bank instead";
-    if (with_state && c.fdn) return "#U voices of a two-stage (FDN reverb) class cannot be replaced in place";
+    if (with_state && c.form == Form::fdn) return "#U voices of a two-stage (FDN reverb) class cannot be replaced in place";
     TRY(sh_check(voice, l.shared));
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
     const std::vector<uint32_t> S0 = reset_state ? *reset_state : l.reset_image();
@@ -431,7 +437,7 @@ std::string Bank::regroup(HNode* node, int at, uint32_t* voice, const Carry* car
   if (!n) return std::string("#A ") + what + ": null node";
   if (n->inputs() != nin || n->outputs() != nout) return std::string("#U ") + what + ": the unit's arity differs from the bank's";
   if (tree_mix && at < 0) return "#U add: a bank extracted from a Net mixes in the Net's order; rebuild it from the edited Net";
-  for (auto& c : classes) if (c.fdn || c.conv) return std::string("#U ") + what + ": banks with a two-stage class (FDN reverb, tensor-core convolver) cannot be regrouped in place; rebuild the bank";
+  for (auto& c : classes) if (c.form != Form::plain) return std::string("#U ") + what + ": banks with a two-stage class (FDN reverb, tensor-core convolver) cannot be regrouped in place; rebuild the bank";
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
   Lowering l0, l;
@@ -567,7 +573,7 @@ std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode
   if (VoiceClass* cp = locate(classes, voice, &i)) {
     VoiceClass& c = *cp;
     const uint32_t Vc = c.V();
-    if (c.fdn || c.ns < 4 || ((c.ns - 4) & 1u) || (c.dl_floats & 1u)) return "slot: unexpected class layout";
+    if (c.form == Form::fdn || c.ns < 4 || ((c.ns - 4) & 1u) || (c.dl_floats & 1u)) return "slot: unexpected class layout";
     CU(cudaStreamSynchronize(stream));
     uint32_t head[2] = {0, 0};   // which, has_next of this voice
     CU(cudaMemcpy2D(head, 4, c.d_state + i, (size_t)Vc * 4, 4, 2, cudaMemcpyDeviceToHost));
@@ -697,7 +703,7 @@ std::string Bank::push_event(HNode* node, uint32_t* voice) {   // Sequencer::pus
   std::string want; n->sig(want);
   if (!l.ok) return "#U " + l.why;
   for (auto& c : classes) {
-    if (c.sig != want || c.uniform != l.U || c.fdn) continue;
+    if (c.sig != want || c.uniform != l.U || c.form == Form::fdn) continue;
     for (uint32_t v : c.voices) {
       if (!event_times(nodes[v].get(), &s0, &e0)) break;
       if (!(e0 <= seq_time + 0.5 * sd)) continue;   // Event::plan's end-of-event test at the start of the next block: still sounding
@@ -730,8 +736,7 @@ std::string Bank::reset() {  // AudioUnit::reset: back to the construction-time 
     { uint64_t at = 0;
       auto span = [&](uint64_t a, uint64_t b) -> cudaError_t { return b > a ? cudaMemsetAsync(c.d_dline + a * Vc, 0, (size_t)(b - a) * Vc * sizeof(float), stream) : cudaSuccess; };
       if (c.dl_floats) { for (auto& k : c.keep_d) { CU(span(at, k.first)); at = std::max(at, k.second); } CU(span(at, c.dl_floats)); } }
-    if (c.ring_floats) CU(cudaMemsetAsync(c.d_ring, 0, (size_t)c.ring_floats * c.V() * sizeof(float), stream));
-    if (c.conv) { CU(cudaMemsetAsync(c.d_cx, 0, (size_t)c.V() * c.conv_stride * sizeof(float), stream)); CU(cudaMemsetAsync(c.d_cxl, 0, (size_t)c.V() * c.conv_stride * sizeof(float), stream)); }
+    TRY(c.clear_history(stream));
   }
   CU(cudaStreamSynchronize(stream));
   dirty = false; seq_time = 0.0;
@@ -743,8 +748,7 @@ std::string Bank::reset() {  // AudioUnit::reset: back to the construction-time 
 // (process()-sized) read the tables through L1/L2 instead
 static size_t table_bytes_of(const VoiceClass& c, uint32_t len) {
   const int wk = c.k ? c.k->wave_kind : -1;
-  static const uint32_t tb_min = [] { const char* e = getenv("FDSP_TB_MIN"); return e ? (uint32_t)atoi(e) : 32u; }();  // at 64 samples the TMA-staged tables already win
-  return (wk >= 0 && len >= tb_min) ? device_wavetable(wk).data.size() * sizeof(float) : 0;
+  return (wk >= 0 && len >= 32u) ? device_wavetable(wk).data.size() * sizeof(float) : 0;   // at 64 samples the TMA-staged tables already win
 }
 // SMs of a device (the CTA shapes below are sized by it)
 static uint32_t sm_count(int device) {
@@ -756,13 +760,11 @@ static uint32_t sm_count(int device) {
 // Stage-pipelined kernels (dsp/bank_kernel_st.cuh): programs with a heavy serial leaf (Moog ...) run their stages in different warps.
 // Used for launches long enough to fill the pipeline and for classes too small to give every warp scheduler a voice-warp of its own
 // (V <= SMs x 32: with a warp per scheduler already, stages only add hand-off work).
-// FDSP_STAGED=0 switches them off (A/B), FDSP_STAGED_MAXV moves the class-size bound.
+// FDSP_STAGED=0 switches them off (A/B).
 static bool use_staged(const Program* k, uint32_t V, uint32_t len, uint32_t sms) {
   const char* e = getenv("FDSP_STAGED");            // read per call: the tests toggle it inside one process
-  const char* m = getenv("FDSP_STAGED_MAXV");
   const int on = e ? atoi(e) : 1;
-  const uint32_t maxv = m ? (uint32_t)atoi(m) : sms * 32u;
-  return on != 0 && k && k->stages >= 2 && len >= 256u && V <= maxv;
+  return on != 0 && k && k->stages >= 2 && len >= 256u && V <= sms * 32u;
 }
 // CTAs (the rows of its partial mix), voices per CTA and kernel form of class c's voice program in a launch of len samples. Stage-pipelined:
 // 32 voices per CTA while that still leaves SMs free, else 128 spread evenly (FDSP_STAGED_W=128 forces the wide shape: lets the tests reach
@@ -778,7 +780,7 @@ static ClassGrid class_grid(const VoiceClass& c, uint32_t len, int device) {
   g.staged = use_staged(c.k.get(), V, len, nsm);
   if (g.staged && V <= nsm * 32u && !(w && atoi(w) == 128)) { g.vpc = 32u; g.ctas = (V + 31u) / 32u; }
   else if (g.staged) g.ctas = bank_grid(V, 128u, nsm, &g.vpc);
-  else if (c.fdn || getenv("FDSP_NO_SPREAD")) g.ctas = (V + g.vpc - 1) / g.vpc;
+  else if (c.form == Form::fdn) g.ctas = (V + g.vpc - 1) / g.vpc;
   else g.ctas = bank_grid(V, g.vpc, nsm, &g.vpc);
   return g;
 }
@@ -813,7 +815,7 @@ std::string Bank::rt_process(uint32_t size, const float* in, float* out, bool* s
   if (has_parked()) { process_streak = 0; return ""; }   // parked Slot / crossfade updates are armed between launches (render_device)
   if (classes.size() != 1 || !(out_mode & 2u) || tree_mix || nout > 8 || nin > 8) return "";
   VoiceClass& c = classes[0];
-  if (c.fdn || c.conv || !c.k || !c.k->has_rt) return "";
+  if (c.form != Form::plain || !c.k || !c.k->has_rt) return "";
   if (!sh_cells.empty()) return "";   // Shared controls are exchanged between calls, on the launch path (sh_pull / sh_push)
   uint32_t vpc = (uint32_t)c.k->threads;
   const uint32_t grid = bank_grid(c.V(), (uint32_t)c.k->threads, sm_count(device), &vpc);
@@ -904,6 +906,136 @@ std::string Bank::voice_args(VoiceClass& c, uint32_t len, uint32_t vpc, BankArgs
   return "";
 }
 
+// One chunk of a render_device_run call, as its classes see it
+struct Bank::Chunk {
+  uint64_t t0, index; uint32_t len;
+  bool want_v, want_m;                        // rows and partial mix wanted of the classes (a tree mix takes their rows and mixes them itself)
+  float* out; uint32_t out_stride, out_t0;    // the rows: the caller's, or the tree mix's own from column 0
+  float* mix; uint32_t mix_stride;
+  bool pipelined;                             // two-stage classes run as a two-stream software pipeline
+};
+struct Bank::Pending { VoiceClass* c; Chunk w; int buf; };   // a partial-mix reduction of a pipelined class, issued one chunk late
+
+static cudaError_t launch_program(const VoiceClass& c, const BankArgs& a, int mode, const ClassGrid& g, cudaStream_t st) {   // over a.n samples
+  return g.staged ? c.k->launch_staged(a, mode, table_bytes_of(c, a.n), st) : c.k->launch(a, mode, table_bytes_of(c, a.n), st);
+}
+
+// the `grid` rows of a class's CTA-partial mix summed into the chunk's mix, or added to it (nothing when no mix is wanted)
+std::string Bank::reduce_mix(const float* partial, uint32_t grid, const Chunk& w, bool accumulate, cudaStream_t st) {
+  if (!w.want_m) return "";
+  CU(launch_mix_reduce(partial, grid, (uint32_t)nout, w.len, w.mix, w.mix_stride, (uint32_t)w.t0, accumulate ? 1 : 0, st));
+  launches++;
+  return "";
+}
+
+// the deferred reductions (all, or those of class `only`), on `stream` behind the FDN kernel each one reads
+std::string Bank::flush_pending(std::vector<Pending>& pending, const VoiceClass* only) {
+  for (size_t q = 0; q < pending.size();) {
+    Pending& pd = pending[q];
+    if (only && pd.c != only) { q++; continue; }
+    CU(cudaStreamWaitEvent(stream, pd.c->e_fdn[pd.buf], 0));
+    TRY(reduce_mix(pd.buf ? pd.c->d_partial2 : pd.c->d_partial, pd.c->V(), pd.w, true, stream));
+    pending.erase(pending.begin() + (long)q);
+  }
+  return "";
+}
+
+// stage 1 of a two-stage class, on `stream`: its program writes each voice's rows (d_dryrows) into `rows`, `stride` apart, from column `offset`
+std::string Bank::launch_dry(VoiceClass& c, BankArgs d, const ClassGrid& g, float* rows, uint32_t stride, uint32_t offset) {
+  d.out = rows; d.partial = nullptr; d.out_stride = stride; d.out_offset = offset; d.row_map = c.d_dryrows;
+  CU(launch_program(c, d, 1, g, stream));
+  launches++;
+  return "";
+}
+
+// A plain class: its program, which finishes the mix-down itself in process()-sized launches (one launch instead of two), else the reduction
+// of its partial mix. Concurrent classes run on their own streams; the caller reduces them once all are launched.
+std::string Bank::run_plain(VoiceClass& c, const Chunk& w, const ClassGrid& g, BankArgs& a, bool first, bool concurrent) {
+  const cudaStream_t ks = concurrent ? c.cstream : stream;
+  const bool fused_mix = w.want_m && w.len <= 64;
+  if (fused_mix) a.ticket = d_ticket;
+  TRY(dom_mark(ks));
+  CU(launch_program(c, a, (w.want_v ? 1 : 0) | (w.want_m ? 2 : 0), g, ks));
+  TRY(dom_mark(ks));
+  launches++;
+  if (concurrent) CU(cudaEventRecord(c.e_done, ks));
+  else if (!fused_mix) TRY(reduce_mix(c.d_partial, g.ctas, w, !first, stream));
+  return "";
+}
+
+// An FDN class: the warp-per-voice reverb kernel on the rows of its dry stage, or on the bank's stereo input. Behind a dry stage in a
+// pipelined call, stage 1 of chunk k runs on `stream` and stage 2 on `stream2`, the buffers alternate, and chunk k-1's partial mix is
+// reduced after stage 1 of chunk k has been queued, so that the two stages of neighbouring chunks run side by side.
+std::string Bank::run_fdn(VoiceClass& c, const Chunk& w, const ClassGrid& g, const BankArgs& a, bool first, std::vector<Pending>& pending) {
+  const uint32_t V = c.V();
+  if (w.len > TIME_CHUNK) return "internal: chunk";
+  const bool pipe = w.pipelined && c.k;
+  // voices (= warps) per CTA. Pipelined: leave SMs free for the CTAs of the dry stage of the next chunk (their shared-memory tables cannot
+  // share an SM with an FDN CTA), otherwise the two stages serialise on SM residency
+  const int cap = fdn_max_warps();
+  const uint32_t nsm = sm_count(device);
+  uint32_t sms = nsm;
+  if (pipe) sms = g.ctas < nsm / 2 ? nsm - g.ctas : nsm / 2;
+  int warps = (int)((V + sms - 1) / sms); if (warps > cap) warps = cap; if (warps < 1) warps = 1;
+  FdnArgs f;
+  f.params = c.d_params; f.state = c.d_state; f.uniform = c.d_uniform; f.p0 = c.p0; f.s0 = c.s0; f.u0 = c.u0; f.scalar_row = c.scalar_row;
+  f.out = w.want_v ? w.out : nullptr; f.row_map = c.d_rowmap; f.out_stride = w.out_stride; f.out_offset = w.out_t0;
+  f.partial = a.partial;
+  f.ring = c.d_ring; f.ring_voice_stride = c.ring_floats; f.V = V; f.n = w.len;
+  const int buf = (int)(w.index & 1);
+  const bool solo = classes.size() == 1;
+  cudaStream_t fs = stream;   // the FDN kernel's stream
+  if (pipe) {
+    float* dry = buf ? c.d_dry2 : c.d_dry;
+    if (w.want_m && c.d_partial2.size() < (size_t)V * nout * w.len) TRY(c.d_partial2.grow((size_t)V * nout * PIPE_CHUNK));
+    CU(cudaStreamWaitEvent(stream, c.e_fdn[buf], 0));   // FDN of chunk k-2 has consumed this dry buffer (no-op before the first record)
+    TRY(launch_dry(c, a, g, dry, PIPE_CHUNK, 0));
+    CU(cudaEventRecord(c.e_dry[buf], stream));
+    // A bank of this one class keeps `stream` for the dry stage alone — chunk k + 1 follows chunk k with nothing in between, so it
+    // holds its SMs before the wide FDN kernel of chunk k floods the rest — and reduces on stream2 behind the FDN kernel. With other
+    // classes in the bank every reduction stays on `stream` (they accumulate into the same mix region), one chunk late.
+    if (!solo) TRY(flush_pending(pending, &c));   // reduce chunk k-1 of this class (waits for its FDN)
+    f.dry = dry; f.dry_voice_stride = 2ull * PIPE_CHUNK; f.dry_ch_stride = PIPE_CHUNK; f.dry_offset = 0;
+    if (w.want_m && buf) f.partial = c.d_partial2;
+    CU(cudaStreamWaitEvent(stream2, c.e_dry[buf], 0));
+    fs = stream2;
+  } else if (c.k) {  // stage 1: the fused dry program writes stereo rows [V][2][TIME_CHUNK]
+    TRY(launch_dry(c, a, g, c.d_dry, TIME_CHUNK, 0));
+    f.dry = c.d_dry; f.dry_voice_stride = 2ull * TIME_CHUNK; f.dry_ch_stride = TIME_CHUNK; f.dry_offset = 0;
+  } else {    // reverb applied straight to the bank's stereo input
+    f.dry = a.in; f.dry_voice_stride = 0; f.dry_ch_stride = a.in_stride; f.dry_offset = a.in_offset;
+  }
+  TRY(dom_mark(fs));
+  CU(launch_fdn(f, warps, fs));
+  TRY(dom_mark(fs));
+  launches++;
+  if (!pipe) return reduce_mix(c.d_partial, V, w, !first, stream);
+  CU(cudaEventRecord(c.e_fdn[buf], stream2));
+  if (!solo) pending.push_back({&c, w, buf});
+  else TRY(reduce_mix(buf ? c.d_partial2 : c.d_partial, V, w, true, stream2));
+  return "";
+}
+
+// A convolver class, on `stream`: the program in front of the convolver writes its rows behind the history columns; then x_lo, the
+// Toeplitz GEMM tiles (rows straight into the caller's buffer, or an internal one), the history shift, and the voice-order fold of the rows
+std::string Bank::run_conv(VoiceClass& c, const Chunk& w, const ClassGrid& g, const BankArgs& a) {
+  const uint32_t V = c.V();
+  TRY(launch_dry(c, a, g, c.d_cx, c.conv_stride, c.conv_H));
+  CU(launch_conv_split(c.d_cx, c.d_cxl, V, c.conv_stride, c.conv_H, w.len, stream));
+  float* y = w.want_v ? w.out : nullptr; uint32_t ys = w.out_stride, yo = w.out_t0;
+  if (!y) {
+    TRY(c.d_crows.grow((size_t)V * TIME_CHUNK));
+    y = c.d_crows; ys = TIME_CHUNK; yo = 0;
+  }
+  TRY(dom_mark(stream));
+  CU(launch_conv_tc(c.conv_maps, y, ys, yo, c.d_dryrows, V, w.len, c.conv_K, c.conv_H, stream));
+  TRY(dom_mark(stream));
+  CU(launch_conv_history(c.d_cx, c.d_cxl, V, c.conv_stride, c.conv_H, w.len, stream));
+  launches += 3;
+  if (w.want_m) { CU(launch_tree_mix(y, V, 1u, ys, yo, w.len, w.mix, w.mix_stride, (uint32_t)w.t0, 0, stream)); launches++; }
+  return "";
+}
+
 std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in_stride, float* out_dev, uint64_t out_stride, float* mix_dev,
                                     uint64_t mix_stride) {
   CU(cudaSetDevice(device));
@@ -913,7 +1045,6 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
   const bool want_v = (out_mode & 1u) && out_dev, want_m = (out_mode & 2u) && mix_dev;
   if (!want_v && !want_m) return "#A no output buffer matches the bank's out_mode";
   if (n == 0) return "";
-  const bool save_want_m_ = want_m;
   if (in_stride > 0xffffffffull || out_stride > 0xffffffffull || mix_stride > 0xffffffffull) return "#A stride too large";
   if (timing) { CU(cudaEventRecord(ev0, stream)); dom_n = 0; }
   // Net-ordered mix: the voice kernels materialise per-voice rows (user buffer, or an internal one) and tree_mix_kernel adds
@@ -921,211 +1052,75 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
   const bool tree = tree_mix != 0 && want_m;
   // two-stage classes (fused dry program + warp-per-voice FDN) run as a two-stream software pipeline over PIPE_CHUNK samples
   bool pipelined = false;
-  if (!tree && !getenv("FDSP_NO_PIPELINE")) for (auto& c : classes) pipelined = pipelined || (c.fdn && c.k);
+  if (!tree && !getenv("FDSP_NO_PIPELINE")) for (auto& c : classes) pipelined = pipelined || c.fdn_with_dry();
   const uint32_t CH = tree ? 4096u : (pipelined ? PIPE_CHUNK : TIME_CHUNK);
-  struct Pending { VoiceClass* c; uint32_t grid, len; uint64_t t0; int buf; };
   std::vector<Pending> pending;   // deferred CTA-partial reductions of pipelined classes (issued one chunk late, on `stream`)
-  auto flush_pending = [&](VoiceClass* only) -> std::string {
-    for (size_t q = 0; q < pending.size();) {
-      Pending& pd = pending[q];
-      if (only && pd.c != only) { q++; continue; }
-      CU(cudaStreamWaitEvent(stream, pd.c->e_fdn[pd.buf], 0));
-      if (save_want_m_) { CU(launch_mix_reduce(pd.buf ? pd.c->d_partial2 : pd.c->d_partial, pd.grid, (uint32_t)nout, pd.len, mix_dev, (uint32_t)mix_stride, (uint32_t)pd.t0, 1, stream)); launches++; }
-      pending.erase(pending.begin() + (long)q);
-    }
-    return "";
-  };
-  uint64_t chunk_index = 0;
-  bool joined = true;
-  // FDSP_PIPE_TRACE=1: print the device timeline of the two pipeline stages (diagnostic; synchronises)
-  const bool trace = pipelined && getenv("FDSP_PIPE_TRACE") != nullptr;
-  std::vector<Event> tev;   // per chunk: dry start, dry end, fdn start, fdn end
-  auto tmark = [&](cudaStream_t st) { if (trace) { tev.emplace_back(); cudaEventCreate(tev.back().put()); cudaEventRecord(tev.back(), st); } };
   if (tree && !want_v) TRY(d_rows.grow((size_t)V() * nout * CH));
-  const bool save_want_v = want_v, save_want_m = want_m;
   // pipelined banks accumulate into a zeroed mix: cleared once for the whole call, so that nothing sits between the dry-stage launches of
   // consecutive chunks on `stream` (a gap there lets the wide FDN kernel of the previous chunk take every SM first)
-  if (pipelined && save_want_m) CU(cudaMemset2DAsync(mix_dev, (size_t)mix_stride * 4, 0, (size_t)n * 4, (size_t)nout, stream));
-  for (uint64_t t0 = 0; t0 < n; t0 += CH, chunk_index++) {
-    const uint32_t len = (uint32_t)std::min<uint64_t>(CH, n - t0);
-    bool first = true;
-    if (pipelined && save_want_m) first = false;   // every class accumulates into the mix region zeroed above (reductions of pipelined classes arrive late)
-    bool want_v = save_want_v, want_m = save_want_m;
-    float* out_dev_c = out_dev; uint64_t out_stride_c = out_stride; uint64_t out_t0 = t0;
-    if (tree) { want_m = false; if (!save_want_v) { want_v = true; out_dev_c = d_rows; out_stride_c = CH; out_t0 = 0; } }
-    const int mode = (want_v ? 1 : 0) | (want_m ? 2 : 0);
+  if (pipelined && want_m) CU(cudaMemset2DAsync(mix_dev, (size_t)mix_stride * 4, 0, (size_t)n * 4, (size_t)nout, stream));
+  for (uint64_t t0 = 0, index = 0; t0 < n; t0 += CH, index++) {
+    Chunk w;
+    w.t0 = t0; w.index = index; w.len = (uint32_t)std::min<uint64_t>(CH, n - t0);
+    w.mix = mix_dev; w.mix_stride = (uint32_t)mix_stride; w.pipelined = pipelined;
+    w.want_v = want_v; w.want_m = want_m; w.out = out_dev; w.out_stride = (uint32_t)out_stride; w.out_t0 = (uint32_t)t0;
+    if (tree) { w.want_m = false; if (!want_v) { w.want_v = true; w.out = d_rows; w.out_stride = CH; w.out_t0 = 0; } }
+    bool first = !(pipelined && want_m);   // every class accumulates into the mix region zeroed above (reductions of pipelined classes arrive late)
     // several plain classes: launch the class kernels concurrently (own streams, forked from and joined back into `stream`); the
     // partial mixes are still reduced on `stream` in class order, so the result does not depend on how the kernels overlap
-    bool concurrent = classes.size() > 1 && !pipelined && len > 64 && !getenv("FDSP_NO_CONCURRENT");
-    for (auto& c : classes) concurrent = concurrent && !c.fdn;
+    bool concurrent = classes.size() > 1 && !pipelined && w.len > 64 && !getenv("FDSP_NO_CONCURRENT");
+    for (auto& c : classes) concurrent = concurrent && c.form == Form::plain;
     if (concurrent) CU(cudaEventRecord(e_begin, stream));
-    // (Launching the class with the longest dependency chain first, on a high-priority stream, is worse for config 5 than class order:
-    // its CTAs hold ~195 KB of shared memory, so every light class then waits for all of it.
-    // FDSP_HEAVY_FIRST=1 keeps that order for experiments; FDSP_CARVEOUT=<percent> makes every class kernel ask for the same carve-out.)
-    std::vector<size_t> order(classes.size());
-    for (size_t q = 0; q < order.size(); q++) order[q] = q;
-    if (concurrent && getenv("FDSP_HEAVY_FIRST"))
-      std::stable_sort(order.begin(), order.end(), [&](size_t x, size_t y) { return (classes[x].k && classes[x].k->stages > 1) > (classes[y].k && classes[y].k->stages > 1); });
-    struct CarveGuard { int saved; CarveGuard() : saved(launch_carveout()) {} ~CarveGuard() { launch_carveout() = saved; } } carve_guard;
+    // (The classes start in class order: starting the one with the longest dependency chain first, on a high-priority stream, was worse for
+    // config 5. Its CTAs hold ~195 KB of shared memory, so every light class then waits for all of it.)
     // Concurrent classes ask for ONE carve-out, the maximum: the class that stages the wavetables (~195 KB per CTA) needs it anyway, and kernels
     // that prefer different L1 / shared-memory splits do not share an SM.
-    if (concurrent) { const char* cv = getenv("FDSP_CARVEOUT"); launch_carveout() = cv ? atoi(cv) : 100; }
-    for (size_t oi = 0; oi < order.size(); oi++) {
-      auto& c = classes[order[oi]];
-      const uint32_t V = c.V();
-      cudaStream_t ks = stream;
+    struct CarveGuard { int saved; CarveGuard() : saved(launch_carveout()) {} ~CarveGuard() { launch_carveout() = saved; } } carve_guard;
+    if (concurrent) launch_carveout() = 100;
+    for (auto& c : classes) {
+      // the class's own stream, forked from `stream` before its arguments are built and joined back into it below (voice_args may upload
+      // a looping sequencer's reset image: with the fork after that upload, such banks rendered wrong on an H100)
       if (concurrent) {
         if (!c.cstream) { CU(cudaStreamCreateWithFlags(c.cstream.put(), cudaStreamNonBlocking)); CU(cudaEventCreateWithFlags(c.e_done.put(), cudaEventDisableTiming)); }
-        ks = c.cstream;
-        CU(cudaStreamWaitEvent(ks, e_begin, 0));
+        CU(cudaStreamWaitEvent(c.cstream, e_begin, 0));
       }
-      const ClassGrid g = class_grid(c, len, device);
-      int fdn_warps = 1;   // voices (= warps) per CTA of the FDN kernel
-      if (c.fdn) {
-        const int cap = fdn_max_warps();
-        // pipelined: leave SMs free for the CTAs of the dry stage of the next chunk (their shared-memory tables cannot share an SM
-        // with an FDN CTA), otherwise the two stages serialise on SM residency
-        const uint32_t nsm = sm_count(device);
-        uint32_t sms = nsm;
-        if (pipelined && c.k) sms = g.ctas < nsm / 2 ? nsm - g.ctas : nsm / 2;
-        fdn_warps = (int)((V + sms - 1) / sms); if (fdn_warps > cap) fdn_warps = cap; if (fdn_warps < 1) fdn_warps = 1;
-      }
-      auto launch_voice = [&](const BankArgs& args, int md, cudaStream_t st) { return g.staged ? c.k->launch_staged(args, md, table_bytes_of(c, len), st) : c.k->launch(args, md, table_bytes_of(c, len), st); };
-      const uint32_t grid = c.fdn ? V : g.ctas;   // rows of the partial-mix buffer: one per CTA of a voice program, one per VOICE of the FDN kernel (its warps never meet)
+      const ClassGrid g = class_grid(c, w.len, device);
       BankArgs a;
-      TRY(voice_args(c, len, g.vpc, &a));
+      TRY(voice_args(c, w.len, g.vpc, &a));
       a.in = in_dev; a.in_stride = (uint32_t)in_stride; a.in_offset = (uint32_t)t0;
-      if (c.conv) {
-        // stage 1: the program in front of the convolver writes its rows behind the history columns; then x_lo, the Toeplitz GEMM tiles
-        // (rows straight into the caller's buffer, or an internal one), the history shift, and the voice-order fold of the rows
-        BankArgs d = a;
-        d.out = c.d_cx; d.out_stride = c.conv_stride; d.out_offset = c.conv_H; d.row_map = c.d_dryrows;
-        CU(launch_voice(d, 1, stream));
-        CU(launch_conv_split(c.d_cx, c.d_cxl, V, c.conv_stride, c.conv_H, len, stream));
-        float* y = want_v ? out_dev_c : nullptr; uint32_t ys = (uint32_t)out_stride_c, yo = (uint32_t)out_t0;
-        if (!y) {
-          TRY(c.d_crows.grow((size_t)V * TIME_CHUNK));
-          y = c.d_crows; ys = TIME_CHUNK; yo = 0;
+      if (c.form != Form::conv) {   // the window of the programs that write rows and a partial mix
+        if (w.want_m) {   // one row per CTA of a voice program, one per VOICE of the FDN kernel (its warps never meet); sized for TIME_CHUNK
+          const uint32_t grid = c.form == Form::fdn ? c.V() : g.ctas;
+          if (c.d_partial.size() < (size_t)grid * nout * w.len) TRY(c.d_partial.grow((size_t)grid * nout * TIME_CHUNK));
+          a.partial = c.d_partial;
         }
-        TRY(dom_mark(stream));
-        CU(launch_conv_tc(c.conv_maps, y, ys, yo, c.d_dryrows, V, len, c.conv_K, c.conv_H, stream));
-        TRY(dom_mark(stream));
-        CU(launch_conv_history(c.d_cx, c.d_cxl, V, c.conv_stride, c.conv_H, len, stream));
-        launches += 4;
-        if (want_m) { CU(launch_tree_mix(y, V, 1u, ys, yo, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, 0, stream)); launches++; }
-        first = false;
-        continue;
+        a.out = w.want_v ? w.out : nullptr; a.out_stride = w.out_stride; a.out_offset = w.out_t0;
+        a.mix = w.mix; a.mix_stride = w.mix_stride; a.mix_offset = (uint32_t)t0; a.mix_accumulate = first ? 0 : 1;
+        if (t0 > 0xffffffffull - TIME_CHUNK) return "#A render too long for one call";
       }
-      if (want_m) {   // (sized for the longest launch: TIME_CHUNK, or PIPE_CHUNK for the second buffer of a pipelined class)
-        const size_t need = (size_t)grid * nout * len;
-        if (c.d_partial.size() < need) TRY(c.d_partial.grow((size_t)grid * nout * TIME_CHUNK));
-        if (pipelined && c.fdn && c.k && c.d_partial2.size() < need) TRY(c.d_partial2.grow((size_t)grid * nout * PIPE_CHUNK));
+      switch (c.form) {
+        case Form::plain: TRY(run_plain(c, w, g, a, first, concurrent)); break;
+        case Form::fdn: TRY(run_fdn(c, w, g, a, first, pending)); break;
+        case Form::conv: TRY(run_conv(c, w, g, a)); break;
       }
-      a.out = want_v ? out_dev_c : nullptr;
-      if (want_m) a.partial = c.d_partial;
-      a.out_stride = (uint32_t)out_stride_c; a.out_offset = (uint32_t)out_t0;
-      // process()-sized launches of plain voice programs finish their mix-down inside the kernel (one launch instead of two)
-      const bool fused_mix = want_m && !c.fdn && len <= 64;
-      if (fused_mix) a.ticket = d_ticket;
-      a.mix = mix_dev; a.mix_stride = (uint32_t)mix_stride; a.mix_offset = (uint32_t)t0; a.mix_accumulate = first ? 0 : 1;
-      if (t0 > 0xffffffffull - TIME_CHUNK) return "#A render too long for one call";
-      if (c.fdn && len > TIME_CHUNK) return "internal: chunk";
-      // long launches of wavetable programs stage the table set in shared memory (TMA bulk copy, ~160 KB per CTA);
-      // short ones (process()-sized) read the tables through L1/L2 instead
-      if (c.fdn) {
-        FdnArgs f;
-        f.params = c.d_params; f.state = c.d_state; f.uniform = c.d_uniform; f.p0 = c.p0; f.s0 = c.s0; f.u0 = c.u0; f.scalar_row = c.scalar_row;
-        f.out = want_v ? out_dev_c : nullptr; f.row_map = c.d_rowmap; f.out_stride = (uint32_t)out_stride_c; f.out_offset = (uint32_t)out_t0;
-        f.partial = a.partial;
-        f.ring = c.d_ring; f.ring_voice_stride = c.ring_floats; f.V = V; f.n = len;
-        if (c.k && pipelined) {
-          // stage 1 of chunk k on `stream`, stage 2 on `stream2`; buffers alternate, chunk k-1's partial mix is reduced after
-          // stage 1 of chunk k has been queued so that the two stages of neighbouring chunks run side by side
-          const int buf = (int)(chunk_index & 1);
-          float* dry = buf ? c.d_dry2 : c.d_dry;
-          CU(cudaStreamWaitEvent(stream, c.e_fdn[buf], 0));   // FDN of chunk k-2 has consumed this dry buffer (no-op before the first record)
-          BankArgs d = a;
-          d.out = dry; d.partial = nullptr; d.out_stride = PIPE_CHUNK; d.out_offset = 0; d.row_map = c.d_dryrows;
-          tmark(stream);
-          CU(launch_voice(d, 1, stream));
-          launches++;
-          tmark(stream);
-          CU(cudaEventRecord(c.e_dry[buf], stream));
-          // A bank of this one class keeps `stream` for the dry stage alone — chunk k + 1 follows chunk k with nothing in between, so it
-          // holds its SMs before the wide FDN kernel of chunk k floods the rest — and reduces on stream2 behind the FDN kernel. With other
-          // classes in the bank every reduction stays on `stream` (they accumulate into the same mix region), one chunk late.
-          const bool solo = classes.size() == 1;
-          if (!solo) TRY(flush_pending(&c));   // reduce chunk k-1 of this class (waits for its FDN)
-          f.dry = dry; f.dry_voice_stride = 2ull * PIPE_CHUNK; f.dry_ch_stride = PIPE_CHUNK; f.dry_offset = 0;
-          if (want_m && buf) f.partial = c.d_partial2;
-          CU(cudaStreamWaitEvent(stream2, c.e_dry[buf], 0));
-          tmark(stream2);
-          TRY(dom_mark(stream2));
-          CU(launch_fdn(f, fdn_warps, stream2));
-          TRY(dom_mark(stream2));
-          launches++;
-          tmark(stream2);
-          CU(cudaEventRecord(c.e_fdn[buf], stream2));
-          if (!solo) pending.push_back({&c, grid, len, t0, buf});
-          else {
-            if (want_m) { CU(launch_mix_reduce(buf ? c.d_partial2 : c.d_partial, grid, (uint32_t)nout, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, 1, stream2)); launches++; }
-            joined = false;   // stream2 carries work `stream` has not waited for (rows written by the FDN kernel, the reduction): joined after the loop
-          }
-          continue;
-        }
-        if (c.k) {  // stage 1: the fused dry program writes stereo rows [V][2][TIME_CHUNK]
-          BankArgs d = a;
-          d.out = c.d_dry; d.partial = nullptr; d.out_stride = TIME_CHUNK; d.out_offset = 0; d.row_map = c.d_dryrows;
-          CU(launch_voice(d, 1, stream));
-          launches++;
-          f.dry = c.d_dry; f.dry_voice_stride = 2ull * TIME_CHUNK; f.dry_ch_stride = TIME_CHUNK; f.dry_offset = 0;
-        } else {    // reverb applied straight to the bank's stereo input
-          f.dry = in_dev; f.dry_voice_stride = 0; f.dry_ch_stride = (uint32_t)in_stride; f.dry_offset = (uint32_t)t0;
-        }
-        TRY(dom_mark(stream));
-        CU(launch_fdn(f, fdn_warps, stream));
-        TRY(dom_mark(stream));
-      } else {
-        TRY(dom_mark(ks));
-        CU(launch_voice(a, mode, ks));
-        TRY(dom_mark(ks));
-      }
-      launches++;
-      if (concurrent) { CU(cudaEventRecord(c.e_done, ks)); continue; }   // reduced below, after every class has been launched
-      if (want_m && !fused_mix) {
-        CU(launch_mix_reduce(c.d_partial, grid, (uint32_t)nout, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, first ? 0 : 1, stream));
-        launches++;
-      }
-      first = false;
+      if (!concurrent) first = false;
     }
-    if (concurrent) {
-      for (auto& c : classes) {
-        CU(cudaStreamWaitEvent(stream, c.e_done, 0));
-        if (want_m) {
-          CU(launch_mix_reduce(c.d_partial, class_grid(c, len, device).ctas, (uint32_t)nout, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, first ? 0 : 1, stream));
-          launches++;
-        }
-        first = false;
-      }
+    if (concurrent) for (auto& c : classes) {
+      CU(cudaStreamWaitEvent(stream, c.e_done, 0));
+      TRY(reduce_mix(c.d_partial, class_grid(c, w.len, device).ctas, w, !first, stream));
+      first = false;
     }
     if (tree) {
       const size_t sc = tree_mix == 1 ? tree_mix_scratch_floats(V(), (uint32_t)nout, CH) : 0;   // balanced tree of a big bank: subtree sums first
       TRY(d_treepart.grow(sc));
-      CU(launch_tree_mix(out_dev_c, V(), (uint32_t)nout, (uint32_t)out_stride_c, (uint32_t)out_t0, len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, tree_mix == 1 ? 1 : 0, stream, sc ? d_treepart.get() : nullptr));
+      CU(launch_tree_mix(w.out, V(), (uint32_t)nout, w.out_stride, w.out_t0, w.len, mix_dev, (uint32_t)mix_stride, (uint32_t)t0, tree_mix == 1 ? 1 : 0, stream, sc ? d_treepart.get() : nullptr));
       launches += sc ? 2 : 1;
     }
   }
-  TRY(flush_pending(nullptr));   // also joins stream2 back into `stream`
-  if (!joined) { CU(cudaEventRecord(e_begin, stream2)); CU(cudaStreamWaitEvent(stream, e_begin, 0)); }   // solo two-stage class: its reductions ran on stream2
+  TRY(flush_pending(pending, nullptr));   // also joins stream2 back into `stream`
+  // a two-stage class alone in its bank reduces on stream2
+  if (pipelined && classes.size() == 1) { CU(cudaEventRecord(e_begin, stream2)); CU(cudaStreamWaitEvent(stream, e_begin, 0)); }
   if (timing) CU(cudaEventRecord(ev1, stream));
-  if (trace) {
-    CU(cudaStreamSynchronize(stream));
-    for (size_t q = 0; q + 3 < tev.size(); q += 4) {
-      float t[4];
-      for (int w = 0; w < 4; w++) cudaEventElapsedTime(&t[w], ev0, tev[q + w]);
-      fprintf(stderr, "[pipe] chunk %zu: dry %.3f..%.3f ms   fdn %.3f..%.3f ms\n", q / 4, t[0], t[1], t[2], t[3]);
-    }
-  }
   dirty = true; advance_clock(n);
   return "";
 }
@@ -1193,7 +1188,7 @@ std::string Bank::process(uint32_t size, const float* in, float* out) {  // Audi
   struct NoTiming { bool& t; explicit NoTiming(bool& x) : t(x) { t = false; } ~NoTiming() { t = true; } } no_timing(timing);  // no event records on this path
   struct InProcess { bool& f; explicit InProcess(bool& x) : f(x) { f = true; } ~InProcess() { f = false; } } in_proc(in_process);
   bool two_stage = false;   // pipelined classes clear / accumulate the mix region on the device: keep that in device memory
-  for (auto& c : classes) two_stage = two_stage || (c.fdn && c.k);
+  for (auto& c : classes) two_stage = two_stage || c.fdn_with_dry();
   if (mix && two_stage) {
     TRY(render_device(size, d_in, 64, nullptr, 64, d_mix, 64));
     CU(cudaMemcpyAsync(h_out, d_mix, rows * 64 * 4, cudaMemcpyDeviceToHost, stream));
@@ -1225,7 +1220,7 @@ std::string Bank::clone_into(Bank& dst) const {
     if (!s.state0.empty()) CU(cudaMemcpy(d.d_state, s.d_state, s.state0.size() * 4, cudaMemcpyDeviceToDevice));
     if (s.dl_floats) CU(cudaMemcpy(d.d_dline, s.d_dline, (size_t)s.dl_floats * s.V() * 4, cudaMemcpyDeviceToDevice));
     if (s.ring_floats && s.d_ring && d.d_ring) CU(cudaMemcpy(d.d_ring, s.d_ring, (size_t)s.ring_floats * s.V() * 4, cudaMemcpyDeviceToDevice));
-    if (s.conv && d.conv) { CU(cudaMemcpy(d.d_cx, s.d_cx, (size_t)s.V() * s.conv_stride * 4, cudaMemcpyDeviceToDevice)); CU(cudaMemcpy(d.d_cxl, s.d_cxl, (size_t)s.V() * s.conv_stride * 4, cudaMemcpyDeviceToDevice)); }
+    if (s.form == Form::conv && d.form == Form::conv) { CU(cudaMemcpy(d.d_cx, s.d_cx, (size_t)s.V() * s.conv_stride * 4, cudaMemcpyDeviceToDevice)); CU(cudaMemcpy(d.d_cxl, s.d_cxl, (size_t)s.V() * s.conv_stride * 4, cudaMemcpyDeviceToDevice)); }
   }
   dst.dirty = dirty; dst.seq_time = seq_time;
   for (auto& kv : slot_latest) { SlotLatest& w = dst.slot_latest[kv.first]; w.unit.reset(kv.second.unit->clone()); w.ease = kv.second.ease; w.fade_time = kv.second.fade_time; }

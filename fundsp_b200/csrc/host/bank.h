@@ -19,19 +19,25 @@ namespace host {
 // Error convention of the runtime: "" = ok, otherwise the message, which may start with a status tag that csrc/capi.cpp turns into the
 // ABI's code and strips: "#U " unsupported (FDSP_ERR_UNSUPPORTED), "#A " bad argument (FDSP_ERR_ARG), "#N " no free slot (push_event falls
 // back to growing the bank). Untagged messages are device / driver failures (FDSP_ERR_CUDA). Codes never depend on the wording.
+// How a class runs on the device (Bank::lower_and_upload chooses it): one fused voice program; a reverb_stereo tail in the warp-per-voice
+// FDN kernel (dsp/fdn_kernel.cuh), `k` then being the dry-stage program in front of it (may be null); a `... >> convolve(h)` tail on tensor
+// cores (dsp/conv_tc_kernel.cuh), `k` then being the program in front of the Convolver. The convolver form is for one-class banks.
+enum class Form { plain, fdn, conv };
+struct ClassGrid;   // the launch shape of a class's program (bank.cpp class_grid)
 struct VoiceClass {
   std::string sig;
   std::shared_ptr<const Program> k;
+  Form form = Form::plain;
   std::vector<uint32_t> voices;     // global voice indices, ascending
   std::vector<uint32_t> uniform;    // class-uniform words (delay lengths ...)
   uint64_t dl_floats = 0;           // delay-line floats per voice (thread-per-voice layout [pos][voice])
   uint32_t np = 0, ns = 0, nu = 0;  // words per voice (whole graph)
-  // reverb_stereo tail handled by the warp-per-voice FDN kernel (dsp/fdn_kernel.cuh); `k` is then the dry-stage program (may be null)
-  bool fdn = false; int scalar_row = -1; uint32_t p0 = 0, s0 = 0, u0 = 0; uint64_t ring_floats = 0;
+  // FDN form: where the reverb's words start, its rings, the rows its dry stage writes
+  int scalar_row = -1; uint32_t p0 = 0, s0 = 0, u0 = 0; uint64_t ring_floats = 0;
   Array<float> d_ring, d_dry; Array<uint32_t> d_dryrows;
-  // `... >> convolve(h)` tail on tensor cores (dsp/conv_tc_kernel.cuh): `k` is then the program in front of the Convolver; its output rows
-  // live in d_cx [V][conv_H + chunk] (history columns in front), d_cxl = their TF32 remainders, d_th / d_tl = Toeplitz(h) hi / lo
-  bool conv = false; uint32_t conv_K = 0, conv_H = 0, conv_J = 0, conv_stride = 0, conv_off = 0;
+  // convolver form: the output rows of `k` live in d_cx [V][conv_H + chunk] (history columns in front), d_cxl = their TF32 remainders,
+  // d_th / d_tl = Toeplitz(h) hi / lo
+  uint32_t conv_K = 0, conv_H = 0, conv_J = 0, conv_stride = 0, conv_off = 0;
   Array<float> d_cx, d_cxl, d_th, d_tl, d_crows;
   ConvTcMaps conv_maps;
   // two-stage classes are software-pipelined over sub-chunks: dry stage of chunk k+1 (stream) runs beside the FDN of chunk k (stream2)
@@ -51,6 +57,8 @@ struct VoiceClass {
   Array<uint32_t> d_params, d_state, d_uniform, d_rowmap;
   Array<float> d_dline, d_partial;
   uint32_t V() const { return (uint32_t)voices.size(); }
+  bool fdn_with_dry() const { return form == Form::fdn && k; }   // two stages, software-pipelined by render_device_run
+  std::string clear_history(cudaStream_t st);   // zeroes what the form's own buffers carry from call to call (on upload and reset)
 };
 
 struct Bank {
@@ -119,6 +127,14 @@ struct Bank {
   std::string slot_service(uint64_t n, uint64_t* cut);   // arms parked units whose fade is over; *cut = samples (<= n) after which the first running fade with a parked unit ends
   std::string voice_args(VoiceClass& c, uint32_t len, uint32_t vpc, BankArgs* a);   // class c's part of a launch's arguments; the window starts empty
   std::string render_device_run(uint64_t n, const float* in_dev, uint64_t in_stride, float* out_dev, uint64_t out_stride, float* mix_dev, uint64_t mix_stride);
+  // the steps of render_device_run (bank.cpp): a chunk's window, a deferred reduction of a pipelined class, and the launches of each form
+  struct Chunk; struct Pending;
+  std::string reduce_mix(const float* partial, uint32_t grid, const Chunk& w, bool accumulate, cudaStream_t st);
+  std::string flush_pending(std::vector<Pending>& pending, const VoiceClass* only);
+  std::string launch_dry(VoiceClass& c, BankArgs d, const ClassGrid& g, float* rows, uint32_t stride, uint32_t offset);
+  std::string run_plain(VoiceClass& c, const Chunk& w, const ClassGrid& g, BankArgs& a, bool first, bool concurrent);
+  std::string run_fdn(VoiceClass& c, const Chunk& w, const ClassGrid& g, const BankArgs& a, bool first, std::vector<Pending>& pending);
+  std::string run_conv(VoiceClass& c, const Chunk& w, const ClassGrid& g, const BankArgs& a);
   std::string push_event(HNode* event, uint32_t* voice);                      // Sequencer::push on a running bank: takes the slot of a finished event of the same class; consumes event
   std::string set(uint32_t voice, const Setting& s);  // AudioUnit::set on one voice of a live bank (parameters only; state continues)
   std::string ensure_staging(uint32_t chunk);
