@@ -113,7 +113,7 @@ std::string Bank::init(std::vector<HNode*>& voices, int dev, uint32_t mode) {
   CU(cudaStreamCreateWithPriority(stream.put(), cudaStreamNonBlocking, prio_hi));
   CU(cudaStreamCreateWithPriority(stream2.put(), cudaStreamNonBlocking, prio_lo));
   CU(cudaEventCreate(ev0.put())); CU(cudaEventCreate(ev1.put())); CU(cudaEventCreateWithFlags(e_begin.put(), cudaEventDisableTiming));
-  TRY(d_ticket.grow(1)); CU(cudaMemset(d_ticket, 0, 4));
+  TRY(d_ticket.grow(1)); CU(cudaMemsetAsync(d_ticket, 0, 4, stream));
   return lower_and_upload(true);
 }
 
@@ -204,7 +204,7 @@ std::string Bank::lower_and_upload(bool upload_state) {
   }
   for (auto& c : classes) {
     const uint32_t V = c.V(); const int NP = (int)c.np, NS = (int)c.ns;
-    std::vector<uint32_t> P((size_t)NP * V), S((size_t)NS * V), rows(V);
+    std::vector<uint32_t> P((size_t)NP * V), S((size_t)NS * V), rows(V), id;
     for (uint32_t i = 0; i < V; i++) {
       const Lowering& l = lows[c.voices[i]].l;
       for (int k = 0; k < NP; k++) P[(size_t)k * V + i] = l.P[k];
@@ -235,23 +235,21 @@ std::string Bank::lower_and_upload(bool upload_state) {
       }
       if (c.fdn_with_dry() || c.form == Form::conv) {   // the rows the dry stage writes (two per voice) or the convolver reads (one per voice)
         TRY(c.d_dryrows.grow(V));
-        std::vector<uint32_t> id(V);
+        id.resize(V);
         for (uint32_t i = 0; i < V; i++) id[i] = c.form == Form::conv ? i : 2 * i;
-        CU(cudaMemcpy(c.d_dryrows, id.data(), V * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpyAsync(c.d_dryrows, id.data(), V * 4, cudaMemcpyHostToDevice, stream));
       }
-      CU(cudaMemcpy(c.d_rowmap, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice));
-      if (!c.uniform.empty()) CU(cudaMemcpy(c.d_uniform, c.uniform.data(), c.uniform.size() * 4, cudaMemcpyHostToDevice));
+      CU(cudaMemcpyAsync(c.d_rowmap, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, stream));
+      if (!c.uniform.empty()) CU(cudaMemcpyAsync(c.d_uniform, c.uniform.data(), c.uniform.size() * 4, cudaMemcpyHostToDevice, stream));
     }
-    if (!P.empty()) CU(cudaMemcpy(c.d_params, P.data(), P.size() * 4, cudaMemcpyHostToDevice));
+    if (!P.empty()) CU(cudaMemcpyAsync(c.d_params, P.data(), P.size() * 4, cudaMemcpyHostToDevice, stream));
     if (upload_state) {
-      if (!S.empty()) CU(cudaMemcpy(c.d_state, S.data(), S.size() * 4, cudaMemcpyHostToDevice));
-      if (c.dl_floats) CU(cudaMemset(c.d_dline, 0, (size_t)c.dl_floats * V * sizeof(float)));
-      TRY(c.clear_history(0));   // (on the default stream, like the cudaMemset above)
-      if (c.form == Form::conv) {
-        CU(launch_conv_toeplitz(reinterpret_cast<const float*>(c.d_uniform + c.conv_off + 2), c.conv_K, c.d_th, c.d_tl, c.conv_J, stream));
-        CU(cudaStreamSynchronize(stream));
-      }
+      if (!S.empty()) CU(cudaMemcpyAsync(c.d_state, S.data(), S.size() * 4, cudaMemcpyHostToDevice, stream));
+      if (c.dl_floats) CU(cudaMemsetAsync(c.d_dline, 0, (size_t)c.dl_floats * V * sizeof(float), stream));
+      TRY(c.clear_history(stream));
+      if (c.form == Form::conv) CU(launch_conv_toeplitz(reinterpret_cast<const float*>(c.d_uniform + c.conv_off + 2), c.conv_K, c.d_th, c.d_tl, c.conv_J, stream));
     }
+    CU(cudaStreamSynchronize(stream));   // P, S, rows and id are pageable and go out of scope
   }
   // 3. wavetables used by any class (a class that arrives later — add_voice — may bring a waveform the bank has not loaded yet)
   {
@@ -266,12 +264,12 @@ std::string Bank::lower_and_upload(bool upload_state) {
       h_wt[kind].n = (int)t.pitch.size(); h_wt[kind].total = (int)t.data.size();
       for (size_t i = 0; i < t.pitch.size() && i < 48; i++) { h_wt[kind].pitch[i] = t.pitch[i]; h_wt[kind].off[i] = t.off[i]; h_wt[kind].len[i] = t.len[i]; }
       TRY(d_wtdata[kind].grow(t.data.size()));
-      CU(cudaMemcpy(d_wtdata[kind], t.data.data(), t.data.size() * 4, cudaMemcpyHostToDevice));
+      CU(cudaMemcpyAsync(d_wtdata[kind], t.data.data(), t.data.size() * 4, cudaMemcpyHostToDevice, stream));
       h_wt[kind].data = d_wtdata[kind];
       changed = true;
     }
     if (!d_wt) { TRY(d_wt.grow(6)); changed = true; }
-    if (changed) CU(cudaMemcpy(d_wt, h_wt, sizeof(h_wt), cudaMemcpyHostToDevice));
+    if (changed) { CU(cudaMemcpyAsync(d_wt, h_wt, sizeof(h_wt), cudaMemcpyHostToDevice, stream)); CU(cudaStreamSynchronize(stream)); }   // (h_wt is pageable)
   }
   if (upload_state) dirty = false;
   return sh_rebuild();
@@ -341,7 +339,11 @@ std::string Bank::state0_to_device(VoiceClass& c, const uint32_t** out) {
   *out = nullptr;
   if (!(loop_arg > 0.0) || c.state0.empty() || c.sig.compare(0, 6, "Event<") != 0) return "";
   if (!c.d_state0) { TRY(c.d_state0.grow(c.state0.size())); c.state0_stale = true; }
-  if (c.state0_stale) { CU(cudaMemcpy(c.d_state0, c.state0.data(), c.state0.size() * 4, cudaMemcpyHostToDevice)); c.state0_stale = false; }
+  if (c.state0_stale) {   // on `stream` ahead of the launches that read it (render_device_run uploads before it forks the class streams)
+    CU(cudaMemcpyAsync(c.d_state0, c.state0.data(), c.state0.size() * 4, cudaMemcpyHostToDevice, stream));
+    CU(cudaStreamSynchronize(stream));   // c.state0 is pageable and changes with the next edit of a voice
+    c.state0_stale = false;
+  }
   *out = c.d_state0;
   return "";
 }
@@ -1070,6 +1072,7 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
     // partial mixes are still reduced on `stream` in class order, so the result does not depend on how the kernels overlap
     bool concurrent = classes.size() > 1 && !pipelined && w.len > 64 && !getenv("FDSP_NO_CONCURRENT");
     for (auto& c : classes) concurrent = concurrent && c.form == Form::plain;
+    for (auto& c : classes) { const uint32_t* s0 = nullptr; TRY(state0_to_device(c, &s0)); }   // (uploads stale reset images before the fork)
     if (concurrent) CU(cudaEventRecord(e_begin, stream));
     // (The classes start in class order: starting the one with the longest dependency chain first, on a high-priority stream, was worse for
     // config 5. Its CTAs hold ~195 KB of shared memory, so every light class then waits for all of it.)
@@ -1078,8 +1081,7 @@ std::string Bank::render_device_run(uint64_t n, const float* in_dev, uint64_t in
     struct CarveGuard { int saved; CarveGuard() : saved(launch_carveout()) {} ~CarveGuard() { launch_carveout() = saved; } } carve_guard;
     if (concurrent) launch_carveout() = 100;
     for (auto& c : classes) {
-      // the class's own stream, forked from `stream` before its arguments are built and joined back into it below (voice_args may upload
-      // a looping sequencer's reset image: with the fork after that upload, such banks rendered wrong on an H100)
+      // every device operation of a bank is ordered on the bank's own streams: a class's stream is forked from `stream` and joined back below
       if (concurrent) {
         if (!c.cstream) { CU(cudaStreamCreateWithFlags(c.cstream.put(), cudaStreamNonBlocking)); CU(cudaEventCreateWithFlags(c.e_done.put(), cudaEventDisableTiming)); }
         CU(cudaStreamWaitEvent(c.cstream, e_begin, 0));
@@ -1214,14 +1216,17 @@ std::string Bank::clone_into(Bank& dst) const {
   for (auto& n : dst.nodes) n->set_sample_rate(sr);
   TRY(dst.lower_and_upload(true));
   CU(cudaSetDevice(device));
-  CU(cudaStreamSynchronize(stream));
+  // the running state is copied on the source's stream, behind its renders and ahead of its next one; the clone's stream waits for it
+  auto copy = [&](void* d, const void* s, size_t bytes) { return cudaMemcpyAsync(d, s, bytes, cudaMemcpyDeviceToDevice, stream); };
   for (size_t i = 0; i < classes.size(); i++) {
     const VoiceClass& s = classes[i]; VoiceClass& d = dst.classes[i];
-    if (!s.state0.empty()) CU(cudaMemcpy(d.d_state, s.d_state, s.state0.size() * 4, cudaMemcpyDeviceToDevice));
-    if (s.dl_floats) CU(cudaMemcpy(d.d_dline, s.d_dline, (size_t)s.dl_floats * s.V() * 4, cudaMemcpyDeviceToDevice));
-    if (s.ring_floats && s.d_ring && d.d_ring) CU(cudaMemcpy(d.d_ring, s.d_ring, (size_t)s.ring_floats * s.V() * 4, cudaMemcpyDeviceToDevice));
-    if (s.form == Form::conv && d.form == Form::conv) { CU(cudaMemcpy(d.d_cx, s.d_cx, (size_t)s.V() * s.conv_stride * 4, cudaMemcpyDeviceToDevice)); CU(cudaMemcpy(d.d_cxl, s.d_cxl, (size_t)s.V() * s.conv_stride * 4, cudaMemcpyDeviceToDevice)); }
+    if (!s.state0.empty()) CU(copy(d.d_state, s.d_state, s.state0.size() * 4));
+    if (s.dl_floats) CU(copy(d.d_dline, s.d_dline, (size_t)s.dl_floats * s.V() * 4));
+    if (s.ring_floats && s.d_ring && d.d_ring) CU(copy(d.d_ring, s.d_ring, (size_t)s.ring_floats * s.V() * 4));
+    if (s.form == Form::conv && d.form == Form::conv) { CU(copy(d.d_cx, s.d_cx, (size_t)s.V() * s.conv_stride * 4)); CU(copy(d.d_cxl, s.d_cxl, (size_t)s.V() * s.conv_stride * 4)); }
   }
+  CU(cudaEventRecord(dst.e_begin, stream));
+  CU(cudaStreamWaitEvent(dst.stream, dst.e_begin, 0));
   dst.dirty = dirty; dst.seq_time = seq_time;
   for (auto& kv : slot_latest) { SlotLatest& w = dst.slot_latest[kv.first]; w.unit.reset(kv.second.unit->clone()); w.ease = kv.second.ease; w.fade_time = kv.second.fade_time; }
   for (auto& kv : xfade_latest) { SlotLatest& w = dst.xfade_latest[kv.first]; w.unit.reset(kv.second.unit->clone()); w.ease = kv.second.ease; w.fade_time = kv.second.fade_time; }

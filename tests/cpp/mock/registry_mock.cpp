@@ -24,9 +24,11 @@ typedef int (*LaunchFn)(const BankArgs*, int);
 typedef int (*LaunchExFn)(const BankArgs*, int, const float*, uint64_t);
 struct MockProgram : Program {
   LaunchFn fn = nullptr; LaunchExFn fn_ex = nullptr;
-  cudaError_t launch(const BankArgs& a, int mode, size_t, cudaStream_t) const override {
+  cudaError_t launch(const BankArgs& a, int mode, size_t, cudaStream_t st) const override {
     mode &= 3;
-    return (mode && fn && fn(&a, mode) == 0) ? cudaSuccess : cudaErrorLaunchFailure;
+    if (!mode || !fn) return cudaErrorLaunchFailure;
+    const LaunchFn f = fn;
+    return mock_launch(st, [f, a, mode] { return f(&a, mode) == 0 ? cudaSuccess : cudaErrorLaunchFailure; });
   }
 };
 std::mutex g_mu;
@@ -69,67 +71,74 @@ int registry_size() { return 0; }
 const KernelEntry* registry_at(int) { return nullptr; }
 const char* registry_key(int) { return ""; }
 
-cudaError_t launch_mix_reduce(const float* partial, uint32_t nparts, uint32_t outs, uint32_t n, float* mix, uint32_t mix_stride, uint32_t mix_offset, int accumulate, cudaStream_t) {
-  for (uint32_t c = 0; c < outs; c++)
-    for (uint32_t t = 0; t < n; t++) {   // mix_reduce_kernel: CTA-order left fold
-      float s = partial[(size_t)c * n + t];
-      for (uint32_t b = 1; b < nparts; b++) s += partial[((size_t)b * outs + c) * n + t];
-      float* p = mix + (size_t)c * mix_stride + mix_offset + t;
-      *p = accumulate ? *p + s : s;
-    }
-  return cudaSuccess;
+// The kernels below are queued on their stream like the programs' (cuda_runtime.h): each body runs when the mock device reaches it.
+cudaError_t launch_mix_reduce(const float* partial, uint32_t nparts, uint32_t outs, uint32_t n, float* mix, uint32_t mix_stride, uint32_t mix_offset, int accumulate, cudaStream_t st) {
+  return mock_launch(st, [=] {
+    for (uint32_t c = 0; c < outs; c++)
+      for (uint32_t t = 0; t < n; t++) {   // mix_reduce_kernel: CTA-order left fold
+        float s = partial[(size_t)c * n + t];
+        for (uint32_t b = 1; b < nparts; b++) s += partial[((size_t)b * outs + c) * n + t];
+        float* p = mix + (size_t)c * mix_stride + mix_offset + t;
+        *p = accumulate ? *p + s : s;
+      }
+    return cudaSuccess;
+  });
 }
-cudaError_t launch_tree_mix(const float* rows, uint32_t V, uint32_t outs, uint32_t row_stride, uint32_t row_offset, uint32_t n, float* mix, uint32_t mix_stride, uint32_t mix_offset, int pairwise, cudaStream_t, float*) {
-  for (uint32_t ch = 0; ch < outs; ch++)
-    for (uint32_t t = 0; t < n; t++) {   // tree_mix_kernel: the binary-carry stack of the balanced tree, or the left fold
-      const float* p = rows + (size_t)ch * row_stride + row_offset + t;
-      const size_t vstep = (size_t)outs * row_stride;
-      float x;
-      if (pairwise) {
-        float st[32];
-        for (uint32_t v = 0; v < V; v++) { float y = p[(size_t)v * vstep]; uint32_t q = v; int lvl = 0; while (q & 1u) { y = st[lvl] + y; q >>= 1; lvl++; } st[lvl] = y; }
-        int lvl = 0; uint32_t q = V;
-        while (!(q & 1u)) { q >>= 1; lvl++; }
-        x = st[lvl]; q >>= 1; lvl++;
-        for (; q; q >>= 1, lvl++) if (q & 1u) x = st[lvl] + x;
-      } else { x = p[0]; for (uint32_t v = 1; v < V; v++) x += p[(size_t)v * vstep]; }
-      mix[(size_t)ch * mix_stride + mix_offset + t] = x;
-    }
-  return cudaSuccess;
+cudaError_t launch_tree_mix(const float* rows, uint32_t V, uint32_t outs, uint32_t row_stride, uint32_t row_offset, uint32_t n, float* mix, uint32_t mix_stride, uint32_t mix_offset, int pairwise, cudaStream_t st, float*) {
+  return mock_launch(st, [=] {
+    for (uint32_t ch = 0; ch < outs; ch++)
+      for (uint32_t t = 0; t < n; t++) {   // tree_mix_kernel: the binary-carry stack of the balanced tree, or the left fold
+        const float* p = rows + (size_t)ch * row_stride + row_offset + t;
+        const size_t vstep = (size_t)outs * row_stride;
+        float x;
+        if (pairwise) {
+          float st[32];
+          for (uint32_t v = 0; v < V; v++) { float y = p[(size_t)v * vstep]; uint32_t q = v; int lvl = 0; while (q & 1u) { y = st[lvl] + y; q >>= 1; lvl++; } st[lvl] = y; }
+          int lvl = 0; uint32_t q = V;
+          while (!(q & 1u)) { q >>= 1; lvl++; }
+          x = st[lvl]; q >>= 1; lvl++;
+          for (; q; q >>= 1, lvl++) if (q & 1u) x = st[lvl] + x;
+        } else { x = p[0]; for (uint32_t v = 1; v < V; v++) x += p[(size_t)v * vstep]; }
+        mix[(size_t)ch * mix_stride + mix_offset + t] = x;
+      }
+    return cudaSuccess;
+  });
 }
 // The warp-per-voice FDN kernel (dsp/fdn_kernel.cuh) computes `reverb_stereo` exactly like the generic thread-per-voice program (the GPU
 // tests compare the two bit for bit), so the mock runs that generic program on the kernel's argument block: the last words of the
 // class are the reverb's words, the rings are its delay lines, the input is each voice's dry stereo rows. This puts the HOST side of the
 // two-stage classes (dry buffers, chunk pipeline, deferred reductions, wet gain row) under the CPU suite.
 static const char* kRevSig = "Pipe<Pipe<MultiSplit<2,16>,Feedback<1,Multi<30,0,32,Pipe<Delay,Fir<3>>>>>,Binop<2,Multi<31,0,32,Panner<1>>,Constant<2>>>";
-cudaError_t launch_fdn(const FdnArgs& f, int warps, cudaStream_t) {
+cudaError_t launch_fdn(const FdnArgs& f, int warps, cudaStream_t st) {
   std::string err;
   auto prog = std::dynamic_pointer_cast<const MockProgram>(get_program(kRevSig, 0, err));
   if (!prog || warps < 1) return cudaErrorLaunchFailure;
-  const uint32_t V = f.V, n = f.n, grid = V;   // the kernel writes one partial-mix row pair per voice
-  std::vector<float> rev((size_t)V * 2 * n, 0.0f);
-  std::vector<uint32_t> rows(V);
-  for (uint32_t v = 0; v < V; v++) rows[v] = 2 * v;
-  BankArgs a; memset(&a, 0, sizeof(a));
-  a.params = f.params + (size_t)f.p0 * V; a.state = f.state + (size_t)f.s0 * V; a.uniform = f.uniform + f.u0;
-  a.dline = f.ring; a.wt = nullptr; a.out = rev.data(); a.V = V; a.n = n; a.vpc = 0;
-  a.in = f.dry; a.in_stride = f.dry_ch_stride; a.in_offset = f.dry_offset; a.out_stride = n; a.out_offset = 0; a.row_map = rows.data();
-  a.sr = 0.0f; a.sd64 = 0.0f; a.sd32 = 0.0f;   // (the reverb's nodes do not read the rate: delay lengths are class-uniform words)
-  if (prog->fn_ex(&a, 1, f.dry_voice_stride ? f.dry : nullptr, f.dry_voice_stride) != 0) return cudaErrorLaunchFailure;
-  if (f.partial) for (size_t e = 0; e < (size_t)grid * 2 * n; e++) f.partial[e] = 0.0f;
-  for (uint32_t v = 0; v < V; v++)
-    for (uint32_t ch = 0; ch < 2; ch++)
-      for (uint32_t t = 0; t < n; t++) {
-        float y = rev[((size_t)2 * v + ch) * n + t];
-        if (f.scalar_row >= 0) {   // Bus<MultiPass<2>, Unop<3, Reverb>>: dry + reverb * g
-          float g; memcpy(&g, f.params + (size_t)f.scalar_row * V + v, 4);
-          const float dry = f.dry[(size_t)v * f.dry_voice_stride + (size_t)ch * f.dry_ch_stride + f.dry_offset + t];
-          y = dry + y * g;
+  return mock_launch(st, [f, prog] {
+    const uint32_t V = f.V, n = f.n, grid = V;   // the kernel writes one partial-mix row pair per voice
+    std::vector<float> rev((size_t)V * 2 * n, 0.0f);
+    std::vector<uint32_t> rows(V);
+    for (uint32_t v = 0; v < V; v++) rows[v] = 2 * v;
+    BankArgs a; memset(&a, 0, sizeof(a));
+    a.params = f.params + (size_t)f.p0 * V; a.state = f.state + (size_t)f.s0 * V; a.uniform = f.uniform + f.u0;
+    a.dline = f.ring; a.wt = nullptr; a.out = rev.data(); a.V = V; a.n = n; a.vpc = 0;
+    a.in = f.dry; a.in_stride = f.dry_ch_stride; a.in_offset = f.dry_offset; a.out_stride = n; a.out_offset = 0; a.row_map = rows.data();
+    a.sr = 0.0f; a.sd64 = 0.0f; a.sd32 = 0.0f;   // (the reverb's nodes do not read the rate: delay lengths are class-uniform words)
+    if (prog->fn_ex(&a, 1, f.dry_voice_stride ? f.dry : nullptr, f.dry_voice_stride) != 0) return cudaErrorLaunchFailure;
+    if (f.partial) for (size_t e = 0; e < (size_t)grid * 2 * n; e++) f.partial[e] = 0.0f;
+    for (uint32_t v = 0; v < V; v++)
+      for (uint32_t ch = 0; ch < 2; ch++)
+        for (uint32_t t = 0; t < n; t++) {
+          float y = rev[((size_t)2 * v + ch) * n + t];
+          if (f.scalar_row >= 0) {   // Bus<MultiPass<2>, Unop<3, Reverb>>: dry + reverb * g
+            float g; memcpy(&g, f.params + (size_t)f.scalar_row * V + v, 4);
+            const float dry = f.dry[(size_t)v * f.dry_voice_stride + (size_t)ch * f.dry_ch_stride + f.dry_offset + t];
+            y = dry + y * g;
+          }
+          if (f.out) f.out[(size_t)(f.row_map[v] + ch) * f.out_stride + f.out_offset + t] = y;
+          if (f.partial) f.partial[((size_t)v * 2 + ch) * n + t] += y;
         }
-        if (f.out) f.out[(size_t)(f.row_map[v] + ch) * f.out_stride + f.out_offset + t] = y;
-        if (f.partial) f.partial[((size_t)v * 2 + ch) * n + t] += y;
-      }
-  return cudaSuccess;
+    return cudaSuccess;
+  });
 }
 size_t tree_mix_scratch_floats(uint32_t, uint32_t, uint32_t) { return 0; }
 int fdn_max_warps() { return 8; }

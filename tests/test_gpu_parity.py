@@ -211,6 +211,53 @@ def test_reset_and_clone_and_continuation():
     assert np.array_equal(a1, full[..., :1000])
 
 
+def _concurrent_voice(i):   # two plain classes: the bank runs them on streams of their own
+    return (noise().seed(i) >> lowpass_hz(500.0 + 40.0 * i, 1.0)) if i % 2 else (saw_hz(100.0 + 7.0 * i) >> lowpass_hz(900.0 + 10.0 * i, 0.8))
+
+
+def _oracle_units(voices, sr):
+    from oracle import OracleUnit
+    olib().fo_set_denormal_emulation(0)
+    us = [OracleUnit(v) for v in voices]
+    for u in us:
+        u.set_sample_rate(sr)
+    return us
+
+
+def test_clone_and_source_render_alternately():
+    """A clone and its source take turns, each call uploading nothing and reading the state the other's copy or render left: the clone's
+    state is copied behind the source's renders and ahead of the clone's. Both continue like the oracle units, bit for bit."""
+    from fundsp_b200.bank import GpuBank
+    V = 30
+    b = GpuBank([_concurrent_voice(i) for i in range(V)], per_voice=True, sample_rate=SR)
+    assert len(b.classes()) == 2
+    us = _oracle_units([_concurrent_voice(i) for i in range(V)], SR)
+    g, _ = b.render_samples(640)
+    assert np.array_equal(g, np.stack([u.process_many(640) for u in us]))
+    c = b.clone()
+    for n in (1024, 320, 2048, 64, 128):
+        gb, _ = b.render_samples(n)
+        gc, _ = c.render_samples(n)
+        o = np.stack([u.process_many(n) for u in us])
+        assert np.array_equal(gb, o) and np.array_equal(gc, o), n
+
+
+def test_set_sample_rate_of_a_running_bank():
+    """AudioUnit::set_sample_rate on a bank that has rendered: the parameters are uploaded again and the next render reads them."""
+    from fundsp_b200.bank import GpuBank
+    V = 30
+    b = GpuBank([_concurrent_voice(i) for i in range(V)], per_voice=True, sample_rate=SR)
+    us = _oracle_units([_concurrent_voice(i) for i in range(V)], SR)
+    for sr, n in ((SR, 1024), (44100.0, 1536), (96000.0, 640)):
+        if sr != SR:
+            b.set_sample_rate(sr)
+            for u in us:
+                u.set_sample_rate(sr)
+        g, _ = b.render_samples(n)
+        o = np.stack([u.process_many(n) for u in us])
+        assert np.abs(o).max() > 1e-3 and np.array_equal(g, o), (sr, int((g != o).sum()))
+
+
 def test_mixed_bank_two_stage_and_plain_classes():
     """A bank holding a pipelined two-stage class (dry program + FDN kernel on a second stream) next to plain classes: per-voice
     rows stay bit-exact and the mix (cleared, then accumulated by every class) equals the f64 sum of the rows."""

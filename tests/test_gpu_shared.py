@@ -61,6 +61,37 @@ def test_two_shareds_many_voices_ragged_process_and_render():
         check_mix(mix, rows, classes, launch_segments(n, classes, BIG, 1, True, False), False, "render")
 
 
+def test_readers_change_before_every_call_and_device_renders_overlap():
+    """A Shared that changes before every call: process() calls, then render_device calls with no synchronise between them, so each call
+    stages its reader rows while the previous call may still run. Every voice bit for bit against the oracle units."""
+    s = shared(0.5)
+    V, K, n = 40, 6, 640
+    mk = lambda i: saw_voice(s, i)
+    bank = GpuBank([mk(i) for i in range(V)], per_voice=True, mix=False, sample_rate=SR)
+    us = units([mk(i) for i in range(V)])
+    for k, size in enumerate((64, 64, 17, 64, 1, 64)):
+        set_both(s, 0.1 * k - 0.2)
+        got = bank.process(size)
+        want = oracle_rows(us, size)
+        assert np.array_equal(got.reshape(want.shape), want), (k, size)
+    if MOCK:   # (device memory is host memory on the mock device)
+        buf = np.full((V, K * n), np.nan, dtype=np.float32)
+        ptr, fetch = buf.ctypes.data, lambda: buf
+    else:
+        import torch
+        dev = torch.full((V, K * n), float("nan"), dtype=torch.float32, device="cuda")
+        torch.cuda.synchronize()
+        ptr, fetch = dev.data_ptr(), lambda: dev.cpu().numpy()
+    want = []
+    for k in range(K):
+        set_both(s, 0.3 - 0.15 * k)
+        bank.render_device(n, out_ptr=ptr + 4 * k * n, out_stride=K * n, sync=False)
+        want.append(oracle_rows(us, n).reshape(V, n))
+    bank.sync()
+    got, want = fetch(), np.concatenate(want, axis=1)
+    assert np.array_equal(got, want), [k for k in range(K) if not np.array_equal(got[:, k * n:(k + 1) * n], want[:, k * n:(k + 1) * n])]
+
+
 def test_keys_pattern_var_follow_drives_a_cutoff():
     cut = shared(800.0)   # examples/keys.rs:171-178: var(&s) >> follow(0.01)
     mk = lambda i: (saw_hz(55.0 + 11.0 * i) | var(cut) >> follow(0.01) | dc(1.0)) >> lowpass()

@@ -182,6 +182,44 @@ def test_sequencer_bank_live_edit_and_push():
     assert b.push_event(event(voice(440.0), b.time() + 1.0, b.time() + 2.0)) in (0, 1)   # both saw voices have finished: a slot is reused
 
 
+def test_push_event_grows_a_bank_whose_render_is_still_running():
+    """A note-on that grows the bank right behind a render_device call nobody has synchronised: the running state is read back behind that
+    render. Per-voice rows bit for bit against a twin bank whose render was synchronised before the same push."""
+    import ctypes
+    from fundsp_b200.bank import GpuBank
+    from fundsp_b200.prelude import sine_hz
+    from fundsp_b200.sequencer import Sequencer, Fade, ReplayMode, event
+    from test_gpu_mix import MOCK
+    sr, n1, n2 = 44100.0, 64 * 30 + 5, 64 * 20 + 3
+
+    def build():
+        q = Sequencer(0, 1, ReplayMode.None_)
+        q.push(0.0, 10.0, Fade.Smooth, 0.001, 0.0, live_voice(110.0))
+        q.push(0.0, 10.0, Fade.Power, 0.002, 0.0, arp_voice(165.0))
+        return GpuBank.from_sequencer(q, per_voice=True, mix=True, sample_rate=sr)
+
+    a, b = build(), build()
+    rows = 2 * a.voice_outputs()
+    if MOCK:   # (device memory is host memory on the mock device)
+        out, mix = np.full((rows, n1), np.nan, np.float32), np.full((1, n1), np.nan, np.float32)
+        ptrs, fetch = (out.ctypes.data, mix.ctypes.data), lambda: (out, mix)
+    else:
+        import torch
+        out_d = torch.full((rows, n1), float("nan"), device="cuda"); mix_d = torch.full((1, n1), float("nan"), device="cuda")
+        torch.cuda.synchronize()
+        ptrs, fetch = (out_d.data_ptr(), mix_d.data_ptr()), lambda: (out_d.cpu().numpy(), mix_d.cpu().numpy())
+    a.render_device(n1, out_ptr=ptrs[0], out_stride=n1, mix_ptr=ptrs[1], mix_stride=n1, sync=False)
+    rb, mb = b.render_samples(n1)
+    t = b.time() + 0.001
+    assert a.push_event(event(sine_hz(500.0) * 0.5, t, t + 0.02, Fade.Power, 0.002, 0.002)) == 2
+    assert b.push_event(event(sine_hz(500.0) * 0.5, t, t + 0.02, Fade.Power, 0.002, 0.002)) == 2
+    ra, ma = fetch()
+    assert np.array_equal(ra, rb.reshape(ra.shape)) and np.array_equal(ma, mb)
+    ra2, ma2 = a.render_samples(n2)
+    rb2, mb2 = b.render_samples(n2)
+    assert np.abs(rb2).max() > 0.1 and np.array_equal(ra2, rb2) and np.array_equal(ma2, mb2)
+
+
 def test_gpu_sequencer_note_ons_while_running():
     """An arpeggio played live: every 1024 samples a note-on (push_relative) with a short fade, eight reserved voices that the notes
     cycle through as earlier notes finish; the oracle Sequencer receives the same calls at the same times."""

@@ -1,13 +1,16 @@
 """The HOST runtime (csrc/host/bank.cpp, graph.cpp, capi.cpp: class building, word layout, launch sequencing, mix reduction, process()
 path, settings on a live bank, sequencer clock / edit / push / growth in place, clone, reset ...) exercised WITHOUT a GPU.
 
-tests/cpp/mock/ builds the host sources against a stand-in <cuda_runtime.h> ("device" memory is host memory, calls are synchronous) and
-replaces the kernels by the device node library compiled for the CPU (FDSP_HOST_EMUL), one small shared object per graph class walking
-every voice through bank_kernel's per-thread block structure, and summing each CTA's partial mix in the association of the kernel's mix
-tile (so the exact mix model of tests/test_gpu_mix.py holds on the mock too). The whole GPU test-suite then runs against that library in a
-subprocess (FDSP_B200_LIB selects it there and only there). What this does NOT cover is the CUDA side proper — the shared-memory tile itself, TMA table
-staging, the warp-per-voice FDN kernel itself (the mock runs the equivalent generic reverb program on its argument block, so the host side of
-the two-stage classes IS covered), stream concurrency — which the same tests check on a B200.
+tests/cpp/mock/ builds the host sources against a stand-in <cuda_runtime.h> ("device" memory is host memory) and replaces the kernels by the
+device node library compiled for the CPU (FDSP_HOST_EMUL), one small shared object per graph class walking every voice through bank_kernel's
+per-thread block structure, and summing each CTA's partial mix in the association of the kernel's mix tile (so the exact mix model of
+tests/test_gpu_mix.py holds on the mock too). The mock device runs every stream's work as late as CUDA allows (FDSP_MOCK_SCHEDULE, `late` here),
+so a missing dependency between the bank's device operations changes a result (tests/test_mock_streams_cpu.py runs the suite again with the
+streams drained in reverse order). The whole GPU test-suite then runs against that library in a subprocess (FDSP_B200_LIB selects it there and
+only there). What this does NOT cover is the CUDA side proper — the shared-memory tile itself, TMA table staging, the warp-per-voice FDN kernel
+itself (the mock runs the equivalent generic reverb program on its argument block, so the host side of the two-stage classes IS covered), and
+the ordering of the paths the mock never takes (the resident process() kernel, the tensor-core convolver, NCCL) — which the same tests check on
+an H100.
 The mock is test infrastructure: it is never built into, or loaded by, the product."""
 import hashlib
 import os
@@ -32,6 +35,7 @@ def _tree_hash():
     return h.hexdigest()[:16]
 
 
+GPU_SUITE = ("test_gpu_jit.py", "test_gpu_conv.py", "test_gpu_parity.py", "test_gpu_wider.py", "test_gpu_mix.py", "test_gpu_wavetable.py", "test_gpu_shared.py")
 SAN = os.environ.get("FDSP_MOCK_SANITIZE", "")   # "address" or "undefined": build the mock device and every class module with that sanitizer
 
 
@@ -50,7 +54,7 @@ def mock_env():
         subprocess.check_call(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-w", "-shared", "-fPIC", "-DFDSP_HOST_EMUL=1", *san, "-I", MOCK, "-I", CSRC,
                                "-x", "c++", *srcs, "-o", lib + ".tmp", "-ldl"])
         os.replace(lib + ".tmp", lib)
-    env = dict(os.environ, FDSP_B200_LIB=lib, FDSP_MOCK_ROOT=ROOT, FDSP_MOCK_CACHE=os.path.join(build, "classes"))
+    env = dict(os.environ, FDSP_B200_LIB=lib, FDSP_MOCK_ROOT=ROOT, FDSP_MOCK_CACHE=os.path.join(build, "classes"), FDSP_MOCK_SCHEDULE="late")
     if SAN:   # every "device" buffer is a host allocation here, so the sanitizer sees each out-of-bounds word the GPU would silently read or write
         rt = subprocess.check_output(["gcc", "-print-file-name=lib" + ("asan" if SAN == "address" else "ubsan") + ".so"], text=True).strip()
         env.update(LD_PRELOAD=rt, ASAN_OPTIONS="detect_leaks=0", UBSAN_OPTIONS="halt_on_error=1",
@@ -58,13 +62,17 @@ def mock_env():
     return env
 
 
-def test_gpu_suite_runs_on_the_mock_device(mock_env):
-    files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_jit.py", "test_gpu_conv.py", "test_gpu_parity.py", "test_gpu_wider.py", "test_gpu_mix.py", "test_gpu_wavetable.py")]
+def run_gpu_suite(env):
+    files = [os.path.join(ROOT, "tests", f) for f in GPU_SUITE]
     r = subprocess.run([sys.executable, "-m", "pytest", *files, "-m", "gpu", "-q", "-n", "8", "-p", "no:cacheprovider", "--tb=short"],
-                       capture_output=True, text=True, env=mock_env, cwd=ROOT, timeout=3000)
+                       capture_output=True, text=True, env=env, cwd=ROOT, timeout=3000)
     tail = r.stdout[-3000:]
     assert r.returncode == 0, tail
     assert " passed" in tail and "failed" not in tail and "error" not in tail.lower(), tail
+
+
+def test_gpu_suite_runs_on_the_mock_device(mock_env):
+    run_gpu_suite(mock_env)
 
 
 def test_sharded_bank_on_the_mock_device(mock_env):
