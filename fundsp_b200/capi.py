@@ -59,6 +59,7 @@ _SIG = {
     "fdsp_shaper_adaptive": (P, [D, I, F, F]), "fdsp_nl_biquad_adaptive": (P, [I, I, D, I, F, F, I, F, F, F]),
     "fdsp_envelope_in": (P, [D, I, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
     "fdsp_envelope_text": (P, [D, I, C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
+    "fdsp_update": (P, [P, F, C.c_char_p, I, C.POINTER(C.c_char_p), FP]),
     "fdsp_pipe": (P, [P, P]), "fdsp_stack": (P, [P, P]), "fdsp_branch": (P, [P, P]), "fdsp_bus": (P, [P, P]), "fdsp_thru": (P, [P]),
     "fdsp_binop": (P, [I, P, P]), "fdsp_unop": (P, [I, F, P]), "fdsp_multi": (P, [I, I, I, C.POINTER(P)]), "fdsp_feedback": (P, [P, I]),
     "fdsp_net_new": (P, [I, I]), "fdsp_net_push": (I, [P, P]), "fdsp_net_connect": (I, [P, I, I, I, I]), "fdsp_net_connect_input": (I, [P, I, I, I]),
@@ -217,6 +218,7 @@ class GpuBackend:
     def b_shape_fn(self, text, caps): return _closure_node(self.L.fdsp_shape_fn(text.encode(), *_caps(caps)))
     def b_envelope_in(self, interval, text, nin, nout, caps): return _closure_node(self.L.fdsp_envelope_in(interval, nin, nout, text.encode(), *_caps(caps)))
     def b_envelope_text(self, interval, text, nout, caps): return _closure_node(self.L.fdsp_envelope_text(interval, nout, text.encode(), *_caps(caps)))
+    def b_update(self, dt, text, caps, x): return _closure_node(self.L.fdsp_update(x, dt, text.encode(), *_caps(caps)))
     def b_pipe(self, x, y): return _node(self.L.fdsp_pipe(x, y), "pipe")
     def b_stack(self, x, y): return _node(self.L.fdsp_stack(x, y), "stack")
     def b_branch(self, x, y): return _node(self.L.fdsp_branch(x, y), "branch")

@@ -151,6 +151,12 @@ API fdsp_node* fdsp_envelope_in(double interval, int inputs, int outputs, const 
 API fdsp_node* fdsp_envelope_text(double interval, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values) {
   return closure_node(CL_ENVELOPE, 0, outputs, interval, closure, ncaptures, names, values);
 }
+API fdsp_node* fdsp_update(fdsp_node* x, float dt, const char* closure, int ncaptures, const char* const* names, const float* values) {
+  std::string e;
+  HNode* n = mk_update(x ? take(x) : nullptr, dt, closure, ncaptures, names, values, e);
+  if (!n) { g_err = e; return nullptr; }
+  return wrap(n, "update");
+}
 API fdsp_node* fdsp_shaper_adaptive(double timescale, int inner_kind, float p0, float p1) {
   std::string e;
   HNode* n = mk_shaper_adaptive(timescale, inner_kind, p0, p1, e);

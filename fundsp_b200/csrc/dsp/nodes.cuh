@@ -2519,6 +2519,122 @@ template <int HAD, class X> struct WaveKind<Feedback<HAD, X>> : WaveKind<X> {};
 template <int HAD, class X, class Y> struct WaveKind<Feedback2<HAD, X, Y>> : Wk2<X, Y> {};
 
 
+// ---------------------------------------------------------------- System<X, F> (src/system.rs:47-97, ID 67): `update(x, dt, f)`
+// At the start of each of X's blocks (and before each tick) the update point test of System::process / tick: when due, the compiled
+// update function f(t, dt, x) (closure text, csrc/host/closure.cpp CL_UPDATE) gives the arguments of its `x.set(..)` statements; the host
+// resolved each statement to a target leaf of X (UpdTarget: its kind, the hops to it, which argument writes which of its set values). The
+// set values are state words; the target's coefficients are recomputed from them with the function its host set() uses (graph.cpp), so
+// the device's coefficients are the reference's bits. They are recomputed too when a launch loads the voice: its words hold the values
+// the host lowered, and the sample rate may have changed (FixedSvf::set_sample_rate recomputes from the last-set cutoff). Between update
+// points X runs its own block path, 8-sample groups included.
+template <int... H> struct UpdAt {};
+template <bool B, class T, class F> struct UpdSel { typedef T type; };
+template <class T, class F> struct UpdSel<false, T, F> { typedef F type; };
+template <class N, class P> struct UpdNav;   // the registers of the leaf at hops P inside N's
+template <class N> struct UpdNav<N, UpdAt<>> { typedef N T; static FDSP_DEV typename N::R& get(typename N::R& r) { return r; } };
+template <class X, class Y, int H, int... Hs> struct UpdNav2 {   // a binary combinator: hop 0 is X, 1 is Y
+  typedef typename UpdNav<typename UpdSel<H == 0, X, Y>::type, UpdAt<Hs...>>::T T;
+  template <class RR> static FDSP_DEV typename T::R& get(RR& r) {
+    if constexpr (H == 0) return UpdNav<X, UpdAt<Hs...>>::get(r.x); else return UpdNav<Y, UpdAt<Hs...>>::get(r.y);
+  }
+};
+template <class X, class Y, int H, int... Hs> struct UpdNav<Pipe<X, Y>, UpdAt<H, Hs...>> : UpdNav2<X, Y, H, Hs...> {};
+template <class X, class Y, int H, int... Hs> struct UpdNav<Stack<X, Y>, UpdAt<H, Hs...>> : UpdNav2<X, Y, H, Hs...> {};
+template <class X, class Y, int H, int... Hs> struct UpdNav<Branch<X, Y>, UpdAt<H, Hs...>> : UpdNav2<X, Y, H, Hs...> {};
+template <class X, class Y, int H, int... Hs> struct UpdNav<Bus<X, Y>, UpdAt<H, Hs...>> : UpdNav2<X, Y, H, Hs...> {};
+template <int K, class X, class Y, int H, int... Hs> struct UpdNav<Binop<K, X, Y>, UpdAt<H, Hs...>> : UpdNav2<X, Y, H, Hs...> {};
+template <class X, class P> struct UpdNav1 {   // Unop / Thru: the setting passes through
+  typedef typename UpdNav<X, P>::T T;
+  template <class RR> static FDSP_DEV typename T::R& get(RR& r) { return UpdNav<X, P>::get(r.x); }
+};
+template <int K, class X, int H, int... Hs> struct UpdNav<Unop<K, X>, UpdAt<H, Hs...>> : UpdNav1<X, UpdAt<Hs...>> {};
+template <class X, int H, int... Hs> struct UpdNav<Thru<X>, UpdAt<H, Hs...>> : UpdNav1<X, UpdAt<Hs...>> {};
+template <int KIND, int OP, int N, class X, int H, int... Hs> struct UpdNav<Multi<KIND, OP, N, X>, UpdAt<H, Hs...>> {
+  typedef typename UpdNav<X, UpdAt<Hs...>>::T T;
+  template <class RR> static FDSP_DEV typename T::R& get(RR& r) { return UpdNav<X, UpdAt<Hs...>>::get(r.x[H]); }
+};
+// KIND (graph.cpp SystemN): 0 FixedSvf<MODE>, 1 ButterLowpass, 3 Biquad, 4 Lowpole, 5 Highpole, 6 DCBlock, 7 Constant, 8 Panner<U1> (a
+// Resonator, 2, takes no setting and is never a target); its set values are sv[OFF..): (cutoff, q, gain), (cutoff), (a1, a2, b0, b1, b2),
+// (cutoff), (cutoff), (cutoff), (value), (pan).
+// Ak: the update's argument that writes value k (-1: none does).
+template <int KIND, int MODE, int OFF, int A0, int A1, int A2, int A3, int A4, class P> struct UpdTarget {
+  static FDSP_DEV void take(float* sv, const float* a) {
+    if (A0 >= 0) sv[OFF] = a[A0 < 0 ? 0 : A0];
+    if (A1 >= 0) sv[OFF + 1] = a[A1 < 0 ? 0 : A1];
+    if (A2 >= 0) sv[OFF + 2] = a[A2 < 0 ? 0 : A2];
+    if (A3 >= 0) sv[OFF + 3] = a[A3 < 0 ? 0 : A3];
+    if (A4 >= 0) sv[OFF + 4] = a[A4 < 0 ? 0 : A4];
+  }
+  template <class X> static FDSP_DEV void apply(typename X::R& xr, const float* sv, float sr) {
+    typedef typename UpdNav<X, P>::T T;
+    auto& r = UpdNav<X, P>::get(xr);
+    const float* v = sv + OFF;
+    if constexpr (KIND == 0) { const SvfCoefs k = svf_coefs<MODE>(sr, v[0], v[1], v[2]); r.a1 = k.a1; r.a2 = k.a2; r.a3 = k.a3; r.m0 = k.m0; r.m1 = k.m1; r.m2 = k.m2; }
+    else if constexpr (KIND == 1) { const BqCoefs k = bq_butter_lowpass(sr, v[0]); r.a1 = k.a1; r.a2 = k.a2; r.b0 = k.b0; r.b1 = k.b1; r.b2 = k.b2; }
+    else if constexpr (KIND == 3) { r.a1 = v[0]; r.a2 = v[1]; r.b0 = v[2]; r.b1 = v[3]; r.b2 = v[4]; }
+    else if constexpr (KIND == 4 || KIND == 5) r.coeff = m::expf_(-TAU_F * v[0] / sr);
+    else if constexpr (KIND == 6) r.coeff = 1.0f - TAU_F / sr * v[0];
+    else if constexpr (KIND == 7) { for (int c = 0; c < T::OUT; c++) r.v[c] = v[0]; }
+    else pan_weights(v[0], r.lw, r.rw);
+  }
+};
+template <class... Tg> struct UpdTargets {
+  static FDSP_DEV void take(float* sv, const float* a) { (Tg::take(sv, a), ...); }
+  template <class X> static FDSP_DEV void apply(typename X::R& xr, const float* sv, float sr) { (Tg::template apply<X>(xr, sv, sr), ...); }
+};
+template <class E> struct UpdArity;
+template <class... Es> struct UpdArity<Ex::Out<Es...>> { static constexpr int value = sizeof...(Es); };
+template <class A, class B> struct UpdArity<Ex::Let<A, B>> : UpdArity<B> {};
+
+template <class X, int NSV, int NC, class E, class TG> struct System {
+  static constexpr int NA = UpdArity<E>::value;
+  FDSP_NODE(X::IN, X::OUT, 1 + NC + X::NP, 2 + NSV + X::NS, X::NU);
+  struct R { float interval, time, dtime; float c[NC > 0 ? NC : 1]; float sv[NSV > 0 ? NSV : 1]; bool fresh; typename X::R x; };
+  static FDSP_DEV void load(R& r, Loader& l) {
+    r.interval = l.Pf();
+#pragma unroll
+    for (int k = 0; k < NC; k++) r.c[k] = l.Pf();
+    r.time = l.Sf(); r.dtime = l.Sf();
+#pragma unroll
+    for (int k = 0; k < NSV; k++) r.sv[k] = l.Sf();
+    r.fresh = true;
+    X::load(r.x, l);
+  }
+  static FDSP_DEV void save(const R& r, Saver& s) {
+    s.Sf(r.time); s.Sf(r.dtime);
+#pragma unroll
+    for (int k = 0; k < NSV; k++) s.Sf(r.sv[k]);
+    X::save(r.x, s);
+  }
+  // the update point test and the clock (process :74-84 with delta_now = size / sample_rate, tick :61-72 with 1 / sample_rate); the
+  // process form's `size > 0` always holds here, since the device runs no empty block
+  static FDSP_DEV void advance(R& r, float sr, float delta_now) {
+    if (r.fresh) { TG::template apply<X>(r.x, r.sv, sr); r.fresh = false; }
+    if (r.dtime >= r.interval || r.time == 0.0f) {
+      const float t[2] = {r.time, r.dtime};
+      float a[NA];
+      const Ex::Root s{t, r.c, 0.0f};
+      Ex::Emit<E>::out(s, a);
+      TG::take(r.sv, a);
+      TG::template apply<X>(r.x, r.sv, sr);
+      r.dtime = 0.0f;
+    }
+    r.time += delta_now;
+    r.dtime += delta_now;
+  }
+  template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<X::IN>& in, Fr<X::OUT>& o) {
+    if (T) advance(r, c.sr, 1.0f / c.sr);
+    else if (c.i == 0) advance(r, c.sr, (float)c.n / c.sr);
+    X::template step<T>(r.x, c, in, o);
+  }
+  typedef void GroupStep;
+  template <class C> static FDSP_DEV void step8(R& r, C& c, const Fr8<X::IN>& in, Fr8<X::OUT>& o) {
+    if (c.i == 0) advance(r, c.sr, (float)c.n / c.sr);
+    group_step<X>(r.x, c, in, o);
+  }
+  static FDSP_DEV void end_simd(R& r) { X::end_simd(r.x); }
+};
+
 // Rough per-sample instruction cost of a graph type: picks how far the 8-sample group is unrolled (big bodies
 // thrash the instruction cache when only one warp runs per scheduler).
 template <class G> struct Cost { static constexpr int value = 8; };
@@ -2544,6 +2660,8 @@ template <int NC, class E> struct Cost<ShaperFn<NC, E>> { static constexpr int v
 template <int NO, int NC, class E> struct Cost<VarFn<NO, NC, E>> { static constexpr int value = NO; };
 template <int NI, int NO, int NC, class E> struct Cost<EnvelopeInFn<NI, NO, NC, E>> { static constexpr int value = 120; };
 template <int NO, int NC, class E> struct Cost<EnvelopeFn<NO, NC, E>> { static constexpr int value = 120; };
+template <class X, int NSV, int NC, class E, class TG> struct Cost<System<X, NSV, NC, E, TG>> { static constexpr int value = Cost<X>::value + 4; };
+template <class X, int NSV, int NC, class E, class TG> struct WaveKind<System<X, NSV, NC, E, TG>> : WaveKind<X> {};
 template <> struct Cost<Delay> { static constexpr int value = 12; };
 template <int N> struct Cost<Panner<N>> { static constexpr int value = N == 1 ? 2 : 80; };
 template <int K, class X, class Y> struct Cost<Binop<K, X, Y>> { static constexpr int value = Cost<X>::value + Cost<Y>::value + 1; };
@@ -2790,6 +2908,7 @@ template <int KIND, int OP, int N, class X> struct GroupPlan<Multi<KIND, OP, N, 
 
 template <class X> struct GroupPlan<Slot<X>> { static constexpr bool ok = GroupPlan<X>::ok; static constexpr int code = GroupPlan<X>::code + 16; };
 template <class X, class Y> struct GroupPlan<Xfade<X, Y>> { static constexpr bool ok = GroupPlan<X>::ok && GroupPlan<Y>::ok; static constexpr int code = GroupPlan<X>::code + GroupPlan<Y>::code + 16; };
+template <class X, int NSV, int NC, class E, class TG> struct GroupPlan<System<X, NSV, NC, E, TG>> { static constexpr bool ok = GroupPlan<X>::ok; static constexpr int code = GroupPlan<X>::code + 4; };
 template <class X> struct GroupPlan<Event<X>> { static constexpr bool ok = GroupPlan<X>::ok; static constexpr int code = GroupPlan<X>::code + 24; };
 template <int NIN, int NOUT, class... V, class OS> struct GroupPlan<Dag<NIN, NOUT, VList<V...>, OS>> {
   static constexpr bool ok = (true && ... && GroupPlan<typename V::Unit>::ok);

@@ -305,9 +305,13 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
     if (l.U != c.uniform || l.P.size() != c.np || l.S.size() != c.ns)
       return "#U set: the setting changes a class-uniform word (a delay length); rebuild the bank instead";
     TRY(sh_check(voice, l.shared));
-    // parameters take effect at once (one strided column of the [NP][V] block); running state is left alone, the
+    // parameters take effect at once (one strided column of the [NP][V] block); running state is left alone (below), the
     // construction-time state (what reset() restores) follows the setting like the reference's stored phase/seed
     if (c.np) CU(cudaMemcpy2DAsync(c.d_params + i, (size_t)Vc * 4, l.P.data(), 4, 4, c.np, cudaMemcpyHostToDevice, stream));
+    // ... except the state words the setting itself wrote (the values a System's update function also sets): they hold from now on
+    for (auto& w : l.liveS)
+      if (w.second > w.first && w.second <= c.ns)
+        CU(cudaMemcpy2DAsync(c.d_state + (size_t)w.first * Vc + i, (size_t)Vc * 4, l.S.data() + w.first, 4, 4, w.second - w.first, cudaMemcpyHostToDevice, stream));
     CU(cudaStreamSynchronize(stream));  // `l` is pageable and goes out of scope
     const std::vector<uint32_t> S0 = l.reset_image();
     for (uint32_t k = 0; k < c.ns; k++) c.state0[(size_t)k * Vc + i] = S0[k];

@@ -100,7 +100,12 @@ const char* NOT_RESTATED[] = {"log", "log2", "log10", "exp2", "atan", "xerp", "x
 const char* KEYWORDS[] = {"as", "for", "while", "loop", "return", "mut", "match", "fn", "break", "continue", "in", "true", "false",
                           "self", "struct", "impl", "unsafe", "ref", "static", "const", "else", "let", "if", "move"};
 
-enum PKind { PK_TIME, PK_FRAME, PK_SCALAR, PK_FRAME_OR_SCALAR };
+enum PKind { PK_TIME, PK_FRAME, PK_SCALAR, PK_FRAME_OR_SCALAR, PK_NODE };   // PK_NODE: update's node parameter, the receiver of `.set(..)`
+
+// the settings an update function may make (src/setting.rs:130-170), numbered as the C ABI's (include/fundsp_b200.h)
+struct SettingKind { const char* name; int kind, nargs; };
+const SettingKind UPDATE_SETTINGS[] = {{"center", 1, 1}, {"center_q", 2, 2}, {"center_q_gain", 3, 3}, {"value", 4, 1}, {"biquad", 6, 5}, {"pan", 11, 1}};
+constexpr int MAX_ADDRESS = 6;   // Setting's ArrayVec<[Address; 6]>
 struct Param { std::string name; PKind kind; int index; };
 
 struct Parser {
@@ -281,6 +286,7 @@ struct Parser {
       return V{std::string(lets[i].second == BOOL ? "Ex::BVar<" : "Ex::Var<") + std::to_string(idx) + ">", lets[i].second, 0};
     }
     if (const Param* q = param(k.s)) {
+      if (q->kind == PK_NODE) fail_at(k, "the node parameter can only be the receiver of `.set(..)`");
       if (q->kind == PK_TIME) return V{"Ex::T", F32, 0};
       if (q->kind == PK_SCALAR) return V{"Ex::In<" + std::to_string(q->index) + ">", F32, 0};
       if (is("[")) {
@@ -312,25 +318,25 @@ struct Parser {
     if (a.ty != b.ty || a.n != b.n) fail_at(k, "the arms of `if` have different types");
     return V{"Ex::If<" + c.s + "," + a.s + "," + b.s + ">", a.ty, a.n};
   }
+  void let_(std::vector<std::string>& vals) {   // after `let`
+    if (is_id("mut")) fail_at(cur(), "mutation is not supported");
+    const Tok n = cur();
+    if (n.k != T_ID || keyword(n.s)) fail_at(n, "expected a name");
+    p++;
+    if (is(":")) { p++; skip_type(); }
+    expect("=");
+    const Tok at = cur();
+    V v = expr();
+    if (v.ty == TUPLE) fail_at(at, "a tuple can only be the closure's value");
+    expect(";");
+    vals.push_back(v.s);
+    lets.push_back({n.s, v.ty});
+  }
   V block() {
     expect("{");
     std::vector<std::string> vals;
     const size_t depth = lets.size();
-    while (is_id("let")) {
-      p++;
-      if (is_id("mut")) fail_at(cur(), "mutation is not supported");
-      const Tok n = cur();
-      if (n.k != T_ID || keyword(n.s)) fail_at(n, "expected a name");
-      p++;
-      if (is(":")) { p++; skip_type(); }
-      expect("=");
-      const Tok at = cur();
-      V v = expr();
-      if (v.ty == TUPLE) fail_at(at, "a tuple can only be the closure's value");
-      expect(";");
-      vals.push_back(v.s);
-      lets.push_back({n.s, v.ty});
-    }
+    while (is_id("let")) { p++; let_(vals); }
     const Tok at = cur();
     V body = expr();
     if (is(";")) fail_at(cur(), "only `let` statements are allowed; the block ends with its value");
@@ -339,6 +345,65 @@ struct Parser {
     for (size_t i = vals.size(); i-- > 0;) body.s = "Ex::Let<" + vals[i] + "," + body.s + ">";
     lets.resize(depth);
     return body;
+  }
+  // update's body: `x.set(Setting::kind(args)[.left() | .right() | .index(N)]*)` statements after any `let`s, in braces or alone. Every
+  // argument of every statement is one value of the tuple the body evaluates to, so the lets are evaluated once per update.
+  V update_body(std::vector<UpdateSet>& sets) {
+    const bool braces = is("{");
+    if (braces) p++;
+    std::vector<std::string> vals, argv;
+    auto at_end = [&]() { return braces ? is("}") : cur().k == T_END; };
+    while (!at_end()) {
+      if (is_id("let")) {
+        if (!sets.empty()) fail_at(cur(), "a `let` after a `set` is not supported; put the `let`s first");
+        p++; let_(vals); continue;
+      }
+      if (is_id("if")) fail_at(cur(), "a `set` inside an `if` is not supported; put the `if` inside the setting's arguments");
+      const Tok r = cur();
+      const Param* q = r.k == T_ID ? param(r.s) : nullptr;
+      if (!q || q->kind != PK_NODE) fail_at(r, "expected `let` or a `.set(..)` of the node parameter");
+      p++; expect(".");
+      if (!is_id("set")) fail_at(cur(), "only `.set(..)` can be called on the node parameter");
+      p++; expect("(");
+      if (!is_id("Setting")) fail_at(cur(), "expected `Setting::..`");
+      p++; expect("::");
+      const Tok kt = cur();
+      const SettingKind* sk = nullptr;
+      for (const SettingKind& x : UPDATE_SETTINGS) if (kt.k == T_ID && kt.s == x.name) sk = &x;
+      if (!sk) fail_at(kt, "setting not supported in an update function (center, center_q, center_q_gain, value, pan, biquad)");
+      p++; expect("(");
+      std::vector<V> a = args();
+      if ((int)a.size() != sk->nargs)
+        fail_at(kt, "takes " + std::to_string(sk->nargs) + " argument" + (sk->nargs == 1 ? "" : "s") + ", given " + std::to_string(a.size()));
+      UpdateSet st{sk->kind, (int)argv.size(), sk->nargs, r.col, {}};
+      for (const V& v : a) argv.push_back(v.s);
+      while (is(".")) {
+        p++;
+        const Tok m = cur();
+        if (m.k == T_ID && (m.s == "left" || m.s == "right")) { p++; expect("("); expect(")"); st.address.push_back(m.s == "left" ? 0 : 1); }
+        else if (m.k == T_ID && m.s == "index") {
+          p++; expect("(");
+          const Tok ix = cur();
+          if (ix.k != T_INT) fail_at(ix, "`.index()` takes an integer literal");
+          p++; expect(")");
+          st.address.push_back(strtoull(ix.s.c_str(), nullptr, 10));
+        } else if (m.k == T_ID && m.s == "node") fail_at(m, "`.node()` addressing is not supported in an update function");
+        else fail_at(m, "expected `.left()`, `.right()` or `.index(N)`");
+        if ((int)st.address.size() > MAX_ADDRESS) fail_at(m, "an address has at most " + std::to_string(MAX_ADDRESS) + " steps");
+      }
+      expect(")");
+      op();
+      sets.push_back(std::move(st));
+      if (is(";")) { p++; continue; }
+      if (!at_end()) fail_at(cur(), "expected `;`");
+    }
+    if (sets.empty()) fail_at(cur(), "the update function sets nothing; it needs at least one `.set(..)` of the node parameter");
+    if (braces) p++;
+    std::string body = "Ex::Out<";
+    for (size_t i = 0; i < argv.size(); i++) body += (i ? "," : "") + argv[i];
+    body += ">";
+    for (size_t i = vals.size(); i-- > 0;) body = "Ex::Let<" + vals[i] + "," + body + ">";
+    return V{body, TUPLE, (int)argv.size()};
   }
   void skip_type() {   // a type annotation, ignored: tokens up to `,` or `|` outside brackets
     int depth = 0;
@@ -392,6 +457,9 @@ std::string parse_closure(const char* text, ClosureKind kind, int inputs, int ou
     } else if (kind == CL_ENVELOPE) {
       if (np != 1) return arity("envelope takes one time parameter |t|");
       ps.params.push_back({names[0], PK_TIME, 0});
+    } else if (kind == CL_UPDATE) {
+      if (np != 3) return arity("update takes |t, dt, x|");
+      ps.params.push_back({names[0], PK_SCALAR, 0}); ps.params.push_back({names[1], PK_SCALAR, 1}); ps.params.push_back({names[2], PK_NODE, 0});
     } else {
       if (np == 2 && inputs != 1) { ps.params.push_back({names[0], PK_TIME, 0}); ps.params.push_back({names[1], PK_FRAME, 0}); }
       else if (np == 2 && inputs == 1) { ps.params.push_back({names[0], PK_TIME, 0}); ps.params.push_back({names[1], PK_FRAME_OR_SCALAR, 0}); }
@@ -401,6 +469,13 @@ std::string parse_closure(const char* text, ClosureKind kind, int inputs, int ou
     for (size_t i = 0; i < names.size(); i++)
       for (size_t j = 0; j < i; j++) if (names[i] == names[j]) return "parameter `" + names[i] + "` appears twice";
     const Tok at = ps.cur();
+    if (kind == CL_UPDATE) {
+      V body = ps.update_body(out.sets);
+      if (ps.cur().k != T_END) fail_at(ps.cur(), "");
+      out.expr = body.s;
+      out.caps = ps.caps;
+      return "";
+    }
     V body = ps.expr();
     if (ps.cur().k != T_END) fail_at(ps.cur(), "");
     if (body.ty == BOOL) fail_at(at, "the closure's value is a bool; it must be f32 or a tuple of f32");

@@ -1092,6 +1092,164 @@ struct Multi : HNode {  // MultiBus 28, MultiStack 30, Reduce 31, MultiBranch 33
   HCLONE(Multi)
 };
 
+// ---------------------------------------------------------------- System<X, F> (src/system.rs, ID 67): `update(x, dt, f)`
+// f is closure text (closure.cpp, CL_UPDATE) whose `x.set(..)` statements are resolved here, once, to the leaves of X they reach, by
+// the rules of the combinators' `set` above (Index peels one step into a binary or Multi combinator; Unop and Thru pass the setting on).
+// A reached leaf is a target when the device can recompute its coefficients as its host `set` does (nodes.cuh System); a setting the leaf
+// ignores is ignored. The values each target was last set to are STATE words of the System (they survive launches, reset and clone,
+// and set_sample_rate recomputes the coefficients from them); dt and the captures are parameter words.
+struct SystemN : HNode {
+  // target kinds (nodes.cuh UpdTarget): 0 FixedSvf, 1 ButterLowpass, 2 Resonator (reached, but it takes no setting), 3 Biquad, 4 Lowpole, 5 Highpole, 6 DCBlock, 7 Constant, 8 Panner<U1>
+  struct Target { int kind, mode; std::vector<int> hops; uint32_t off; int nsv; int arg[5]; };
+  Kid x; float interval; std::string expr; std::vector<float> caps; std::vector<UpdateSet> sets;
+  std::vector<Target> tg; uint32_t nsv = 0; std::string refused;
+  std::vector<std::pair<uint32_t, uint32_t>> pending;   // set-value words a set() has just written (relative to the first); a copy starts with none
+  SystemN(HNode* x_, float dt, std::string e, std::vector<float> c, std::vector<UpdateSet> st) : x(x_), interval(dt), expr(std::move(e)), caps(std::move(c)), sets(std::move(st)) {
+    for (const UpdateSet& u : sets) {
+      Setting s; s.kind = u.kind;
+      for (uint64_t a : u.address) s.address.push_back({1, a});
+      std::vector<int> hops; std::string why;
+      HNode* n = reach(s, hops);
+      if (!n) continue;                                                    // the address leads nowhere: the reference ignores the setting
+      int kind = -1, mode = 0, n_sv = 0;
+      if (!classify(n, &kind, &mode, &n_sv)) {
+        if (ignores(n, s)) continue;                                       // e.g. a center reaching an oscillator
+        if (refused.empty()) {
+          std::string g; n->sig(g);
+          refused = "update: Setting::" + std::string(setting_name(u.kind)) + " at column " + std::to_string(u.col) + " reaches " + g.substr(0, 80) + " (ID " +
+                    std::to_string(n->id()) + "), which an update function cannot set on the device (its targets: FixedSvf, the fixed ButterLowpass / Biquad, "
+                    "the fixed one-poles, Constant and Panner<U1>)";
+        }
+        continue;
+      }
+      int slots[5];
+      if (!accepts(kind, u.kind, slots)) continue;                         // a setting the target ignores
+      Target* t = nullptr;
+      for (Target& q : tg) if (q.hops == hops) t = &q;
+      if (!t) { tg.push_back(Target{kind, mode, hops, nsv, n_sv, {-1, -1, -1, -1, -1}}); t = &tg.back(); nsv += (uint32_t)n_sv; }
+      for (int k = 0; k < u.nargs; k++) if (slots[k] >= 0) t->arg[slots[k]] = u.arg + k;   // the last statement to write a value wins
+    }
+    ctor_ping();   // System::new: the inner node is pinged from AttoHash::new(67) through System::ping (src/system.rs:27-39)
+  }
+  SystemN(const SystemN& o) : HNode(o), x(o.x), interval(o.interval), expr(o.expr), caps(o.caps), sets(o.sets), tg(o.tg), nsv(o.nsv), refused(o.refused) {}
+  // where the setting goes inside X, as the combinators' set() route it; `hops`: the child taken at each step (nodes.cuh UpdAt)
+  HNode* reach(Setting s, std::vector<int>& hops) const {
+    HNode* n = x.p.get();
+    for (;;) {
+      const Address d = s.direction();
+      if (Binary* b = dynamic_cast<Binary*>(n)) {
+        if (d.type != 1 || d.value > 1) return nullptr;
+        hops.push_back((int)d.value); n = d.value == 0 ? b->x.p.get() : b->y.p.get(); s = s.peel();
+      } else if (Unary* u = dynamic_cast<Unary*>(n)) {
+        if (u->k == Unary::FEEDBACK) return nullptr;
+        hops.push_back(0); n = u->x.p.get();
+      } else if (Multi* m = dynamic_cast<Multi*>(n)) {
+        if (d.type != 1 || d.value >= m->x.size()) return nullptr;
+        hops.push_back((int)d.value); n = m->x[d.value].p.get(); s = s.peel();
+      } else return n;
+    }
+  }
+  static const char* setting_name(int kind) {
+    switch (kind) { case P_CENTER: return "center"; case P_CENTER_Q: return "center_q"; case P_CENTER_Q_GAIN: return "center_q_gain";
+      case P_VALUE: return "value"; case P_BIQUAD: return "biquad"; default: return "pan"; }
+  }
+  // a leaf that is not a target but whose set() leaves every word it lowers as it was ignores the setting, as the reference's node does
+  static bool ignores(const HNode* n, Setting s) {
+    std::unique_ptr<HNode> c(n->clone());
+    for (float& v : s.v) v = 1234.5f;
+    s.address.clear();
+    Lowering a, b;
+    c->lower(a); c->set(s); c->lower(b);
+    return a.ok && b.ok && a.P == b.P && a.S == b.S && a.U == b.U;
+  }
+  static bool classify(HNode* n, int* kind, int* mode, int* n_sv) {
+    if (Svf* f = dynamic_cast<Svf*>(n)) { if (!f->fixed) return false; *kind = 0; *mode = f->mode; *n_sv = 3; return true; }
+    if (Biquad* b = dynamic_cast<Biquad*>(n)) {
+      if (b->nin != 1) return false;
+      *kind = b->kind == 1 ? 1 : (b->kind == 2 ? 2 : 3); *n_sv = b->kind == 1 ? 1 : (b->kind == 2 ? 0 : 5); return true;
+    }
+    if (OnePoleN* o = dynamic_cast<OnePoleN*>(n)) {
+      if (o->nin != 1 || !(o->kind == 0 || o->kind == 1 || o->kind == 3)) return false;
+      *kind = o->kind == 0 ? 4 : (o->kind == 1 ? 5 : 6); *n_sv = 1; return true;
+    }
+    if (dynamic_cast<Constant*>(n)) { *kind = 7; *n_sv = 1; return true; }
+    if (Panner* p = dynamic_cast<Panner*>(n)) { if (p->nin != 1) return false; *kind = 8; *n_sv = 1; return true; }
+    return false;
+  }
+  // the set values a setting of `setting` kind writes on a target of `kind`: slots[k] for its k-th argument (-1: unused); false: ignored
+  static bool accepts(int kind, int setting, int* slots) {
+    for (int k = 0; k < 5; k++) slots[k] = -1;
+    const int n = kind == 0 ? (setting == P_CENTER ? 1 : setting == P_CENTER_Q ? 2 : setting == P_CENTER_Q_GAIN ? 3 : 0)   // FixedSvf::set (src/svf.rs)
+                : kind == 1 ? (setting == P_CENTER ? 1 : 0)
+                : kind == 2 ? 0                                    // Resonator has no set(): AudioNode's default ignores every setting (src/biquad.rs:340-387)
+                : kind == 3 ? (setting == P_BIQUAD ? 5 : 0)
+                : kind <= 6 ? (setting == P_CENTER ? 1 : 0)
+                : kind == 7 ? (setting == P_VALUE ? 1 : 0)
+                : (setting == P_PAN ? 1 : 0);
+    for (int k = 0; k < n; k++) slots[k] = k;
+    return n > 0;
+  }
+  HNode* at(const std::vector<int>& hops) const {
+    HNode* n = x.p.get();
+    for (int h : hops) {
+      if (Binary* b = dynamic_cast<Binary*>(n)) n = h == 0 ? b->x.p.get() : b->y.p.get();
+      else if (Unary* u = dynamic_cast<Unary*>(n)) n = u->x.p.get();
+      else n = static_cast<Multi*>(n)->x[h].p.get();
+    }
+    return n;
+  }
+  // the target's current set values, as its host node holds them
+  void values(const Target& t, float* v) const {
+    HNode* n = at(t.hops);
+    switch (t.kind) {
+      case 0: { Svf* f = static_cast<Svf*>(n); v[0] = f->cutoff; v[1] = f->q; v[2] = f->gain; break; }
+      case 1: v[0] = static_cast<Biquad*>(n)->f; break;
+      case 3: { const BqCoefs& c = static_cast<Biquad*>(n)->c; v[0] = c.a1; v[1] = c.a2; v[2] = c.b0; v[3] = c.b1; v[4] = c.b2; break; }
+      case 4: case 5: case 6: v[0] = static_cast<OnePoleN*>(n)->param; break;
+      case 7: v[0] = static_cast<Constant*>(n)->v[0]; break;
+      default: v[0] = static_cast<Panner*>(n)->value; break;
+    }
+  }
+  int inputs() const override { return x->inputs(); } int outputs() const override { return x->outputs(); }
+  uint64_t id() const override { return 67; }
+  void reset() override { x->reset(); }
+  void set_sample_rate(double s) override { x->set_sample_rate(s); }
+  void set(const Setting& s) override {   // System::set forwards to x; the values it writes on a target are the target's state words too
+    x->set(s);
+    std::vector<int> hops;
+    if (!reach(s, hops)) return;
+    int slots[5];
+    for (const Target& t : tg)
+      if (t.hops == hops && accepts(t.kind, s.kind, slots))
+        for (int k = 0; k < 5; k++) if (slots[k] >= 0) pending.emplace_back(t.off + (uint32_t)slots[k], t.off + (uint32_t)slots[k] + 1u);
+  }
+  AttoHash ping(bool probe, AttoHash h) override { return x->ping(probe, h.hash(id())); }
+  void sig(std::string& o) const override {
+    o += "System<"; x->sig(o);
+    o += "," + I((int)nsv) + "," + I((int)caps.size()) + "," + expr + ",UpdTargets<";
+    for (size_t i = 0; i < tg.size(); i++) {
+      const Target& t = tg[i];
+      o += std::string(i ? "," : "") + "UpdTarget<" + I(t.kind) + "," + I(t.mode) + "," + I((int)t.off);
+      for (int k = 0; k < 5; k++) o += "," + I(t.arg[k]);
+      o += ",UpdAt<";
+      for (size_t j = 0; j < t.hops.size(); j++) o += (j ? "," : "") + I(t.hops[j]);
+      o += ">>";
+    }
+    o += ">>";
+  }
+  HCLONE(SystemN)
+  void lower(Lowering& l) const override {
+    if (!refused.empty()) { l.fail(refused); return; }
+    l.p(interval); for (float c : caps) l.p(c);
+    l.s(0.0f); l.s(0.0f);                                   // time, delta_time
+    const uint32_t s0 = (uint32_t)l.S.size();
+    for (const Target& t : tg) { float v[5]; values(t, v); for (int k = 0; k < t.nsv; k++) l.s(v[k]); }
+    l.keepS.emplace_back(s0, (uint32_t)l.S.size());        // a target's reset leaves its settings alone (e.g. FixedSvf::reset)
+    for (auto& w : pending) l.liveS.emplace_back(s0 + w.first, s0 + w.second);
+    x->lower(l);
+  }
+};
+
 // ---------------------------------------------------------------- Net (src/net.rs, src/vertex.rs)
 struct NetPort { int type; int node; int port; };  // 0 Zero, 1 Global(port), 2 Local(node, port)
 struct HNet : HNode {
@@ -1447,6 +1605,24 @@ HNode* mk_feedback2(HNode* x, HNode* y, int hadamard) {
 HNode* mk_pan(float value) { return new Panner(value, 1); }
 HNode* mk_panner() { return new Panner(0.0f, 2); }
 HNode* mk_adsr_live(float a, float d, float s, float r) { return new AdsrLive(a, d, s, r); }
+// the captured values in Cap<k> order from (name, value) pairs; "" or the reason
+static std::string bind_captures(const Closure& c, int ncaptures, const char* const* names, const float* values, std::vector<float>& v) {
+  v.assign(c.caps.size(), 0.0f);
+  for (size_t k = 0; k < c.caps.size(); k++) {
+    int found = -1;
+    for (int j = 0; j < ncaptures; j++) if (names[j] && c.caps[k] == names[j]) found = j;
+    if (found < 0) return "`" + c.caps[k] + "` is neither a parameter nor a captured value: pass its value as a capture";
+    v[k] = values[found];
+  }
+  for (int j = 0; j < ncaptures; j++) {
+    if (!names[j]) return "null capture name";
+    bool used = false;
+    for (const std::string& n : c.caps) used = used || n == names[j];
+    if (!used) return std::string("capture `") + names[j] + "` does not occur in the closure";
+    for (int i = 0; i < j; i++) if (names[i] && strcmp(names[i], names[j]) == 0) return std::string("capture `") + names[j] + "` is given twice";
+  }
+  return "";
+}
 static HNode* mk_closure_of(SharedCell* cell, int kind, int inputs, int outputs, double interval, const char* text, int ncaptures,
                             const char* const* names, const float* values, std::string& err) {
   const char* what = kind == CL_MAP ? "map" : (kind == CL_SHAPE_FN ? "shape_fn" : (kind == CL_VAR_FN ? "var_fn" : (kind == CL_ENVELOPE ? "envelope" : "envelope_in")));
@@ -1458,20 +1634,9 @@ static HNode* mk_closure_of(SharedCell* cell, int kind, int inputs, int outputs,
   Closure c;
   const std::string e = parse_closure(text, (ClosureKind)kind, inputs, outputs, c);
   if (!e.empty()) return bad(e);
-  std::vector<float> v(c.caps.size());
-  for (size_t k = 0; k < c.caps.size(); k++) {
-    int found = -1;
-    for (int j = 0; j < ncaptures; j++) if (names[j] && c.caps[k] == names[j]) found = j;
-    if (found < 0) return bad("`" + c.caps[k] + "` is neither a parameter nor a captured value: pass its value as a capture");
-    v[k] = values[found];
-  }
-  for (int j = 0; j < ncaptures; j++) {
-    if (!names[j]) return bad("null capture name");
-    bool used = false;
-    for (const std::string& n : c.caps) used = used || n == names[j];
-    if (!used) return bad(std::string("capture `") + names[j] + "` does not occur in the closure");
-    for (int i = 0; i < j; i++) if (names[i] && strcmp(names[i], names[j]) == 0) return bad(std::string("capture `") + names[j] + "` is given twice");
-  }
+  std::vector<float> v;
+  const std::string ce = bind_captures(c, ncaptures, names, values, v);
+  if (!ce.empty()) return bad(ce);
   if (kind == CL_VAR_FN) return new VarFnN(cell, outputs, c.expr, std::move(v));
   ClosureN* n = new ClosureN((ClosureKind)kind, kind == CL_SHAPE_FN ? 1 : inputs, kind == CL_SHAPE_FN ? 1 : outputs, c.expr, std::move(v));
   n->interval = (float)interval;   // Envelope<f32> / EnvelopeIn<f32>: F::from_f32 / the f32 interval of prelude32 (src/prelude32.rs:581-724)
@@ -1481,6 +1646,17 @@ HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char
                   std::string& err) {
   if (kind == CL_VAR_FN) { err = "closure: bad kind"; return nullptr; }
   return mk_closure_of(nullptr, kind, inputs, outputs, interval, text, ncaptures, names, values, err);
+}
+HNode* mk_update(HNode* x, float dt, const char* text, int ncaptures, const char* const* names, const float* values, std::string& err) {
+  std::unique_ptr<HNode> keep(x);
+  if (!x) { err = "update: null node"; return nullptr; }
+  if (ncaptures < 0 || (ncaptures > 0 && (!names || !values))) { err = "update: bad capture arrays"; return nullptr; }
+  Closure c;
+  std::string e = parse_closure(text, CL_UPDATE, 0, 0, c);
+  std::vector<float> v;
+  if (e.empty()) e = bind_captures(c, ncaptures, names, values, v);
+  if (!e.empty()) { err = "update: " + e; return nullptr; }
+  return new SystemN(keep.release(), dt, c.expr, std::move(v), c.sets);
 }
 HNode* mk_var_fn(SharedCell* s, int outputs, const char* text, int ncaptures, const char* const* names, const float* values, std::string& err) {
   if (!s) { err = "var_fn: null Shared"; return nullptr; }

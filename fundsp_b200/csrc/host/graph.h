@@ -90,6 +90,9 @@ struct Lowering {
   // (state word, value) pairs where what reset() restores differs from the state a freshly built unit starts from (Adaptive's level
   // estimate: 0.0 after Adaptive::new, 1e-3 after reset, src/shape.rs:173-196). Every other word resets to its lowered value.
   std::vector<std::pair<uint32_t, uint32_t>> resetS;
+  // [begin, end) of state words that the Setting just applied to the node wrote (a System's target values): Bank::set copies them into
+  // the running state, where the device reads them at the next launch
+  std::vector<std::pair<uint32_t, uint32_t>> liveS;
   std::vector<SharedUse> shared;   // Shared readers and writers in evaluation order
   // writers are refused inside units that run on a clock of their own (events, slots, crossfades): the order of their stores is not the bank's
   void no_writers_since(size_t k, const char* where) { for (; k < shared.size(); k++) if (shared[k].kind != SH_READ) { fail(std::string("monitor / timer writing a Shared inside ") + where + " is not supported"); return; } }
@@ -222,6 +225,9 @@ HNode* mk_adsr_live(float a, float d, float s, float r);
 // captures are (name, value) pairs. On failure returns null with the reason in `err` (arity mismatches start with "<what>: arity mismatch").
 HNode* mk_closure(int kind, int inputs, int outputs, double interval, const char* text, int ncaptures, const char* const* names, const float* values,
                   std::string& err);
+// System<X, F> ID 67 (`update(x, dt, f)`): the closure `|t, dt, x| ..` (text, closure.h CL_UPDATE) sets x's parameters every ~dt seconds;
+// consumes x. On failure null with the reason in `err`. A `set` reaching a node the device cannot set is refused when the graph is lowered.
+HNode* mk_update(HNode* x, float dt, const char* text, int ncaptures, const char* const* names, const float* values, std::string& err);
 HNode* mk_pipe(HNode* x, HNode* y);
 HNode* mk_stack(HNode* x, HNode* y);
 HNode* mk_branch(HNode* x, HNode* y);

@@ -575,6 +575,23 @@ def _captures(captures):
     return tuple((str(k), f32(v)) for k, v in captures.items())
 
 
+def update(x, dt, f, **captures):
+    """`update(x, dt, f)` (System ID 67, src/system.rs): runs `f(t, dt, x)` every ~`dt` seconds, at the start of a block, to set x's
+    parameters from time. `f` is text `|t, dt, x| ..` whose body is `let`s and unconditional statements
+    `x.set(Setting::center(..).right())` (center, center_q, center_q_gain, value, pan, biquad; addressed with .left() / .right() /
+    .index(N)); its arguments are expressions of the closure language, of t, dt and the captured values given as keyword arguments:
+        update(saw_hz(110.0) >> lowpass_hz(1000.0, 1.0), 0.002, "|t, dt, x| x.set(Setting::center(500.0 + 400.0 * sin_hz(r, t)).right())", r=0.5)
+    The targets are FixedSvf, the fixed ButterLowpass / Biquad, the fixed one-poles, Constant and Panner<U1>. A setting the reached node
+    ignores is ignored (a Resonator ignores every setting, as in the reference); one that reaches any other node is refused when the bank
+    is built."""
+    if not isinstance(f, str):
+        raise TypeError("update takes its function as text `|t, dt, x| ..` (it is compiled into the voice program); a Python callable cannot run on the GPU")
+    from .capi import GpuBackend, lib
+    a = An("update", (f32(dt), f, _captures(captures)), (x,), x.nin, x.nout)
+    lib().fdsp_node_free(a.lower(GpuBackend()))
+    return a
+
+
 def map_(closure, inputs, outputs, **captures):
     """`map(f)` (Map ID 5): a per-sample function of the input frame `x[0..inputs)`; a tuple value gives several outputs."""
     return _closure("map", (closure, int(inputs), int(outputs), _captures(captures)), int(inputs), int(outputs))

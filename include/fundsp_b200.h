@@ -167,6 +167,12 @@ fdsp_node* fdsp_envelope_in(double interval, int inputs, int outputs, const char
    outputs: the device evaluates it at the reference's jittered sample points (the same points as fdsp_envelope's callback), so it has no
    horizon and stores no table of values. The closure computes in f32; for F = f64 time use fdsp_envelope's callback. */
 fdsp_node* fdsp_envelope_text(double interval, int outputs, const char* closure, int ncaptures, const char* const* names, const float* values);
+/* System ID 67 src/system.rs (`update(x, dt, f)`): f is `|t, dt, x| ..` whose body is `let`s and unconditional statements
+   `x.set(Setting::KIND(args)[.left() | .right() | .index(N)]*);` with KIND center, center_q, center_q_gain, value, pan or biquad; run at the
+   start of a block every ~dt seconds (and at time 0). Consumes x. NULL with the reason as for fdsp_map. A `set` that reaches a node other
+   than FixedSvf, the fixed ButterLowpass / Biquad, the fixed one-poles, Constant or Panner<U1> and that the node does not ignore (a Resonator
+   ignores every setting) makes the bank FDSP_ERR_UNSUPPORTED. */
+fdsp_node* fdsp_update(fdsp_node* x, float dt, const char* closure, int ncaptures, const char* const* names, const float* values);
 /* combinators (src/combinator.rs:289-488; src/audionode.rs) */
 fdsp_node* fdsp_pipe(fdsp_node* x, fdsp_node* y);              /* x >> y  Pipe   ID 6  */
 fdsp_node* fdsp_stack(fdsp_node* x, fdsp_node* y);             /* x | y   Stack  ID 7  */

@@ -299,6 +299,12 @@ inline An envelope(const char* closure, int outputs = 1, Captures captures = {})
   return detail::closure_node(fdsp_envelope_text(0.002, outputs, closure, (int)c.names.size(), c.names.data(), c.values.data()));
 }
 inline An lfo(const char* closure, int outputs = 1, Captures captures = {}) { return envelope(closure, outputs, captures); }
+// update(x, dt, f) (System, src/system.rs) with f as text `|t, dt, x| ..` of `x.set(Setting::..)` statements, e.g.
+// update(saw_hz(110.0f) >> lowpass_hz(1000.0f, 1.0f), 0.002f, "|t, dt, x| x.set(Setting::center(500.0 + 400.0 * sin_hz(r, t)).right())", {{"r", 0.5f}})
+inline An update(An x, float dt, const char* closure, Captures captures = {}) {
+  detail::CaptureArrays c(captures);
+  return detail::closure_node(fdsp_update(x.release(), dt, closure, (int)c.names.size(), c.names.data(), c.values.data()));
+}
 // flanger / phaser (src/prelude.rs:2719-2753): the delay (phase) closure is a closure of time and lowers like `lfo`. phaser's closure
 // returns the allpole delay itself here: lerp(2, 20, clamp01(phase_f(t))) of the reference is the caller's to apply.
 inline An flanger(float feedback_amount, float minimum_delay, float maximum_delay, fdsp_envelope_fn delay_f, void* user = nullptr, double horizon = 10.0) {

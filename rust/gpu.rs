@@ -24,6 +24,7 @@ use crate::combinator::An;
 use crate::math::AttoHash;
 use crate::setting::{Address, Parameter, Setting};
 use crate::signal::{Routing, SignalFrame};
+use crate::system::System;
 use crate::*;
 use core::ffi::{c_char, c_int, c_void};
 use numeric_array::typenum::*;
@@ -60,6 +61,7 @@ extern "C" {
     fn fdsp_shape_fn(closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_envelope_in(interval: f64, inputs: c_int, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_envelope_text(interval: f64, outputs: c_int, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
+    fn fdsp_update(x: *mut FdspNode, dt: f32, closure: *const c_char, ncaptures: c_int, names: *const *const c_char, values: *const f32) -> *mut FdspNode;
     fn fdsp_convolve(response: *const f32, n: c_int) -> *mut FdspNode;
     fn fdsp_shaper(kind: c_int, p0: f32, p1: f32) -> *mut FdspNode;
     fn fdsp_shaper_adaptive(timescale: f64, inner_kind: c_int, p0: f32, p1: f32) -> *mut FdspNode;
@@ -488,6 +490,46 @@ macro_rules! gpu_envelope {
 #[macro_export]
 macro_rules! gpu_lfo {
     ($($t:tt)+) => { $crate::gpu_envelope!($($t)+) };
+}
+
+/// `update(x, dt, f)` (system.rs, System ID 67) that can also run on the GPU: the reference's System (what runs on the CPU), a copy of x
+/// that settings reach too (what is lowered) and the update function's text. Made by `gpu_update!`.
+#[derive(Clone)]
+pub struct GpuSystem<X: AudioNode, F: FnMut(f32, f32, &mut X) + Clone + Send + Sync> {
+    pub node: System<X, F>, pub x: X, pub dt: f32, pub text: &'static str, pub names: Vec<&'static str>, pub values: Vec<f32>,
+}
+impl<X: AudioNode, F: FnMut(f32, f32, &mut X) + Clone + Send + Sync> AudioNode for GpuSystem<X, F> {
+    const ID: u64 = 67;
+    type Inputs = X::Inputs;
+    type Outputs = X::Outputs;
+    fn reset(&mut self) { self.node.reset() }
+    fn set_sample_rate(&mut self, sample_rate: f64) { self.node.set_sample_rate(sample_rate); self.x.set_sample_rate(sample_rate) }
+    fn tick(&mut self, input: &Frame<f32, Self::Inputs>) -> Frame<f32, Self::Outputs> { self.node.tick(input) }
+    fn process(&mut self, size: usize, input: &BufferRef, output: &mut BufferMut) { self.node.process(size, input, output) }
+    fn set(&mut self, setting: Setting) { self.x.set(setting.clone()); self.node.set(setting) }
+    fn ping(&mut self, probe: bool, hash: AttoHash) -> AttoHash { self.node.ping(probe, hash) }
+    fn route(&mut self, input: &SignalFrame, frequency: f64) -> SignalFrame { self.node.route(input, frequency) }
+}
+impl<X: AudioNode + Lower, F: FnMut(f32, f32, &mut X) + Clone + Send + Sync> Lower for GpuSystem<X, F> {
+    unsafe fn lower(&self) -> *mut FdspNode {
+        let text: Vec<u8> = self.text.bytes().chain(core::iter::once(0)).collect();
+        let names: Vec<Vec<u8>> = self.names.iter().map(|n| n.bytes().chain(core::iter::once(0)).collect()).collect();
+        let ptrs: Vec<*const c_char> = names.iter().map(|n| n.as_ptr() as *const c_char).collect();
+        fdsp_update(self.x.lower(), self.dt, text.as_ptr() as *const c_char, self.values.len() as c_int, ptrs.as_ptr(), self.values.as_ptr())
+    }
+}
+/// `gpu_update!(x, dt, [r], |t: f32, dt: f32, x: &mut _| x.set(Setting::center(600.0 + 400.0 * sin_hz(r, t)).right()))`: `update(x, dt, f)`
+/// (prelude.rs, System ID 67) that lowers to `fdsp_update`. The body is `let`s and unconditional `x.set(Setting::..)` statements
+/// (DESIGN.md §2); the GPU runs it at the same update points.
+#[macro_export]
+macro_rules! gpu_update {
+    ($x:expr, $dt:expr, [$($c:ident),*], $($f:tt)+) => {{
+        let x = $x;
+        $crate::combinator::An($crate::gpu::GpuSystem {
+            node: $crate::system::System::new(x.clone(), $dt, $($f)+), x: x.0, dt: $dt,
+            text: stringify!($($f)+), names: vec![$(stringify!($c)),*], values: vec![$($c as f32),*],
+        })
+    }};
 }
 
 /// V voices of typed graphs evaluated in lockstep on one GPU; to the host ONE `AudioUnit` (audiounit.rs:21-95).
