@@ -75,6 +75,38 @@ class GpuBank:
         vals = (C.c_float * max(1, len(values)))(*values)
         check(self.L.fdsp_bank_set(self.h, voice, kind, vals, len(values), seed, (C.c_int64 * max(1, len(addr)))(*addr), len(address)))
 
+    def set_voices(self, kind, values, voices=None, seeds=None, address=()):
+        """`set` on many voices in one call: entry j sets voice `voices[j]` (j when `voices` is None) to `values[j]` (a row of an
+        [n, nvalues] array, or one value when `values` is 1-D) with seed `seeds[j]` (0 when None), all with one `kind` and `address`.
+        The same as calling `set` for each entry in order; on a refusal the FdspError's `entry` is the index of the refused entry (the
+        entries before it are applied, the rest are not)."""
+        vals = np.ascontiguousarray(values, np.float32)
+        if vals.ndim == 1:
+            vals = vals.reshape(-1, 1)
+        if vals.ndim != 2:
+            raise ValueError("values: one row of setting values per entry")
+        n, nv = vals.shape
+        vp = None
+        if voices is not None:
+            vs = np.ascontiguousarray(voices, np.uint32)
+            if vs.shape != (n,):
+                raise ValueError("voices: one voice index per entry")
+            vp = vs.ctypes.data_as(C.POINTER(C.c_uint32))
+        sp = None
+        if seeds is not None:
+            ss = np.ascontiguousarray(seeds, np.uint64)
+            if ss.shape != (n,):
+                raise ValueError("seeds: one seed per entry")
+            sp = ss.ctypes.data_as(C.POINTER(C.c_uint64))
+        addr = [x for pair in address for x in pair]
+        failed = C.c_uint32(0)
+        try:
+            check(self.L.fdsp_bank_set_voices(self.h, kind, vp, n, _fp(vals), nv, sp, (C.c_int64 * max(1, len(addr)))(*addr), len(address),
+                                              C.byref(failed)))
+        except FdspError as e:
+            e.entry = int(failed.value)
+            raise
+
     # ---- sequencer banks (voices built with fundsp_b200.sequencer.event): the mix output is Sequencer::process
     @classmethod
     def from_sequencer(cls, seq, device=0, per_voice=False, mix=True, sample_rate=None):

@@ -323,6 +323,175 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
   return "internal: voice not found in any class";
 }
 
+// A node lowered alone that adds parameter and state words and nothing else (no uniform words, delay lines, Shared uses, reset exemptions
+// or running-state words of a set): its words are then exactly its part of its voice's lowering, wherever it sits.
+static bool words_only(const Lowering& l) {
+  return l.ok && l.U.empty() && l.dlen.empty() && !l.extraU && !l.extraP && !l.conv_K && l.keepS.empty() && l.keepD.empty() && l.liveS.empty() &&
+         l.shared.empty();
+}
+
+// Where the node that `st`'s address reaches lowers its words in class c, found on the class's first voice.
+static VoiceClass::LeafAt leaf_at_of(const VoiceClass& c, HNode* voice, Setting st) {
+  VoiceClass::LeafAt r;
+  bool ignored = false;
+  HNode* leaf = setting_leaf(voice, &st, &ignored);
+  if (!leaf) return r;
+  Lowering whole, alone;
+  whole.mark = leaf;
+  whole.sub(voice);
+  leaf->lower(alone);
+  if (!whole.ok || !whole.marked || whole.P.size() != c.np || whole.S.size() != c.ns || !words_only(alone)) return r;
+  r.p0 = whole.mark_p[0]; r.np = whole.mark_p[1] - whole.mark_p[0]; r.s0 = whole.mark_s[0]; r.ns = whole.mark_s[1] - whole.mark_s[0];
+  r.ok = alone.P.size() == r.np && alone.S.size() == r.ns && std::equal(alone.P.begin(), alone.P.end(), whole.P.begin() + r.p0) &&
+         std::equal(alone.S.begin(), alone.S.end(), whole.S.begin() + r.s0);
+  return r;
+}
+
+std::string Bank::set_voices(const Setting& st, uint32_t n, const uint32_t* voices, const float* values, int nvalues, const uint64_t* seeds, uint32_t* failed) {
+  *failed = n;
+  if (n == 0) return "";
+  CU(cudaSetDevice(device));
+  TRY(rt_end_streak());
+  std::vector<uint64_t> key;
+  for (const Address& a : st.address) { key.push_back((uint64_t)a.type); key.push_back(a.value); }
+  std::vector<SvClass> staged;
+  std::vector<int> staged_of(classes.size(), -1);
+  std::vector<int32_t> entry_of;   // per voice: its entry in its class's staging, -1 none
+  bool applied = false;
+  auto finish = [&]() -> std::string {
+    if (!applied) return "";
+    TRY(sv_flush(staged));
+    // set() ends by re-reading the Shared reader rows from the device, where a row can hold other voices' plain words; the entries
+    // applied here change no reader, so with no reader rows there is nothing to re-read
+    for (const VoiceClass& c : classes) if (!c.sh_rows.empty()) return sh_rebuild();
+    return "";
+  };
+  for (uint32_t j = 0; j < n; j++) {
+    const uint32_t v = voices ? voices[j] : j;
+    Setting s = st;
+    s.seed = seeds ? seeds[j] : 0;
+    for (int k = 0; k < nvalues; k++) s.v[k] = values[(size_t)j * (size_t)nvalues + k];
+    uint32_t i = 0;
+    VoiceClass* c = v < V() ? locate(classes, v, &i) : nullptr;
+    if (c) {
+      Setting leaf_s = s;
+      bool ignored = false;
+      HNode* leaf = setting_leaf(nodes[v].get(), &leaf_s, &ignored);
+      if (ignored) continue;   // the address leads nowhere: set() would change nothing
+      auto it = c->leaf_at.find(key);
+      if (leaf && it == c->leaf_at.end()) it = c->leaf_at.emplace(key, leaf_at_of(*c, nodes[c->voices[0]].get(), st)).first;
+      if (leaf && it->second.ok) {
+        const VoiceClass::LeafAt& at = it->second;
+        // the setting is tried on a copy of the node, as set() tries it on a copy of the voice
+        std::unique_ptr<HNode> trial(leaf->clone());
+        trial->set(leaf_s);
+        Lowering l;
+        trial->lower(l);
+        if (words_only(l) && l.P.size() == at.np && l.S.size() == at.ns) {
+          leaf->set(leaf_s);
+          const uint32_t Vc = c->V();
+          const std::vector<uint32_t> S0 = l.reset_image();
+          for (uint32_t k = 0; k < at.ns; k++) c->state0[(size_t)(at.s0 + k) * Vc + i] = S0[k];
+          c->state0_stale = true;
+          applied = true;
+          if (!at.np) continue;
+          const size_t ci = (size_t)(c - classes.data());
+          if (staged_of[ci] < 0) { staged_of[ci] = (int)staged.size(); staged.push_back(SvClass{c, at, {}, {}}); }
+          SvClass& sc = staged[(size_t)staged_of[ci]];
+          if (entry_of.empty()) entry_of.assign(V(), -1);
+          if (entry_of[v] < 0) {
+            entry_of[v] = (int32_t)sc.cols.size();
+            sc.cols.push_back(i);
+            sc.words.insert(sc.words.end(), l.P.begin(), l.P.end());
+          } else {
+            std::copy(l.P.begin(), l.P.end(), sc.words.begin() + (size_t)entry_of[v] * at.np);
+          }
+          continue;
+        }
+      }
+      // set() writes the voice's whole column from its host graph, which holds this voice's earlier entries: a staged one is dropped
+      if (!entry_of.empty() && entry_of[v] >= 0) { staged[(size_t)staged_of[(size_t)(c - classes.data())]].cols[(size_t)entry_of[v]] = UINT32_MAX; entry_of[v] = -1; }
+    }
+    const std::string e = set(v, s);
+    if (!e.empty()) {
+      *failed = j;
+      TRY(finish());
+      return e;
+    }
+  }
+  return finish();
+}
+
+// The scatter behind Bank::set_voices: params[(row0 + w) * V + cols[e]] = words[w * m + e] for the m entries and k words staged for one
+// class's [NP][V] parameter block (the columns are distinct). One thread per (word, entry); the words are word-major, so the threads of
+// a warp write one row.
+#ifdef FDSP_HOST_EMUL
+// the CPU mock device (tests/cpp/mock) has no kernels: the same writes, queued on the stream as a launch is
+static cudaError_t launch_set_columns(uint32_t* params, uint32_t V, uint32_t row0, uint32_t k, const uint32_t* cols, const uint32_t* words, uint32_t m,
+                                      cudaStream_t st) {
+  return mock_launch(st, [=] {
+    for (uint64_t t = 0; t < (uint64_t)m * k; t++) params[(size_t)(row0 + t / m) * V + cols[t % m]] = words[t];
+    return (cudaError_t)cudaSuccess;
+  });
+}
+#else
+__global__ void __launch_bounds__(256) set_columns_kernel(uint32_t* __restrict__ params, uint32_t V, uint32_t row0, uint32_t k,
+                                                          const uint32_t* __restrict__ cols, const uint32_t* __restrict__ words, uint32_t m) {
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (uint64_t)m * k) return;
+  params[(size_t)(row0 + (uint32_t)(t / m)) * V + cols[t % m]] = words[t];
+}
+static cudaError_t launch_set_columns(uint32_t* params, uint32_t V, uint32_t row0, uint32_t k, const uint32_t* cols, const uint32_t* words, uint32_t m,
+                                      cudaStream_t st) {
+  const uint64_t total = (uint64_t)m * k;
+  if (!total) return cudaSuccess;
+  set_columns_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(params, V, row0, k, cols, words, m);
+  return cudaGetLastError();
+}
+#endif
+
+// The staged parameter words of every class in one copy, then one scatter launch per class that has any.
+std::string Bank::sv_flush(const std::vector<SvClass>& staged) {
+  size_t total = 0;
+  std::vector<uint32_t> live(staged.size(), 0);
+  for (size_t t = 0; t < staged.size(); t++) {
+    for (uint32_t col : staged[t].cols) live[t] += col != UINT32_MAX;
+    total += (size_t)live[t] * (1 + staged[t].at.np);
+  }
+  if (!total) return "";
+  if (sv_pending) { CU(cudaEventSynchronize(sv_copied)); sv_pending = false; }
+  TRY(sv_stage.grow(total));
+  TRY(d_sv.grow(total));
+  // per class: the live entries' columns [m], then their words word-major [np][m] (a warp writes one row of the [NP][V] block)
+  size_t at = 0;
+  for (size_t t = 0; t < staged.size(); t++) {
+    const SvClass& sc = staged[t];
+    const uint32_t m = live[t], np = sc.at.np;
+    uint32_t e = 0;
+    for (size_t q = 0; q < sc.cols.size(); q++) {
+      if (sc.cols[q] == UINT32_MAX) continue;
+      sv_stage[at + e] = sc.cols[q];
+      for (uint32_t w = 0; w < np; w++) sv_stage[at + m + (size_t)w * m + e] = sc.words[q * np + w];
+      e++;
+    }
+    at += (size_t)m * (1 + np);
+  }
+  CU(cudaMemcpyAsync(d_sv, sv_stage, total * 4, cudaMemcpyHostToDevice, stream));
+  if (!sv_copied) CU(cudaEventCreateWithFlags(sv_copied.put(), cudaEventDisableTiming));
+  CU(cudaEventRecord(sv_copied, stream));
+  sv_pending = true;
+  at = 0;
+  for (size_t t = 0; t < staged.size(); t++) {
+    const SvClass& sc = staged[t];
+    const uint32_t m = live[t];
+    if (!m) continue;
+    CU(launch_set_columns(sc.c->d_params, sc.c->V(), sc.at.p0, sc.at.np, d_sv + at, d_sv + at + m, m, stream));
+    launches++;
+    at += (size_t)m * (1 + sc.at.np);
+  }
+  return "";
+}
+
 double Bank::loop_point() const {
   if (!(loop_arg > 0.0)) return std::numeric_limits<double>::infinity();
   const double ur = unit_rate();

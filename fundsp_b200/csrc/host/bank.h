@@ -56,6 +56,10 @@ struct VoiceClass {
   Array<uint32_t> d_state0; bool state0_stale = true;
   Array<uint32_t> d_params, d_state, d_uniform, d_rowmap;
   Array<float> d_dline, d_partial;
+  // Bank::set_voices: per address ((type, value) pairs), where the node that address reaches lowers its words in this class's layout,
+  // found once on one voice (every voice of a class has one structure); !ok: its voices take Bank::set
+  struct LeafAt { bool ok = false; uint32_t p0 = 0, np = 0, s0 = 0, ns = 0; };
+  std::map<std::vector<uint64_t>, LeafAt> leaf_at;
   uint32_t V() const { return (uint32_t)voices.size(); }
   bool fdn_with_dry() const { return form == Form::fdn && k; }   // two stages, software-pipelined by render_device_run
   std::string clear_history(cudaStream_t st);   // zeroes what the form's own buffers carry from call to call (on upload and reset)
@@ -137,6 +141,15 @@ struct Bank {
   std::string run_conv(VoiceClass& c, const Chunk& w, const ClassGrid& g, const BankArgs& a);
   std::string push_event(HNode* event, uint32_t* voice);                      // Sequencer::push on a running bank: takes the slot of a finished event of the same class; consumes event
   std::string set(uint32_t voice, const Setting& s);  // AudioUnit::set on one voice of a live bank (parameters only; state continues)
+  // set() on n (voice, values) entries in order: entry j is voice voices[j] (j when voices is null) with values[j * nvalues ..] and
+  // seeds[j] (0 when seeds is null). On a refusal *failed = j: the entries before it are applied, the rest are not. An entry whose setting
+  // changes only the words of the node it reaches is applied on the host alone; its parameter words reach the device in one copy and one
+  // scatter launch per class at the end. Every other entry takes set().
+  std::string set_voices(const Setting& s, uint32_t n, const uint32_t* voices, const float* values, int nvalues, const uint64_t* seeds, uint32_t* failed);
+  struct SvClass { VoiceClass* c; VoiceClass::LeafAt at; std::vector<uint32_t> cols, words; };   // one class's staged entries ([entry][word])
+  std::string sv_flush(const std::vector<SvClass>& staged);
+  PinnedArray<uint32_t> sv_stage; Array<uint32_t> d_sv;   // set_voices' parameter words: host staging and its device copy
+  Event sv_copied; bool sv_pending = false;               // recorded behind the copy of sv_stage: it is rewritten only after that copy has landed
   std::string ensure_staging(uint32_t chunk);
   std::string render_device(uint64_t n, const float* in_dev, uint64_t in_stride, float* out_dev, uint64_t out_stride, float* mix_dev,
                             uint64_t mix_stride);

@@ -774,7 +774,7 @@ struct EventN : HNode {  // one Sequencer event as a voice (src/sequencer.rs:55-
     uint64_t sb, eb; memcpy(&sb, &cs0, 8); memcpy(&eb, &ce0, 8);
     l.su((uint32_t)sb); l.su((uint32_t)(sb >> 32)); l.su((uint32_t)eb); l.su((uint32_t)(eb >> 32));   // current start / end (a loop wrap moves them while the event sounds)
     const size_t k = l.shared.size();
-    x->lower(l);
+    l.sub(x.p.get());
     l.no_writers_since(k, "a sequencer event");
   }
   HCLONE(EventN)
@@ -1016,7 +1016,7 @@ struct Binary : HNode {
       default: o += "Binop<" + I(op) + ","; }
     x->sig(o); o += ","; y->sig(o); o += ">";
   }
-  void lower(Lowering& l) const override { x->lower(l); y->lower(l); }
+  void lower(Lowering& l) const override { l.sub(x.p.get()); l.sub(y.p.get()); }
   HCLONE(Binary)
 };
 struct PulseWaveN : HNode {  // src/wavetable.rs:439-491: (saw with phase output | width) >> (saw | phase + width >> saw at that phase) >> difference
@@ -1055,7 +1055,7 @@ struct Unary : HNode {
   void lower(Lowering& l) const override {
     if (k == UNOP && kind != 0) l.p(scalar);
     if (k == FEEDBACK) for (int i = 0; i < x->inputs(); i++) l.s(0.0f);
-    x->lower(l);
+    l.sub(x.p.get());
   }
   HCLONE(Unary)
 };
@@ -1088,7 +1088,7 @@ struct Multi : HNode {  // MultiBus 28, MultiStack 30, Reduce 31, MultiBranch 33
     for (auto& c : x) { std::string s; c->sig(s); if (s != first) { o += "Unsupported"; return; } }
     o += "Multi<" + I(kind) + "," + I(op) + "," + I(N()) + "," + first + ">";
   }
-  void lower(Lowering& l) const override { for (auto& c : x) c->lower(l); }
+  void lower(Lowering& l) const override { for (auto& c : x) l.sub(c.p.get()); }
   HCLONE(Multi)
 };
 
@@ -1133,22 +1133,7 @@ struct SystemN : HNode {
   }
   SystemN(const SystemN& o) : HNode(o), x(o.x), interval(o.interval), expr(o.expr), caps(o.caps), sets(o.sets), tg(o.tg), nsv(o.nsv), refused(o.refused) {}
   // where the setting goes inside X, as the combinators' set() route it; `hops`: the child taken at each step (nodes.cuh UpdAt)
-  HNode* reach(Setting s, std::vector<int>& hops) const {
-    HNode* n = x.p.get();
-    for (;;) {
-      const Address d = s.direction();
-      if (Binary* b = dynamic_cast<Binary*>(n)) {
-        if (d.type != 1 || d.value > 1) return nullptr;
-        hops.push_back((int)d.value); n = d.value == 0 ? b->x.p.get() : b->y.p.get(); s = s.peel();
-      } else if (Unary* u = dynamic_cast<Unary*>(n)) {
-        if (u->k == Unary::FEEDBACK) return nullptr;
-        hops.push_back(0); n = u->x.p.get();
-      } else if (Multi* m = dynamic_cast<Multi*>(n)) {
-        if (d.type != 1 || d.value >= m->x.size()) return nullptr;
-        hops.push_back((int)d.value); n = m->x[d.value].p.get(); s = s.peel();
-      } else return n;
-    }
-  }
+  HNode* reach(Setting s, std::vector<int>& hops) const { return reach_setting(x.p.get(), &s, &hops); }
   static const char* setting_name(int kind) {
     switch (kind) { case P_CENTER: return "center"; case P_CENTER_Q: return "center_q"; case P_CENTER_Q_GAIN: return "center_q_gain";
       case P_VALUE: return "value"; case P_BIQUAD: return "biquad"; default: return "pan"; }
@@ -1324,6 +1309,22 @@ struct HNet : HNode {
 
 }  // namespace
 
+HNode* reach_setting(HNode* n, Setting* s, std::vector<int>* hops) {
+  for (;;) {
+    const Address d = s->direction();
+    if (Binary* b = dynamic_cast<Binary*>(n)) {
+      if (d.type != 1 || d.value > 1) return nullptr;
+      hops->push_back((int)d.value); n = d.value == 0 ? b->x.p.get() : b->y.p.get(); *s = s->peel();
+    } else if (Unary* u = dynamic_cast<Unary*>(n)) {
+      if (u->k == Unary::FEEDBACK) return nullptr;
+      hops->push_back(0); n = u->x.p.get();
+    } else if (Multi* m = dynamic_cast<Multi*>(n)) {
+      if (d.type != 1 || d.value >= m->x.size()) return nullptr;
+      hops->push_back((int)d.value); n = m->x[d.value].p.get(); *s = s->peel();
+    } else return n;
+  }
+}
+
 HNode* mk_net(int inputs, int outputs) { return (inputs < 0 || outputs < 0) ? nullptr : new HNet(inputs, outputs); }
 bool is_net(const HNode* n) { return dynamic_cast<const HNet*>(n) != nullptr; }
 int net_push(HNode* net, HNode* unit) {
@@ -1494,6 +1495,14 @@ HNode* mk_xfade(HNode* x, HNode* y, int ease, float fade_time) {
 bool xfade_set_done(HNode* n, bool done) { XfadeN* q = dynamic_cast<XfadeN*>(n); if (!q) return false; q->done = done; return true; }
 bool xfade_fade(const HNode* n, float* fade_time, float* sr) { const XfadeN* q = dynamic_cast<const XfadeN*>(n); if (!q) return false; *fade_time = q->fade_time; *sr = (float)q->sr; return true; }
 const HNode* xfade_unit(const HNode* n, int which) { const XfadeN* q = dynamic_cast<const XfadeN*>(n); return q ? (which ? q->y.p.get() : q->x.p.get()) : nullptr; }
+HNode* setting_leaf(HNode* voice, Setting* s, bool* ignored) {
+  while (EventN* e = dynamic_cast<EventN*>(voice)) voice = e->x.p.get();
+  std::vector<int> hops;
+  HNode* n = reach_setting(voice, s, &hops);
+  *ignored = n == nullptr;
+  if (!n || dynamic_cast<SystemN*>(n) || dynamic_cast<HNet*>(n) || dynamic_cast<SlotN*>(n) || dynamic_cast<XfadeN*>(n)) return nullptr;
+  return n;
+}
 bool event_edit(HNode* n, double end_time, double fade_out) {   // Sequencer::edit on an event (:441-483, no loop: start == original start)
   EventN* e = dynamic_cast<EventN*>(n);
   if (!e) return false;

@@ -78,6 +78,8 @@ struct SharedRef {   // one counted reference
 enum SharedUseKind { SH_READ = 0, SH_MONITOR = 1, SH_TIMER = 2 };
 struct SharedUse { uint32_t word; SharedCell* cell; int kind; };
 
+struct HNode;
+
 struct Lowering {
   std::vector<uint32_t> P, S, U;   // words in DFS order
   std::vector<uint32_t> dlen;      // delay-line lengths (floats per voice) in DFS order
@@ -97,6 +99,10 @@ struct Lowering {
   // writers are refused inside units that run on a clock of their own (events, slots, crossfades): the order of their stores is not the bank's
   void no_writers_since(size_t k, const char* where) { for (; k < shared.size(); k++) if (shared[k].kind != SH_READ) { fail(std::string("monitor / timer writing a Shared inside ") + where + " is not supported"); return; } }
   bool ok = true; std::string why; // set when a node has no device lowering
+  // where one node's words sit in its voice's lowering (Bank::set_voices): the combinators a Setting walks through (reach_setting, and a
+  // sequencer event) lower their children through sub(), which records the [begin, end) of P and S that `mark` lowers
+  const HNode* mark = nullptr; bool marked = false; uint32_t mark_p[2] = {0, 0}, mark_s[2] = {0, 0};
+  inline void sub(const HNode* n);
   void p(float f) { P.push_back(f2u(f)); }
   void s(float f) { S.push_back(f2u(f)); }
   void su(uint32_t u) { S.push_back(u); }
@@ -124,6 +130,22 @@ struct HNode {
   void ctor_ping() { AttoHash h = ping(true, AttoHash(id())); ping(false, h); }
   static std::vector<uint64_t>*& ping_trace();
 };
+inline void Lowering::sub(const HNode* n) {
+  if (n != mark) { n->lower(*this); return; }
+  mark_p[0] = (uint32_t)P.size(); mark_s[0] = (uint32_t)S.size();
+  n->lower(*this);
+  mark_p[1] = (uint32_t)P.size(); mark_s[1] = (uint32_t)S.size(); marked = true;
+}
+
+// Where a Setting goes inside `n`, as the combinators' own set() forwards it: an Index peels one step into a binary combinator or a Multi;
+// Unop and Thru pass the setting on unchanged; Feedback keeps it. Returns the node at which that walk ends, with *s as it arrives there
+// (`hops`: the child taken at each step), or null when the address leads nowhere (the combinator ignores the setting).
+HNode* reach_setting(HNode* n, Setting* s, std::vector<int>* hops);
+// The node that `voice->set(s)` changes, when nothing else changes: reach_setting, entered through a sequencer event (whose set() only
+// forwards to its unit), with *s as that node receives it. *ignored: the setting leads nowhere. Null as well when the walk ends at a node
+// whose set() does more than change its own words: a System (it also writes its targets' values into the running state), a Net, a Slot,
+// a crossfading vertex.
+HNode* setting_leaf(HNode* voice, Setting* s, bool* ignored);
 
 // ---- builders (one per primitive; composites consume their children)
 HNode* mk_constant(int n, const float* v);

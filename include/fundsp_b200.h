@@ -281,6 +281,13 @@ int fdsp_bank_reset(fdsp_bank* b);                                          /* A
 /* AudioUnit::set (src/audiounit.rs:62) on voice `voice` of a live bank: same encoding as fdsp_node_set. Parameters change at
    once, running state continues; FDSP_ERR_UNSUPPORTED when the setting would change a delay length (rebuild the bank). */
 int fdsp_bank_set(fdsp_bank* b, uint32_t voice, int kind, const float* values, int nvalues, uint64_t seed, const int64_t* address_pairs, int naddress);
+/* fdsp_bank_set on n entries in one call: entry j sets voice voices[j] (j when voices is NULL) to values[j*nvalues .. +nvalues) with seed
+   seeds[j] (0 when seeds is NULL); one setting kind and one address for all. The same as calling fdsp_bank_set for j = 0, 1, .. n-1:
+   entries of one voice apply in order, and on the first entry that call would refuse, this one returns its error with *failed_entry = j
+   (the entries before j applied, the rest not; n on success). Values are host memory. The parameter words reach the device in one copy
+   and one launch per class the entries touch. */
+int fdsp_bank_set_voices(fdsp_bank* b, int kind, const uint32_t* voices, uint32_t n, const float* values, int nvalues, const uint64_t* seeds,
+                         const int64_t* address_pairs, int naddress, uint32_t* failed_entry);
 int fdsp_bank_allocate(fdsp_bank* b, uint64_t max_render_samples);          /* AudioUnit::allocate: later calls do not allocate */
 /* AudioUnit::process: size <= 64; host buffers in [inputs][64], out [outputs][64]; size 0 is a no-op */
 int fdsp_bank_process(fdsp_bank* b, uint32_t size, const float* in, float* out);

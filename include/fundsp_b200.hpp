@@ -383,6 +383,16 @@ class Bank {
     for (auto& p : address) { a.push_back(p.first); a.push_back(p.second); }
     check(fdsp_bank_set(b_, voice, kind, values.begin(), (int)values.size(), seed, a.empty() ? nullptr : a.data(), (int)address.size()));
   }
+  // set() on many voices in one call (fdsp_bank_set_voices): entry j sets voice voices[j] (j when `voices` is empty) to
+  // values[j * nvalues ..]; `seeds` is empty or one per entry. A refusal throws with the failing entry's index in *failed_entry.
+  void set_voices(int kind, const std::vector<float>& values, int nvalues, const std::vector<uint32_t>& voices = {},
+                  std::initializer_list<std::pair<int, int64_t>> address = {}, const std::vector<uint64_t>& seeds = {}, uint32_t* failed_entry = nullptr) {
+    std::vector<int64_t> a;
+    for (auto& p : address) { a.push_back(p.first); a.push_back(p.second); }
+    const uint32_t n = voices.empty() ? (nvalues > 0 ? (uint32_t)(values.size() / (size_t)nvalues) : (uint32_t)seeds.size()) : (uint32_t)voices.size();
+    check(fdsp_bank_set_voices(b_, kind, voices.empty() ? nullptr : voices.data(), n, values.data(), nvalues, seeds.empty() ? nullptr : seeds.data(),
+                               a.empty() ? nullptr : a.data(), (int)address.size(), failed_entry));
+  }
   void allocate(uint64_t max_samples = 64) { check(fdsp_bank_allocate(b_, max_samples)); }
   // sequencer banks: Sequencer::time / edit / push on a running bank (a pushed event reuses the slot of a finished event of its class)
   double time() const { return fdsp_bank_time(b_); }

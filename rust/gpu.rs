@@ -141,6 +141,8 @@ extern "C" {
     fn fdsp_bank_reset(b: *mut FdspBank) -> c_int;
     fn fdsp_bank_allocate(b: *mut FdspBank, max_render_samples: u64) -> c_int;
     fn fdsp_bank_set(b: *mut FdspBank, voice: u32, kind: c_int, v: *const f32, nv: c_int, seed: u64, addr: *const i64, naddr: c_int) -> c_int;
+    fn fdsp_bank_set_voices(b: *mut FdspBank, kind: c_int, voices: *const u32, n: u32, v: *const f32, nv: c_int, seeds: *const u64, addr: *const i64,
+                            naddr: c_int, failed_entry: *mut u32) -> c_int;
     fn fdsp_bank_process(b: *mut FdspBank, size: u32, input: *const f32, output: *mut f32) -> c_int;
     fn fdsp_bank_render(b: *mut FdspBank, n: u64, input: *const f32, out_voices: *mut f32, out_mix: *mut f32) -> c_int;
     // multi-GPU mix-down (csrc/host/group.h)
@@ -566,6 +568,20 @@ impl GpuBank {
         let mut b: *mut FdspBank = core::ptr::null_mut();
         check(fdsp_bank_create_from_net(net, device, if mix { FDSP_OUT_MIX } else { FDSP_OUT_VOICES }, &mut b))?;
         Ok(GpuBank { h: b, inputs: fdsp_bank_inputs(b) as usize, outputs: fdsp_bank_outputs(b) as usize, failed: false })
+    }
+    /// `AudioUnit::set` on many voices in one call: entry j sets voice `voices[j]` (j when `voices` is None) to
+    /// `values[j * nvalues..(j + 1) * nvalues]` with Parameter index `kind` and the (type, value) address pairs of `fdsp_node_set`. The same
+    /// as one `set` per entry in order; on a refusal, Err holds the refused entry's index (the entries before it are applied, the rest not).
+    pub fn set_voices(&mut self, kind: i32, values: &[f32], nvalues: usize, voices: Option<&[u32]>, address: &[(i32, i64)]) -> Result<(), (u32, String)> {
+        let n = match voices { Some(v) => v.len(), None => if nvalues > 0 { values.len() / nvalues } else { 0 } };
+        if nvalues > 5 || values.len() < n * nvalues { return Err((0, String::from("set_voices: values holds fewer than n * nvalues values"))); }
+        let addr: Vec<i64> = address.iter().flat_map(|&(t, v)| [t as i64, v]).collect();
+        let mut failed = 0u32;
+        let rc = unsafe {
+            fdsp_bank_set_voices(self.h, kind as c_int, voices.map_or(core::ptr::null(), |v| v.as_ptr()), n as u32, values.as_ptr(), nvalues as c_int,
+                                 core::ptr::null(), addr.as_ptr(), address.len() as c_int, &mut failed)
+        };
+        check(rc).map_err(|e| (failed, e))
     }
     pub fn voice_of_vertex(&self, vertex: usize) -> Option<u32> { let v = unsafe { fdsp_bank_voice_of_vertex(self.h, vertex as c_int) }; if v < 0 { None } else { Some(v as u32) } }
     pub fn replace<X: AudioNode + Lower>(&mut self, voice: u32, unit: &An<X>) -> Result<(), String> { check(unsafe { fdsp_bank_replace_voice(self.h, voice, unit.lower()) }) }   // Net::replace (net.rs:460)
