@@ -25,6 +25,12 @@ static inline float __uint_as_float(uint32_t u) { float f; memcpy(&f, &u, 4); re
 static inline uint32_t __float_as_uint(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
 static inline float __int_as_float(int i) { float f; memcpy(&f, &i, 4); return f; }
 static inline float __fmaf_rn(float a, float b, float c) { return fmaf(a, b, c); }
+static inline float __fadd_rz(float a, float b) {   // exact when the f64 sum is (every use here: |a| < 2^23, b = 2^23)
+  const double s = (double)a + (double)b;
+  float f = (float)s;
+  if (fabs((double)f) > fabs(s)) f = nextafterf(f, 0.0f);
+  return f;
+}
 static inline int __popc(uint32_t x) { return __builtin_popcount(x); }
 static inline double __longlong_as_double(long long x) { double d; memcpy(&d, &x, 8); return d; }
 static inline long long __double_as_longlong(double d) { long long x; memcpy(&x, &d, 8); return x; }

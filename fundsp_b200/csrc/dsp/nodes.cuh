@@ -483,11 +483,21 @@ template <int KIND, int NOUT> struct WaveSynth {  // src/wavetable.rs:244-359, I
     if (C::SMEM_TABLES) { if (c.tsm_kind == KIND) return lds_f32(c.tsm + 4u * (uint32_t)idx); }
     return __ldg(t.data + idx);
   }
+  // (int)p and (float)(int)p of a table position p = len * phase on the FP32 pipe, leaving the conversion unit to wide_floorf: the phase
+  // lies in [0, 1], or below 0 by a few ulps (wide_floorf's rounding), or is NaN, so |p| < 2^23 and (int)p = (int)|p|. Adding 2^23 rounded
+  // toward zero leaves that integer in the low mantissa bits of the sum; the caller masks them to the table (len <= 8192 < 2^23), which also
+  // keeps a NaN phase's index inside it (its output is NaN either way).
+  static FDSP_DEV int trunc_bits(float p, float& fi) {
+    const float t = __fadd_rz(fabsf(p), 8388608.0f);
+    fi = t - 8388608.0f;
+    return (int)__float_as_uint(t);
+  }
   // Tables carry wrap-around guard samples (host device_wavetable): taps i1-1 .. i1+2 modulo len are consecutive floats.
   template <class C> static FDSP_DEV float at(const C& c, const WaveTableDev& t, int off, int len, float phase) {  // :125-155 (i32 index math, truncation)
     float p = (float)len * phase;
-    int i1 = (int)p;
-    float w = p - (float)i1;
+    float fi;
+    const int i1 = trunc_bits(p, fi);
+    float w = p - fi;
     const int b = off + (i1 & (len - 1)) - 1;
     return optimal4x44(tap(c, t, b), tap(c, t, b + 1), tap(c, t, b + 2), tap(c, t, b + 3), w);
   }
@@ -515,8 +525,9 @@ template <int KIND, int NOUT> struct WaveSynth {  // src/wavetable.rs:244-359, I
     const float flen = (float)len;
     FDSP_G8 {
       const float p = flen * ph[j];
-      const int i1 = (int)p;
-      w[j] = p - (float)i1;
+      float fi;
+      const int i1 = trunc_bits(p, fi);
+      w[j] = p - fi;
       const int b = off + (i1 & mask) - 1;
       a0[j] = tap(c, t, b); a1[j] = tap(c, t, b + 1); a2[j] = tap(c, t, b + 2); a3[j] = tap(c, t, b + 3);
     }
