@@ -1,12 +1,12 @@
 // fundsp_b200 scalar f64 math: sin/cos/tan/exp as the Rust `libm` crate (0.2.15) ports them from musl / FreeBSD msun (k_sin.c, k_cos.c,
-// k_tan.c, e_rem_pio2.c, s_sin.c, s_cos.c, s_tan.c, e_exp.c). This is what the reference's f64 nodes call for their coefficients
-// (reference src/lib.rs:520-568: `Float for f64`). Host and device share this one implementation, so coefficients computed at lowering
-// time and those recomputed per sample on the device agree bit for bit.
+// k_tan.c, e_rem_pio2.c, k_rem_pio2.c, s_sin.c, s_cos.c, s_tan.c, e_exp.c). This is what the reference's f64 nodes call for their
+// coefficients (reference src/lib.rs:520-568: `Float for f64`). Host and device share this one implementation, so coefficients computed
+// at lowering time and those recomputed per sample on the device agree bit for bit.
 //
-// Argument reduction: |x| < 2^20 * pi/2 is reduced with e_rem_pio2's Cody-Waite steps (three rounds at most, exact to 151 bits).
-// Larger finite arguments (k_rem_pio2.c's Payne-Hanek path) are NOT restated: they go to the platform's sin/cos/tan (CUDA's on the
-// device, the C library's on the host), which may differ from msun in the last bit and between host and device. No node reaches
-// them: the filters evaluate tan(pi * f / sr) and cos(tau * f / sr) for audible f.
+// Argument reduction: |x| < 2^20 * pi/2 is reduced with e_rem_pio2's Cody-Waite steps (three rounds at most, exact to 151 bits); every
+// larger finite argument with k_rem_pio2's Payne-Hanek path at prec 1 (rem_pio2_large). No path calls the platform's sin/cos/tan (CUDA's
+// on the device, the C library's on the host): they differ from msun and from each other. The filters reach the large path: an
+// audio-rate cutoff of 2.52e10 Hz at 48 kHz puts tan(pi * f / sr) past 2^20 * pi/2, and nothing clamps a control input.
 #pragma once
 #include "libm.cuh"
 
@@ -125,27 +125,122 @@ FDSP_HD Rem rem_pio2_k(double x, int k, bool neg) {   // |x| near k pi/2, k = 1.
   else { const double z = x + P1; q.y0 = z + P1T; q.y1 = (z - q.y0) + P1T; q.n = -k; }
   return q;
 }
-// true when x is reduced here; false for |x| >= 2^20 pi/2 (the large-argument path this file does not restate)
-FDSP_HD bool rem_pio2(double x, Rem& q) {
+// k_rem_pio2.c's __rem_pio2_large(tx, ty, e0, nx, 1) for finite x: |x| = (tx[0] + tx[1] 2^-24 + tx[2] 2^-48) 2^e0 in up to three
+// 24-bit pieces, jk = 4, and prec 1's fold of fq[] into two doubles. Payne-Hanek: only the digits of 2/pi that reach the fraction of
+// x 2/pi are multiplied, 24 bits at a time; when the fraction cancels, more digits are taken and the product recomputed. Returns n with
+// the sign of x (|n| <= 7) and x - n pi/2 = y0 + y1. Out of line on the device: a cold path with five small local arrays.
+FDSP_HD_COLD Rem rem_pio2_large(double x) {
+  // 2/pi in 24-bit digits. The largest finite double has e0 = 1023 - 23 = 1000, so jv = (e0 - 3) / 24 <= 41 and the first product reads
+  // digits up to jv + jk = 45. Recomputation reads one more digit per zero digit of the fraction: the double nearest a multiple of
+  // pi/2 (0x7506ac5b262ca1ff, whose remainder is 2^-61 of its size) needs three, so no argument reads past digit 48 of these 66.
+  static const int32_t ipio2[66] = {
+    0xA2F983, 0x6E4E44, 0x1529FC, 0x2757D1, 0xF534DD, 0xC0DB62, 0x95993C, 0x439041, 0xFE5163, 0xABDEBB, 0xC561B7, 0x246E3A,
+    0x424DD2, 0xE00649, 0x2EEA09, 0xD1921C, 0xFE1DEB, 0x1CB129, 0xA73EE8, 0x8235F5, 0x2EBB44, 0x84E99C, 0x7026B4, 0x5F7E41,
+    0x3991D6, 0x398353, 0x39F49C, 0x845F8B, 0xBDF928, 0x3B1FF8, 0x97FFDE, 0x05980F, 0xEF2F11, 0x8B5A0A, 0x6D1F6D, 0x367ECF,
+    0x27CB09, 0xB74F46, 0x3F669E, 0x5FEA2D, 0x7527BA, 0xC7EBE5, 0xF17B3D, 0x0739F7, 0x8A5292, 0xEA6BFB, 0x5FB11F, 0x8D5D08,
+    0x560330, 0x46FC7B, 0x6BABF0, 0xCFBC20, 0x9AF436, 0x1DA9E3, 0x91615E, 0xE61B08, 0x659985, 0x5F14A0, 0x68408D, 0xFFD880,
+    0x4D7327, 0x310606, 0x1556CA, 0x73A8C9, 0x60E27B, 0xC08C6B};
+  static const uint64_t PIO2[5] = {   // pi/2 in 24-bit pieces (prec 1 reads jp + 1 = 5 of them)
+    0x3FF921FB40000000ull, 0x3E74442D00000000ull, 0x3CF8469880000000ull, 0x3B78CC5160000000ull, 0x39F01B8380000000ull};
+  const int jk = 4;
+  const uint64_t ux = dbits(x);
+  const int e0 = (int)((ux >> 52) & 0x7ff) - (0x3ff + 23);                          // ilogb(|x|) - 23
+  double z = dfromb((ux & 0x000fffffffffffffull) | ((uint64_t)(0x3ff + 23) << 52));   // |x| 2^-e0, in [2^23, 2^24)
+  double tx[3];
+  tx[0] = (double)(int32_t)z; z = (z - tx[0]) * 0x1p24;
+  tx[1] = (double)(int32_t)z; z = (z - tx[1]) * 0x1p24;
+  tx[2] = z;
+  int jx = 2;
+  while (jx > 0 && tx[jx] == 0.0) jx--;                         // nx - 1: trailing zero pieces dropped, the first is never zero
+  int jv = (e0 - 3) / 24;
+  if (jv < 0) jv = 0;
+  int q0 = e0 - 24 * (jv + 1), jz = jk, n, ih, i, j, k;
+  double f[20], q[20], fq[20], fw;
+  int32_t iq[20];
+  for (i = 0, j = jv - jx; i <= jx + jk; i++, j++) f[i] = j < 0 ? 0.0 : (double)ipio2[j];
+  for (i = 0; i <= jk; i++) { for (j = 0, fw = 0.0; j <= jx; j++) fw += tx[j] * f[jx + i - j]; q[i] = fw; }
+  for (;;) {
+    for (i = 0, j = jz, z = q[jz]; j > 0; i++, j--) {             // distill q[] into 24-bit iq[], most significant last
+      fw = (double)(int32_t)(0x1p-24 * z);
+      iq[i] = (int32_t)(z - 0x1p24 * fw);
+      z = q[j - 1] + fw;
+    }
+    z = z * m::pow2d(q0);
+    z -= 8.0 * floor(z * 0.125);
+    n = (int32_t)z;
+    z -= (double)n;
+    ih = 0;
+    if (q0 > 0) { i = iq[jz - 1] >> (24 - q0); n += i; iq[jz - 1] -= i << (24 - q0); ih = iq[jz - 1] >> (23 - q0); }
+    else if (q0 == 0) ih = iq[jz - 1] >> 23;
+    else if (z >= 0.5) ih = 2;
+    if (ih > 0) {                                                 // fraction > 0.5: take 1 - fraction, n + 1
+      int carry = 0;
+      n += 1;
+      for (i = 0; i < jz; i++) {
+        j = iq[i];
+        if (carry == 0) { if (j != 0) { carry = 1; iq[i] = 0x1000000 - j; } }
+        else iq[i] = 0xffffff - j;
+      }
+      if (q0 == 1) iq[jz - 1] &= 0x7fffff;
+      else if (q0 == 2) iq[jz - 1] &= 0x3fffff;
+      if (ih == 2) { z = 1.0 - z; if (carry != 0) z -= m::pow2d(q0); }
+    }
+    if (z != 0.0) break;
+    for (j = 0, i = jz - 1; i >= jk; i--) j |= iq[i];
+    if (j != 0) break;
+    for (k = 1; iq[jk - k] == 0; k++) {}                          // cancellation: k more digits of 2/pi, then again
+    for (i = jz + 1; i <= jz + k; i++) {
+      f[jx + i] = (double)ipio2[jv + i];
+      for (j = 0, fw = 0.0; j <= jx; j++) fw += tx[j] * f[jx + i - j];
+      q[i] = fw;
+    }
+    jz += k;
+  }
+  if (z == 0.0) {                                                 // chop off zero terms
+    jz -= 1; q0 -= 24;
+    while (iq[jz] == 0) { jz--; q0 -= 24; }
+  } else {                                                        // break z into 24-bit pieces if necessary
+    z = z * m::pow2d(-q0);
+    if (z >= 0x1p24) {
+      fw = (double)(int32_t)(0x1p-24 * z);
+      iq[jz] = (int32_t)(z - 0x1p24 * fw);
+      jz += 1; q0 += 24;
+      iq[jz] = (int32_t)fw;
+    } else iq[jz] = (int32_t)z;
+  }
+  fw = m::pow2d(q0);
+  for (i = jz; i >= 0; i--) { q[i] = fw * (double)iq[i]; fw *= 0x1p-24; }
+  for (i = jz; i >= 0; i--) {                                     // PIO2[0..jp] * q[jz..0]
+    for (fw = 0.0, k = 0; k <= jk && k <= jz - i; k++) fw += dfromb(PIO2[k]) * q[i + k];
+    fq[jz - i] = fw;
+  }
+  for (fw = 0.0, i = jz; i >= 0; i--) fw += fq[i];                // prec 1: the sum, then what it left over
+  const double y0 = fw;
+  for (fw = fq[0] - fw, i = 1; i <= jz; i++) fw += fq[i];
+  n &= 7;
+  const bool neg = (ih == 0) == ((ux >> 63) != 0);               // the sign of x, flipped when the fraction was folded
+  Rem r;
+  r.y0 = neg ? -y0 : y0; r.y1 = neg ? -fw : fw; r.n = (ux >> 63) ? -n : n;
+  return r;
+}
+// x = n pi/2 + (y0 + y1) for finite x
+FDSP_HD Rem rem_pio2(double x) {
   const uint32_t ix = hiword(x) & 0x7fffffffu;
   const bool neg = (dbits(x) >> 63) != 0;
   if (ix <= 0x400f6a7au) {                                   // |x| ~<= 5pi/4
-    if ((ix & 0xfffffu) == 0x921fbu) { q = rem_pio2_medium(x, ix); return true; }   // |x| ~= pi/2 or pi: cancellation
-    q = rem_pio2_k(x, ix <= 0x4002d97cu ? 1 : 2, neg);       // 3pi/4 splits the two
-    return true;
+    if ((ix & 0xfffffu) == 0x921fbu) return rem_pio2_medium(x, ix);   // |x| ~= pi/2 or pi: cancellation
+    return rem_pio2_k(x, ix <= 0x4002d97cu ? 1 : 2, neg);    // 3pi/4 splits the two
   }
   if (ix <= 0x401c463bu) {                                   // |x| ~<= 9pi/4
     if (ix <= 0x4015fdbcu) {                                 // |x| ~<= 7pi/4
-      if (ix == 0x4012d97cu) { q = rem_pio2_medium(x, ix); return true; }            // |x| ~= 3pi/2
-      q = rem_pio2_k(x, 3, neg);
-    } else {
-      if (ix == 0x401921fbu) { q = rem_pio2_medium(x, ix); return true; }            // |x| ~= 2pi
-      q = rem_pio2_k(x, 4, neg);
+      if (ix == 0x4012d97cu) return rem_pio2_medium(x, ix);  // |x| ~= 3pi/2
+      return rem_pio2_k(x, 3, neg);
     }
-    return true;
+    if (ix == 0x401921fbu) return rem_pio2_medium(x, ix);    // |x| ~= 2pi
+    return rem_pio2_k(x, 4, neg);
   }
-  if (ix < 0x413921fbu) { q = rem_pio2_medium(x, ix); return true; }                  // |x| ~< 2^20 pi/2
-  return false;
+  if (ix < 0x413921fbu) return rem_pio2_medium(x, ix);       // |x| ~< 2^20 pi/2
+  return rem_pio2_large(x);
 }
 
 FDSP_HD double sin(double x) {   // s_sin.c
@@ -155,8 +250,7 @@ FDSP_HD double sin(double x) {   // s_sin.c
     return k_sin(x, 0.0, 0);
   }
   if (ix >= 0x7ff00000u) return x - x;                       // inf or NaN
-  Rem q;
-  if (!rem_pio2(x, q)) return ::sin(x);
+  const Rem q = rem_pio2(x);
   switch (q.n & 3) {
     case 0: return k_sin(q.y0, q.y1, 1);
     case 1: return k_cos(q.y0, q.y1);
@@ -171,8 +265,7 @@ FDSP_HD double cos(double x) {   // s_cos.c
     return k_cos(x, 0.0);
   }
   if (ix >= 0x7ff00000u) return x - x;
-  Rem q;
-  if (!rem_pio2(x, q)) return ::cos(x);
+  const Rem q = rem_pio2(x);
   switch (q.n & 3) {
     case 0: return k_cos(q.y0, q.y1);
     case 1: return -k_sin(q.y0, q.y1, 1);
@@ -187,8 +280,7 @@ FDSP_HD double tan(double x) {   // s_tan.c
     return k_tan(x, 0.0, 0);
   }
   if (ix >= 0x7ff00000u) return x - x;
-  Rem q;
-  if (!rem_pio2(x, q)) return ::tan(x);
+  const Rem q = rem_pio2(x);
   return k_tan(q.y0, q.y1, q.n & 1);
 }
 

@@ -1,11 +1,12 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see fo_math.h). The f64 sin/cos/tan/exp that the reference's f64 nodes call (reference
 // src/lib.rs:520-568 -> the Rust `libm` crate, a port of musl / FreeBSD msun), restated independently of the product's
 // csrc/dsp/libm64.cuh: word access through unions, k_tan in FreeBSD's `iy = +-1` form, the near-multiples of pi/2 from a table,
-// and exp's final scaling by std::ldexp (correctly rounded, like the crate's scalbn). Arguments with |x| >= 2^20 pi/2 use the C
-// library's functions (msun's k_rem_pio2.c is not restated; the product does the same).
+// and exp's final scaling by std::ldexp (correctly rounded, like the crate's scalbn). Arguments with |x| >= 2^20 pi/2 are reduced by
+// k_rem_pio2.c's Payne-Hanek path at prec 1, restated below with its own digits of 2/pi: no trig path calls the C library's functions.
 #pragma once
 #include <cmath>
 #include <cstdint>
+#include <cstring>
 
 namespace fo {
 namespace m64 {
@@ -69,7 +70,7 @@ inline double kernel_tan(double x, double y, int iy) {
   return t + a * (s + t * v);
 }
 
-// e_rem_pio2.c for |x| < 2^20 pi/2; returns n with x = n pi/2 + y[0] + y[1]
+// e_rem_pio2.c for |x| < 2^20 pi/2 (rem_pio2_big takes the rest); returns n with x = n pi/2 + y[0] + y[1]
 inline int rem_pio2(double x, double* y) {
   const double invpio2 = hexd(0x3FE45F30, 0x6DC9C883), pio2_1 = hexd(0x3FF921FB, 0x54400000), pio2_1t = hexd(0x3DD0B461, 0x1A626331),
                pio2_2 = hexd(0x3DD0B461, 0x1A600000), pio2_2t = hexd(0x3BA3198A, 0x2E037073), pio2_3 = hexd(0x3BA3198A, 0x2E000000),
@@ -106,12 +107,130 @@ inline int rem_pio2(double x, double* y) {
   return n;
 }
 
+// k_rem_pio2.c __rem_pio2_large(x, y, e0, nx, prec) for prec 1 (init_jk[1] = 4, two doubles out): x[0..nx-1] are 24-bit pieces of
+// |arg| 2^-e0, y[0] + y[1] = |arg| - n pi/2 with n returned mod 8.
+// 2/pi to 1584 bits: 66 digits of 24 bits, the 41 + 4 that the largest double's e0 = 1000 reads at once plus room for recomputation.
+static const char TWO_OVER_PI_HEX[] =
+    "a2f9836e4e441529fc2757d1f534ddc0db6295993c439041fe5163abdebbc561b7246e3a424dd2e006492eea09d1921cfe1deb1cb129a73ee88235f5"
+    "2ebb4484e99c7026b45f7e413991d639835339f49c845f8bbdf9283b1ff897ffde05980fef2f118b5a0a6d1f6d367ecf27cb09b74f463f669e5fea2d"
+    "7527bac7ebe5f17b3d0739f78a5292ea6bfb5fb11f8d5d0856033046fc7b6babf0cfbc209af4361da9e391615ee61b086599855f14a068408dffd880"
+    "4d73273106061556ca73a8c960e27bc08c6b";
+const int TWO_OVER_PI_DIGITS = (int)(sizeof(TWO_OVER_PI_HEX) - 1) / 6;
+inline int32_t two_over_pi_digit(int k) {   // 24 bits k of the fraction of 2/pi: hex digits 6k .. 6k + 5
+  int32_t d = 0;
+  for (int h = 6 * k; h < 6 * k + 6; h++) {
+    const char c = TWO_OVER_PI_HEX[h];
+    d = d * 16 + (c <= '9' ? c - '0' : c - 'a' + 10);
+  }
+  return d;
+}
+inline int rem_pio2_large(const double* x, double* y, int e0, int nx) {
+  static const double PIo2[5] = {1.57079625129699707031e+00, 7.54978941586159635335e-08, 5.39030252995776476554e-15,
+                                 3.28200341580791294123e-22, 1.27065575308067607349e-29};
+  const int jk = 4, jp = jk;
+  int32_t jz, jx, jv, carry, n, iq[20], i, j, k, m, q0, ih;
+  double z, fw, f[20], fq[20], q[20];
+  jx = nx - 1;
+  jv = (e0 - 3) / 24; if (jv < 0) jv = 0;
+  q0 = e0 - 24 * (jv + 1);
+  j = jv - jx; m = jx + jk;
+  for (i = 0; i <= m; i++, j++) f[i] = j < 0 ? 0.0 : (double)two_over_pi_digit(j);
+  for (i = 0; i <= jk; i++) { for (j = 0, fw = 0.0; j <= jx; j++) fw += x[j] * f[jx + i - j]; q[i] = fw; }
+  jz = jk;
+recompute:
+  for (i = 0, j = jz, z = q[jz]; j > 0; i++, j--) {
+    fw = (double)(int32_t)(0x1p-24 * z);
+    iq[i] = (int32_t)(z - 0x1p24 * fw);
+    z = q[j - 1] + fw;
+  }
+  z = std::ldexp(z, q0);
+  z -= 8.0 * std::floor(z * 0.125);
+  n = (int32_t)z;
+  z -= (double)n;
+  ih = 0;
+  if (q0 > 0) {
+    i = iq[jz - 1] >> (24 - q0); n += i;
+    iq[jz - 1] -= i << (24 - q0);
+    ih = iq[jz - 1] >> (23 - q0);
+  } else if (q0 == 0) ih = iq[jz - 1] >> 23;
+  else if (z >= 0.5) ih = 2;
+  if (ih > 0) {
+    n += 1; carry = 0;
+    for (i = 0; i < jz; i++) {
+      j = iq[i];
+      if (carry == 0) {
+        if (j != 0) { carry = 1; iq[i] = 0x1000000 - j; }
+      } else iq[i] = 0xffffff - j;
+    }
+    if (q0 > 0) {
+      switch (q0) { case 1: iq[jz - 1] &= 0x7fffff; break; case 2: iq[jz - 1] &= 0x3fffff; break; }
+    }
+    if (ih == 2) { z = 1.0 - z; if (carry != 0) z -= std::ldexp(1.0, q0); }
+  }
+  if (z == 0) {
+    j = 0;
+    for (i = jz - 1; i >= jk; i--) j |= iq[i];
+    if (j == 0) {
+      for (k = 1; iq[jk - k] == 0; k++) {}
+      for (i = jz + 1; i <= jz + k; i++) {
+        f[jx + i] = (double)two_over_pi_digit(jv + i);
+        for (j = 0, fw = 0.0; j <= jx; j++) fw += x[j] * f[jx + i - j];
+        q[i] = fw;
+      }
+      jz += k;
+      goto recompute;
+    }
+  }
+  if (z == 0.0) {
+    jz -= 1; q0 -= 24;
+    while (iq[jz] == 0) { jz--; q0 -= 24; }
+  } else {
+    z = std::ldexp(z, -q0);
+    if (z >= 0x1p24) {
+      fw = (double)(int32_t)(0x1p-24 * z);
+      iq[jz] = (int32_t)(z - 0x1p24 * fw);
+      jz += 1; q0 += 24;
+      iq[jz] = (int32_t)fw;
+    } else iq[jz] = (int32_t)z;
+  }
+  fw = std::ldexp(1.0, q0);
+  for (i = jz; i >= 0; i--) { q[i] = fw * (double)iq[i]; fw *= 0x1p-24; }
+  for (i = jz; i >= 0; i--) {
+    for (fw = 0.0, k = 0; k <= jp && k <= jz - i; k++) fw += PIo2[k] * q[i + k];
+    fq[jz - i] = fw;
+  }
+  fw = 0.0;
+  for (i = jz; i >= 0; i--) fw += fq[i];
+  y[0] = ih == 0 ? fw : -fw;
+  fw = fq[0] - fw;
+  for (i = 1; i <= jz; i++) fw += fq[i];
+  y[1] = ih == 0 ? fw : -fw;
+  return n & 7;
+}
+// e_rem_pio2.c's large case for finite x: |x| 2^-e0 in [2^23, 2^24) split into three 24-bit pieces, trailing zero pieces dropped
+inline int rem_pio2_big(double x, double* y) {
+  const int e0 = std::ilogb(x) - 23;
+  double z = std::ldexp(std::fabs(x), -e0), tx[3];
+  for (int i = 0; i < 2; i++) { tx[i] = std::trunc(z); z = (z - tx[i]) * 0x1p24; }
+  tx[2] = z;
+  int nx = 3;
+  while (nx > 1 && tx[nx - 1] == 0.0) nx--;
+  double ty[2];
+  const int n = rem_pio2_large(tx, ty, e0, nx);
+  if (std::signbit(x)) { y[0] = -ty[0]; y[1] = -ty[1]; return -n; }
+  y[0] = ty[0]; y[1] = ty[1];
+  return n;
+}
+// any finite x: the medium reduction below 2^20 pi/2, the large one above
+inline int rem_pio2_any(double x, double* y) {
+  return (int32_t)(high_word(x) & 0x7fffffff) >= 0x413921fb ? rem_pio2_big(x, y) : rem_pio2(x, y);
+}
+
 inline double sin(double x) {
   const int32_t ix = (int32_t)(high_word(x) & 0x7fffffff);
   if (ix <= 0x3fe921fb) return ix < 0x3e500000 ? x : kernel_sin(x, 0.0, 0);
   if (ix >= 0x7ff00000) return x - x;
-  if (ix >= 0x413921fb) return std::sin(x);
-  double y[2]; const int n = rem_pio2(x, y);
+  double y[2]; const int n = rem_pio2_any(x, y);
   switch (n & 3) {
     case 0: return kernel_sin(y[0], y[1], 1);
     case 1: return kernel_cos(y[0], y[1]);
@@ -123,8 +242,7 @@ inline double cos(double x) {
   const int32_t ix = (int32_t)(high_word(x) & 0x7fffffff);
   if (ix <= 0x3fe921fb) return ix < 0x3e46a09e ? 1.0 : kernel_cos(x, 0.0);
   if (ix >= 0x7ff00000) return x - x;
-  if (ix >= 0x413921fb) return std::cos(x);
-  double y[2]; const int n = rem_pio2(x, y);
+  double y[2]; const int n = rem_pio2_any(x, y);
   switch (n & 3) {
     case 0: return kernel_cos(y[0], y[1]);
     case 1: return -kernel_sin(y[0], y[1], 1);
@@ -136,8 +254,7 @@ inline double tan(double x) {
   const int32_t ix = (int32_t)(high_word(x) & 0x7fffffff);
   if (ix <= 0x3fe921fb) return ix < 0x3e400000 ? x : kernel_tan(x, 0.0, 1);
   if (ix >= 0x7ff00000) return x - x;
-  if (ix >= 0x413921fb) return std::tan(x);
-  double y[2]; const int n = rem_pio2(x, y);
+  double y[2]; const int n = rem_pio2_any(x, y);
   return kernel_tan(y[0], y[1], 1 - ((n & 1) << 1));
 }
 // musl e_exp.c (the crate's exp.rs): reduce x = k ln2 + r, |r| <= ln2 / 2, rational approximation of exp(r), then scale by 2^k

@@ -10,6 +10,13 @@ API double fo64_sin(double x) { return m64::sin(x); }
 API double fo64_cos(double x) { return m64::cos(x); }
 API double fo64_tan(double x) { return m64::tan(x); }
 API double fo64_exp(double x) { return m64::exp(x); }
+// the two argument reductions of the trig functions, for finite x: n with x = n pi/2 + y[0] + y[1] (the large one returns n mod 8)
+API int fo64_rem_pio2_medium(double x, double* y) { return m64::rem_pio2(x, y); }
+API int fo64_rem_pio2_large(double x, double* y) { return m64::rem_pio2_big(x, y); }
+// fn = 0 sin, 1 cos, 2 tan, 3 exp over n arguments
+API void fo64_eval(int fn, const double* x, double* out, int64_t n) {
+  for (int64_t i = 0; i < n; i++) out[i] = fn == 0 ? m64::sin(x[i]) : fn == 1 ? m64::cos(x[i]) : fn == 2 ? m64::tan(x[i]) : m64::exp(x[i]);
+}
 API Node* fo_sine_f64() { return new Sine64(); }
 API Node* fo_fixed_svf_f64(int mode, float cutoff, float q, float gain) { return (mode < 0 || mode > 8) ? nullptr : new Svf64(mode, true, cutoff, q, gain); }
 API Node* fo_svf_f64(int mode, float cutoff, float q, float gain) { return (mode < 0 || mode > 8) ? nullptr : new Svf64(mode, false, cutoff, q, gain); }

@@ -75,6 +75,8 @@ def lib():
             "fo_envelope_in": (P, [D, I, I, S, I, C.POINTER(S), FP]),
             # fo_prelude64.cpp: the prelude64 nodes and the f64 libm
             "fo64_sin": (D, [D]), "fo64_cos": (D, [D]), "fo64_tan": (D, [D]), "fo64_exp": (D, [D]),
+            "fo64_rem_pio2_medium": (I, [D, C.POINTER(D)]), "fo64_rem_pio2_large": (I, [D, C.POINTER(D)]),
+            "fo64_eval": (None, [I, C.POINTER(D), C.POINTER(D), I64]),
             "fo_sine_f64": (P, []), "fo_fixed_svf_f64": (P, [I, F, F, F]), "fo_svf_f64": (P, [I, F, F, F]),
             "fo_biquad_f64": (P, [F, F, F, F, F]), "fo_butterpass_f64": (P, [F, I]), "fo_resonator_f64": (P, [F, F, I]),
             "fo_onepole_f64": (P, [I, F, I]), "fo_sine_f64_phase_after": (D, [U64, D, F, I]),

@@ -300,3 +300,11 @@ def test_gpu_prelude64_file_on_the_mock_device(mock_env):
                         "-p", "no:cacheprovider", "--tb=short"], capture_output=True, text=True, env=mock_env, cwd=ROOT, timeout=1800)
     tail = r.stdout[-3000:]
     assert r.returncode == 0 and " passed" in tail and "failed" not in tail, tail
+
+
+def test_gpu_prelude64_edges_file_on_the_mock_device(mock_env):
+    """tests/test_gpu_prelude64_edges.py (the filters at the edges of their control inputs) with the device templates on the host."""
+    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(ROOT, "tests", "test_gpu_prelude64_edges.py"), "-m", "gpu", "-q", "-n", "4",
+                        "-p", "no:cacheprovider", "--tb=short"], capture_output=True, text=True, env=mock_env, cwd=ROOT, timeout=1800)
+    tail = r.stdout[-3000:]
+    assert r.returncode == 0 and " passed" in tail and "failed" not in tail, tail
