@@ -1550,6 +1550,13 @@ template <class X> struct Oversample {
     Fr<NI> e, d; Fr<NO> y0, y1;
     const bool live = T || c.i < 2 * (c.n / 2);
     if (!live) {   // the odd tail sample of a block
+      if (c.n == 1) {   // process(1): both halves are empty, and each still runs X's process(1) over its one zero inner sample
+        Fr<NI> z; Fr<NO> drop;
+#pragma unroll
+        for (int k = 0; k < NI; k++) z.v[k] = 0.0f;
+        inner(r, c, 0, 1, z, drop);
+        inner(r, c, 0, 1, z, drop);
+      }
 #pragma unroll
       for (int k = 0; k < NO; k++) o.v[k] = 0.0f;
       return;
