@@ -10,9 +10,18 @@ namespace host {
 
 constexpr int NT = 128;
 
+// The opt-in a launch needs when its dynamic shared memory and the kernel's static shared memory (the staged kernel's mbarriers, for
+// one) together pass the 48 KB default: a launch whose dynamic part alone stays at or under 48 KB is refused without it. The
+// static size of each kernel is read once.
+template <auto KERNEL> cudaError_t smem_opt_in(size_t smem) {
+  static const size_t stat = [] { cudaFuncAttributes fa{}; return cudaFuncGetAttributes(&fa, KERNEL) == cudaSuccess ? fa.sharedSizeBytes : (size_t)48 * 1024; }();
+  if (smem + stat <= 48 * 1024) return cudaSuccess;
+  return cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+
 template <class G, int MODE, bool TB> cudaError_t launch_one(const BankArgs& a, unsigned grid, size_t smem, cudaStream_t st) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(bank_kernel<G, NT, MODE, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  {
+    cudaError_t e = smem_opt_in<bank_kernel<G, NT, MODE, TB>>(smem);
     if (e != cudaSuccess) return e;
   }
   if (launch_carveout() >= 0) cudaFuncSetAttribute(bank_kernel<G, NT, MODE, TB>, cudaFuncAttributePreferredSharedMemoryCarveout, launch_carveout());
@@ -32,8 +41,8 @@ template <class G, bool TB> cudaError_t launch_mode(const BankArgs& a, int mode,
 // stage-pipelined variant (bank_kernel_st.cuh): K * NTV threads per CTA, the stages of StagePlan<G> in different warps
 template <class G, int NTV, int MODE, bool TB> cudaError_t launch_st_one(const BankArgs& a, unsigned grid, size_t smem, cudaStream_t st) {
   if constexpr (StagePlan<G>::K >= 2) {
-    if (smem > 48 * 1024) {
-      cudaError_t e = cudaFuncSetAttribute(bank_kernel_st<G, NTV, MODE, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    {
+      cudaError_t e = smem_opt_in<bank_kernel_st<G, NTV, MODE, TB>>(smem);
       if (e != cudaSuccess) return e;
     }
     bank_kernel_st<G, NTV, MODE, TB><<<grid, StagePlan<G>::K * NTV, smem, st>>>(a);
@@ -76,8 +85,8 @@ template <class G> cudaError_t launch_t(const BankArgs& a, int mode, size_t tabl
 }
 // resident process() kernel (bank_kernel_rt.cuh): one launch serves 64-sample blocks on a doorbell until it is told to leave
 template <class G, bool TB> cudaError_t launch_rt_one(const BankArgs& a, const RtArgs& rt, size_t smem, cudaStream_t st) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(bank_kernel_rt<G, NT, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  {
+    cudaError_t e = smem_opt_in<bank_kernel_rt<G, NT, TB>>(smem);
     if (e != cudaSuccess) return e;
   }
   const unsigned vpc = a.vpc ? a.vpc : (unsigned)NT, grid = (a.V + vpc - 1) / vpc;

@@ -612,21 +612,26 @@ struct FixedSvf {  // src/svf.rs:857-1031, ID 43 (coefficients computed on the h
   }
   static FDSP_DEV void end_simd(R&) {}
 };
-template <int MODE> struct Svf {  // src/svf.rs:744-855, ID 36 (audio-rate cutoff/Q[/gain] inputs; recompute on change)
+// The audio-rate f32 filters keep their coefficients in state next to the controls they were computed from, and `ksr`, the rate they
+// were computed at. The reference's set_sample_rate recomputes them from the stored controls (src/svf.rs:823-826, src/biquad.rs:263-266,
+// :349-351, :535-538, :745-748, src/filter.rs:58-61, :392-395, src/rez.rs:59-62), and the next sample's change test then compares the
+// inputs with those stored controls. So a launch at another rate first recomputes from the stored controls, then runs the usual test.
+template <int MODE> struct Svf {  // src/svf.rs:744-855, ID 36 (audio-rate cutoff/Q[/gain] inputs; recompute on change or rate change)
   static constexpr int NI = MODE >= 6 ? 4 : 3;
-  FDSP_NODE(NI, 1, 0, 11, 0);
-  struct R { float cutoff, q, gain; SvfCoefs k; float ic1, ic2; };
+  FDSP_NODE(NI, 1, 0, 12, 0);
+  struct R { float cutoff, q, gain, ksr; SvfCoefs k; float ic1, ic2; };
   static FDSP_DEV void load(R& r, Loader& l) {
-    r.cutoff = l.Sf(); r.q = l.Sf(); r.gain = l.Sf();
+    r.cutoff = l.Sf(); r.q = l.Sf(); r.gain = l.Sf(); r.ksr = l.Sf();
     r.k.a1 = l.Sf(); r.k.a2 = l.Sf(); r.k.a3 = l.Sf(); r.k.m0 = l.Sf(); r.k.m1 = l.Sf(); r.k.m2 = l.Sf();
     r.ic1 = l.Sf(); r.ic2 = l.Sf();
   }
   static FDSP_DEV void save(const R& r, Saver& s) {
-    s.Sf(r.cutoff); s.Sf(r.q); s.Sf(r.gain);
+    s.Sf(r.cutoff); s.Sf(r.q); s.Sf(r.gain); s.Sf(r.ksr);
     s.Sf(r.k.a1); s.Sf(r.k.a2); s.Sf(r.k.a3); s.Sf(r.k.m0); s.Sf(r.k.m1); s.Sf(r.k.m2);
     s.Sf(r.ic1); s.Sf(r.ic2);
   }
   template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<NI>& in, Fr<1>& o) {
+    if (r.ksr != c.sr) { r.ksr = c.sr; r.k = svf_coefs<MODE>(c.sr, r.cutoff, r.q, r.gain); }
     bool ch = in.v[1] != r.cutoff || in.v[2] != r.q;
     if (MODE >= 6) ch = ch || in.v[NI - 1] != r.gain;
     if (ch) { r.cutoff = in.v[1]; r.q = in.v[2]; if (MODE >= 6) r.gain = in.v[NI - 1]; r.k = svf_coefs<MODE>(c.sr, r.cutoff, r.q, r.gain); }
@@ -655,17 +660,18 @@ struct Morph {  // src/svf.rs:1034-1111, ID 62: (peak SVF(audio, cutoff, q) + mo
   static FDSP_DEV void end_simd(R&) {}
 };
 template <int NIN> struct Rez {  // src/rez.rs, ID 75: params = bandpass (and f, fb when the cutoff / q are fixed)
-  FDSP_NODE(NIN, 1, NIN == 1 ? 3 : 1, NIN == 1 ? 2 : 6, 0);
-  struct R { float bandpass, f, fb, cutoff, q, buf0, buf1; };
+  FDSP_NODE(NIN, 1, NIN == 1 ? 3 : 1, NIN == 1 ? 2 : 7, 0);
+  struct R { float bandpass, f, fb, cutoff, q, ksr, buf0, buf1; };
   static FDSP_DEV void load(R& r, Loader& l) {
     r.bandpass = l.Pf();
-    if (NIN == 1) { r.f = l.Pf(); r.fb = l.Pf(); r.cutoff = r.q = 0.0f; } else { r.cutoff = l.Sf(); r.q = l.Sf(); r.f = l.Sf(); r.fb = l.Sf(); }
+    if (NIN == 1) { r.f = l.Pf(); r.fb = l.Pf(); r.cutoff = r.q = r.ksr = 0.0f; } else { r.cutoff = l.Sf(); r.q = l.Sf(); r.ksr = l.Sf(); r.f = l.Sf(); r.fb = l.Sf(); }
     r.buf0 = l.Sf(); r.buf1 = l.Sf();
   }
-  static FDSP_DEV void save(const R& r, Saver& s) { if (NIN > 1) { s.Sf(r.cutoff); s.Sf(r.q); s.Sf(r.f); s.Sf(r.fb); } s.Sf(r.buf0); s.Sf(r.buf1); }
+  static FDSP_DEV void save(const R& r, Saver& s) { if (NIN > 1) { s.Sf(r.cutoff); s.Sf(r.q); s.Sf(r.ksr); s.Sf(r.f); s.Sf(r.fb); } s.Sf(r.buf0); s.Sf(r.buf1); }
   template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<NIN>& in, Fr<1>& o) {
     if (NIN > 1) {
       const float cu = in.v[NIN > 1 ? 1 : 0], qq = in.v[NIN > 2 ? 2 : 0];
+      if (r.ksr != c.sr) { r.ksr = c.sr; r.f = 2.0f * m::sinf_(3.14159274101257324f * r.cutoff / c.sr); r.fb = r.q + r.q / (1.0f - r.f); }
       if (cu != r.cutoff || qq != r.q) { r.cutoff = cu; r.q = qq; r.f = 2.0f * m::sinf_(3.14159274101257324f * cu / c.sr); r.fb = qq + qq / (1.0f - r.f); }
     }
     const float hp = in.v[0] - r.buf0, bp = r.buf0 - r.buf1;
@@ -902,24 +908,27 @@ template <int NT_, int LINEAR> struct Tap {  // Tap<N> ID 50 (Catmull-Rom) / Tap
 
 // ---------------------------------------------------------------- biquads with audio-rate parameters (src/biquad.rs:220-382)
 struct ButterLowpass2 {  // ButterLowpass<f32,U2>, ID 16: (audio, cutoff) -> 1, coefficients recomputed when the cutoff input changes
-  FDSP_NODE(2, 1, 0, 10, 0);
-  struct R { float cutoff; Biquad::R b; };
-  static FDSP_DEV void load(R& r, Loader& l) { r.cutoff = l.Sf(); r.b.a1 = l.Sf(); r.b.a2 = l.Sf(); r.b.b0 = l.Sf(); r.b.b1 = l.Sf(); r.b.b2 = l.Sf(); r.b.x1 = l.Sf(); r.b.x2 = l.Sf(); r.b.y1 = l.Sf(); r.b.y2 = l.Sf(); }
-  static FDSP_DEV void save(const R& r, Saver& s) { s.Sf(r.cutoff); s.Sf(r.b.a1); s.Sf(r.b.a2); s.Sf(r.b.b0); s.Sf(r.b.b1); s.Sf(r.b.b2); s.Sf(r.b.x1); s.Sf(r.b.x2); s.Sf(r.b.y1); s.Sf(r.b.y2); }
+  FDSP_NODE(2, 1, 0, 11, 0);
+  static FDSP_DEV void set(Biquad::R& b, const BqCoefs& k) { b.a1 = k.a1; b.a2 = k.a2; b.b0 = k.b0; b.b1 = k.b1; b.b2 = k.b2; }
+  struct R { float cutoff, ksr; Biquad::R b; };
+  static FDSP_DEV void load(R& r, Loader& l) { r.cutoff = l.Sf(); r.ksr = l.Sf(); r.b.a1 = l.Sf(); r.b.a2 = l.Sf(); r.b.b0 = l.Sf(); r.b.b1 = l.Sf(); r.b.b2 = l.Sf(); r.b.x1 = l.Sf(); r.b.x2 = l.Sf(); r.b.y1 = l.Sf(); r.b.y2 = l.Sf(); }
+  static FDSP_DEV void save(const R& r, Saver& s) { s.Sf(r.cutoff); s.Sf(r.ksr); s.Sf(r.b.a1); s.Sf(r.b.a2); s.Sf(r.b.b0); s.Sf(r.b.b1); s.Sf(r.b.b2); s.Sf(r.b.x1); s.Sf(r.b.x2); s.Sf(r.b.y1); s.Sf(r.b.y2); }
   template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<2>& in, Fr<1>& o) {
-    if (in.v[1] != r.cutoff) { r.cutoff = in.v[1]; BqCoefs k = bq_butter_lowpass(c.sr, r.cutoff); r.b.a1 = k.a1; r.b.a2 = k.a2; r.b.b0 = k.b0; r.b.b1 = k.b1; r.b.b2 = k.b2; }
+    if (r.ksr != c.sr) { r.ksr = c.sr; set(r.b, bq_butter_lowpass(c.sr, r.cutoff)); }
+    if (in.v[1] != r.cutoff) { r.cutoff = in.v[1]; set(r.b, bq_butter_lowpass(c.sr, r.cutoff)); }
     Fr<1> a; a.v[0] = in.v[0];
     Biquad::step<T>(r.b, c, a, o);
   }
   static FDSP_DEV void end_simd(R&) {}
 };
 struct Resonator3 {  // Resonator<f32,U3>, ID 17: (audio, center, q) -> 1
-  FDSP_NODE(3, 1, 0, 11, 0);
-  struct R { float center, q; Biquad::R b; };
-  static FDSP_DEV void load(R& r, Loader& l) { r.center = l.Sf(); r.q = l.Sf(); r.b.a1 = l.Sf(); r.b.a2 = l.Sf(); r.b.b0 = l.Sf(); r.b.b1 = l.Sf(); r.b.b2 = l.Sf(); r.b.x1 = l.Sf(); r.b.x2 = l.Sf(); r.b.y1 = l.Sf(); r.b.y2 = l.Sf(); }
-  static FDSP_DEV void save(const R& r, Saver& s) { s.Sf(r.center); s.Sf(r.q); s.Sf(r.b.a1); s.Sf(r.b.a2); s.Sf(r.b.b0); s.Sf(r.b.b1); s.Sf(r.b.b2); s.Sf(r.b.x1); s.Sf(r.b.x2); s.Sf(r.b.y1); s.Sf(r.b.y2); }
+  FDSP_NODE(3, 1, 0, 12, 0);
+  struct R { float center, q, ksr; Biquad::R b; };
+  static FDSP_DEV void load(R& r, Loader& l) { r.center = l.Sf(); r.q = l.Sf(); r.ksr = l.Sf(); r.b.a1 = l.Sf(); r.b.a2 = l.Sf(); r.b.b0 = l.Sf(); r.b.b1 = l.Sf(); r.b.b2 = l.Sf(); r.b.x1 = l.Sf(); r.b.x2 = l.Sf(); r.b.y1 = l.Sf(); r.b.y2 = l.Sf(); }
+  static FDSP_DEV void save(const R& r, Saver& s) { s.Sf(r.center); s.Sf(r.q); s.Sf(r.ksr); s.Sf(r.b.a1); s.Sf(r.b.a2); s.Sf(r.b.b0); s.Sf(r.b.b1); s.Sf(r.b.b2); s.Sf(r.b.x1); s.Sf(r.b.x2); s.Sf(r.b.y1); s.Sf(r.b.y2); }
   template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<3>& in, Fr<1>& o) {
-    if (in.v[1] != r.center || in.v[2] != r.q) { r.center = in.v[1]; r.q = in.v[2]; BqCoefs k = bq_resonator(c.sr, r.center, r.q); r.b.a1 = k.a1; r.b.a2 = k.a2; r.b.b0 = k.b0; r.b.b1 = k.b1; r.b.b2 = k.b2; }
+    if (r.ksr != c.sr) { r.ksr = c.sr; ButterLowpass2::set(r.b, bq_resonator(c.sr, r.center, r.q)); }
+    if (in.v[1] != r.center || in.v[2] != r.q) { r.center = in.v[1]; r.q = in.v[2]; ButterLowpass2::set(r.b, bq_resonator(c.sr, r.center, r.q)); }
     Fr<1> a; a.v[0] = in.v[0];
     Biquad::step<T>(r.b, c, a, o);
   }
@@ -1010,20 +1019,25 @@ template <int HAD, class X, class Y> struct Feedback2 {  // src/feedback.rs:180-
 
 // ---------------------------------------------------------------- one-pole family (src/filter.rs, F = f32)
 // KIND 0 Lowpole (ID 18), 1 Highpole (ID 47), 2 Allpole (ID 46), 3 DCBlock (ID 22); NIN = 2 adds the audio-rate parameter input
-// (cutoff: coefficient recomputed when it changes, :65-70 / :399-404; allpole delay: every sample, :315-317).
+// (cutoff: coefficient recomputed when it or the rate changes, :65-70 / :399-404, `ksr` as in Svf; allpole delay: every sample, :315-317).
 template <int KIND, int NIN> struct OnePole {
-  FDSP_NODE(NIN, 1, NIN == 1 ? 1 : 0, (KIND == 0 ? 1 : 2) + (NIN > 1 ? 2 : 0), 0);
-  struct R { float coeff, param, x1, y1; };
+  static constexpr bool KSR = NIN > 1 && KIND != 2;
+  FDSP_NODE(NIN, 1, NIN == 1 ? 1 : 0, (KIND == 0 ? 1 : 2) + (NIN > 1 ? 2 : 0) + (KSR ? 1 : 0), 0);
+  struct R { float coeff, param, ksr, x1, y1; };
   static FDSP_DEV void load(R& r, Loader& l) {
     if (NIN == 1) { r.coeff = l.Pf(); r.param = 0.0f; } else { r.param = l.Sf(); r.coeff = l.Sf(); }
+    r.ksr = KSR ? l.Sf() : 0.0f;
     r.x1 = (KIND == 0) ? 0.0f : l.Sf(); r.y1 = l.Sf();
   }
-  static FDSP_DEV void save(const R& r, Saver& s) { if (NIN > 1) { s.Sf(r.param); s.Sf(r.coeff); } if (KIND != 0) s.Sf(r.x1); s.Sf(r.y1); }
+  static FDSP_DEV void save(const R& r, Saver& s) { if (NIN > 1) { s.Sf(r.param); s.Sf(r.coeff); } if (KSR) s.Sf(r.ksr); if (KIND != 0) s.Sf(r.x1); s.Sf(r.y1); }
   template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<NIN>& in, Fr<1>& o) {
     if (NIN > 1) {
       const float p = in.v[NIN > 1 ? 1 : 0];
       if (KIND == 2) r.coeff = (1.0f - p) / (1.0f + p);
-      else if (p != r.param) { r.param = p; r.coeff = m::expf_(-TAU_F * p / c.sr); }
+      else {
+        if (r.ksr != c.sr) { r.ksr = c.sr; r.coeff = m::expf_(-TAU_F * r.param / c.sr); }
+        if (p != r.param) { r.param = p; r.coeff = m::expf_(-TAU_F * p / c.sr); }
+      }
     }
     const float x = in.v[0];
     float y0;
@@ -1166,7 +1180,8 @@ template <int INNER> struct ShaperAdaptive {
 //   BqShape<KIND>: a Shaper kind (0..6) with its words p0, p1;
 //   BqShapeAdaptive<INNER>: Adaptive around a Shaper kind, words smoothing, p0, p1 and one level estimate per clone. The biquads'
 //   set_sample_rate does not reach the shape (:536-539, :745-748), so `smoothing` is the one Adaptive::new computed at 44.1 kHz.
-// Words: P shape words [, a1, a2, b0, b1, b2 for NIN 1]; S [center, q, gain, a1, a2, b0, b1, b2 for NIN > 1], s1, s2, shape1 [, shape2] state.
+//   A rate change recomputes the audio-rate coefficients at the next sample (`ksr`, as in Svf).
+// Words: P shape words [, a1, a2, b0, b1, b2 for NIN 1]; S [center, q, gain, ksr, a1, a2, b0, b1, b2 for NIN > 1], s1, s2, shape1 [, shape2] state.
 template <int KIND> struct BqShape {
   static constexpr int NP = 2, NS = 0;
   struct P { float p0, p1; };
@@ -1186,17 +1201,17 @@ template <int INNER> struct BqShapeAdaptive {
   static FDSP_DEV float shape(const P& p, S& s, float x) { s.st = adaptive_level(p.sm, s.st, x); return shape_tick<INNER>(p.p0, p.p1, x / sqrtf(s.st)); }
 };
 template <int FB, int MODE, class SH, int NIN> struct NlBiquadT {
-  FDSP_NODE(NIN, 1, SH::NP + (NIN == 1 ? 5 : 0), 2 + (NIN > 1 ? 8 : 0) + (FB ? 1 : 2) * SH::NS, 0);
-  struct R { typename SH::P sp; BqCoefs k; float center, q, gain, s1, s2; typename SH::S sh1, sh2; };
+  FDSP_NODE(NIN, 1, SH::NP + (NIN == 1 ? 5 : 0), 2 + (NIN > 1 ? 9 : 0) + (FB ? 1 : 2) * SH::NS, 0);
+  struct R { typename SH::P sp; BqCoefs k; float center, q, gain, ksr, s1, s2; typename SH::S sh1, sh2; };
   static FDSP_DEV void load(R& r, Loader& l) {
     SH::load_p(r.sp, l);
-    if (NIN == 1) { r.k.a1 = l.Pf(); r.k.a2 = l.Pf(); r.k.b0 = l.Pf(); r.k.b1 = l.Pf(); r.k.b2 = l.Pf(); r.center = r.q = r.gain = 0.0f; }
-    else { r.center = l.Sf(); r.q = l.Sf(); r.gain = l.Sf(); r.k.a1 = l.Sf(); r.k.a2 = l.Sf(); r.k.b0 = l.Sf(); r.k.b1 = l.Sf(); r.k.b2 = l.Sf(); }
+    if (NIN == 1) { r.k.a1 = l.Pf(); r.k.a2 = l.Pf(); r.k.b0 = l.Pf(); r.k.b1 = l.Pf(); r.k.b2 = l.Pf(); r.center = r.q = r.gain = r.ksr = 0.0f; }
+    else { r.center = l.Sf(); r.q = l.Sf(); r.gain = l.Sf(); r.ksr = l.Sf(); r.k.a1 = l.Sf(); r.k.a2 = l.Sf(); r.k.b0 = l.Sf(); r.k.b1 = l.Sf(); r.k.b2 = l.Sf(); }
     r.s1 = l.Sf(); r.s2 = l.Sf();
     SH::load_s(r.sh1, l); if (!FB) SH::load_s(r.sh2, l);
   }
   static FDSP_DEV void save(const R& r, Saver& s) {
-    if (NIN > 1) { s.Sf(r.center); s.Sf(r.q); s.Sf(r.gain); s.Sf(r.k.a1); s.Sf(r.k.a2); s.Sf(r.k.b0); s.Sf(r.k.b1); s.Sf(r.k.b2); }
+    if (NIN > 1) { s.Sf(r.center); s.Sf(r.q); s.Sf(r.gain); s.Sf(r.ksr); s.Sf(r.k.a1); s.Sf(r.k.a2); s.Sf(r.k.b0); s.Sf(r.k.b1); s.Sf(r.k.b2); }
     s.Sf(r.s1); s.Sf(r.s2);
     SH::save_s(r.sh1, s); if (!FB) SH::save_s(r.sh2, s);
   }
@@ -1205,6 +1220,7 @@ template <int FB, int MODE, class SH, int NIN> struct NlBiquadT {
       const float ce = in.v[NIN > 1 ? 1 : 0], qq = in.v[NIN > 2 ? 2 : 0], gg = NIN > 3 ? in.v[NIN > 3 ? 3 : 0] : r.gain;
       const float dc = ce - r.center, dq = qq - r.q, dg = gg - r.gain;
       const float test = NIN > 3 ? dc * dc + dq * dq + dg * dg : dc * dc + dq * dq;
+      if (r.ksr != c.sr) { r.ksr = c.sr; r.k = bq_mode(MODE, c.sr, r.center, r.q, r.gain); }
       if (test != 0.0f) { r.center = ce; r.q = qq; r.gain = gg; r.k = bq_mode(MODE, c.sr, ce, qq, gg); }
     }
     const float x0 = in.v[0];

@@ -231,7 +231,7 @@ struct Svf : HNode {  // FixedSvf (ID 43, :857-1031) and Svf (ID 36, :744-855)
   void lower(Lowering& l) const override {
     Coefs6 c = svf_coefs(mode, sr, cutoff, q, gain);
     if (fixed) { l.p(c.a1); l.p(c.a2); l.p(c.a3); l.p(c.m0); l.p(c.m1); l.p(c.m2); l.s(0.0f); l.s(0.0f); }
-    else { l.s(cutoff); l.s(q); l.s(gain); l.s(c.a1); l.s(c.a2); l.s(c.a3); l.s(c.m0); l.s(c.m1); l.s(c.m2); l.s(0.0f); l.s(0.0f); }
+    else { l.s(cutoff); l.s(q); l.s(gain); l.s(sr); l.s(c.a1); l.s(c.a2); l.s(c.a3); l.s(c.m0); l.s(c.m1); l.s(c.m2); l.s(0.0f); l.s(0.0f); }
   }
   HCLONE(Svf)
 };
@@ -370,7 +370,7 @@ struct RezN : HNode {  // src/rez.rs
   void sig(std::string& o) const override { o += "Rez<" + I(nin) + ">"; }
   void lower(Lowering& l) const override {
     l.p(bandpass);
-    if (nin == 1) { l.p(f); l.p(fb); } else { l.s(cutoff); l.s(q); l.s(f); l.s(fb); }
+    if (nin == 1) { l.p(f); l.p(fb); } else { l.s(cutoff); l.s(q); l.s(sr); l.s(f); l.s(fb); }
     l.s(0.0f); l.s(0.0f);
   }
   HCLONE(RezN)
@@ -397,7 +397,8 @@ struct Biquad : HNode {  // Biquad (ID 15), fixed ButterLowpass (ID 16), fixed R
   void sig(std::string& o) const override { o += nin == 1 ? "Biquad" : (kind == 1 ? "ButterLowpass2" : "Resonator3"); }
   void lower(Lowering& l) const override {
     if (nin == 1) { l.p(c.a1); l.p(c.a2); l.p(c.b0); l.p(c.b1); l.p(c.b2); for (int i = 0; i < 4; i++) l.s(0.0f); return; }
-    l.s(f); if (kind == 2) l.s(q);   // audio-rate parameter inputs: the current cutoff / (center, q) and coefficients are state
+    l.s(f); if (kind == 2) l.s(q);   // audio-rate parameter inputs: the current cutoff / (center, q), the rate and the coefficients are state
+    l.s(sr);
     l.s(c.a1); l.s(c.a2); l.s(c.b0); l.s(c.b1); l.s(c.b2); for (int i = 0; i < 4; i++) l.s(0.0f);
   }
   HCLONE(Biquad)
@@ -565,7 +566,7 @@ struct OnePoleN : HNode {  // src/filter.rs: kind 0 Lowpole, 1 Highpole, 2 Allpo
   void sig(std::string& o) const override { if (kind == 4) o += "Pinkpass"; else o += "OnePole<" + I(kind) + "," + I(nin) + ">"; }
   void lower(Lowering& l) const override {
     if (kind == 4) { for (int k = 0; k < 7; k++) l.s(0.0f); return; }
-    if (nin == 1) l.p(coeff); else { l.s(param); l.s(coeff); }
+    if (nin == 1) l.p(coeff); else { l.s(param); l.s(coeff); if (kind != 2) l.s(sr); }
     if (kind != 0) l.s(0.0f);
     l.s(0.0f);
   }
@@ -665,7 +666,7 @@ struct NlBiquadN : HNode {  // src/biquad.rs:494-920
   }
   void lower_filter(Lowering& l) const {
     if (nin == 1) { l.p(c.a1); l.p(c.a2); l.p(c.b0); l.p(c.b1); l.p(c.b2); }
-    else { l.s(center); l.s(q); l.s(gain); l.s(c.a1); l.s(c.a2); l.s(c.b0); l.s(c.b1); l.s(c.b2); }
+    else { l.s(center); l.s(q); l.s(gain); l.s(sr); l.s(c.a1); l.s(c.a2); l.s(c.b0); l.s(c.b1); l.s(c.b2); }
     l.s(0.0f); l.s(0.0f);
   }
   HCLONE(NlBiquadN)

@@ -48,6 +48,7 @@ struct Api {
   CUresult (*FuncSetAttribute)(CUfunction, CUfunction_attribute, int);
   CUresult (*LaunchKernel)(CUfunction, unsigned, unsigned, unsigned, unsigned, unsigned, unsigned, unsigned, CUstream, void**, void**);
   CUresult (*GetErrorString)(CUresult, const char**);
+  CUresult (*FuncGetAttribute)(int*, CUfunction_attribute, CUfunction);
 };
 
 template <class F> bool sym(void* lib, const char* name, F& f) { f = reinterpret_cast<F>(dlsym(lib, name)); return f != nullptr; }
@@ -71,7 +72,8 @@ Api& api() {
     bool ok = sym(a.cuda, "cuModuleLoadData", a.ModuleLoadData) &&
               sym(a.cuda, "cuModuleGetFunction", a.ModuleGetFunction) && sym(a.cuda, "cuModuleGetGlobal_v2", a.ModuleGetGlobal) &&
               sym(a.cuda, "cuMemcpyDtoH_v2", a.MemcpyDtoH) && sym(a.cuda, "cuFuncSetAttribute", a.FuncSetAttribute) &&
-              sym(a.cuda, "cuLaunchKernel", a.LaunchKernel) && sym(a.cuda, "cuGetErrorString", a.GetErrorString);
+              sym(a.cuda, "cuLaunchKernel", a.LaunchKernel) && sym(a.cuda, "cuGetErrorString", a.GetErrorString) &&
+              sym(a.cuda, "cuFuncGetAttribute", a.FuncGetAttribute);
     if (!ok) { a.why = "missing NVRTC / driver symbols"; return; }
     a.ok = true;
   });
@@ -175,6 +177,25 @@ static std::string kernel_expr_of(int mode, int tb, int width) {
   return width ? "fdsp::bank_kernel_st<fdsp::JitG, " + std::to_string(width) + ", " + tail : "fdsp::bank_kernel<fdsp::JitG, 128, " + tail;
 }
 
+// a launch the driver refuses keeps the driver's reason: its launch error codes are the runtime's (CUDA_ERROR_INVALID_VALUE ==
+// cudaErrorInvalidValue, CUDA_ERROR_LAUNCH_OUT_OF_RESOURCES == cudaErrorLaunchOutOfResources, ...), so they are passed on as they are
+static cudaError_t launch_result(CUresult r, const char* what) {
+  if (r == CUDA_SUCCESS) return cudaSuccess;
+  const char* s = nullptr;
+  if (api().GetErrorString(r, &s) != CUDA_SUCCESS) s = nullptr;
+  fprintf(stderr, "fundsp_b200 JIT: %s: cuLaunchKernel: %s (%d)\n", what, s ? s : "unknown error", (int)r);
+  return (cudaError_t)r;
+}
+
+// the opt-in a launch needs when its dynamic shared memory and the kernel's static shared memory together pass the 48 KB default
+// (as smem_opt_in in dsp/launch.cuh)
+static bool smem_opt_in(CUfunction f, size_t smem) {
+  const Api& A = api();
+  int stat = 48 * 1024;
+  if (A.FuncGetAttribute(&stat, CU_FUNC_ATTRIBUTE_SHARED_SIZE_BYTES, f) != CUDA_SUCCESS) stat = 48 * 1024;
+  return smem + (size_t)stat <= 48 * 1024 || A.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem) == CUDA_SUCCESS;
+}
+
 struct JitProgram : Program {
   int device = 0, mid_sum = 0;   // mid_sum: channels crossing the stage boundaries (sizes the hand-off rings)
   mutable std::mutex mu;
@@ -202,13 +223,12 @@ struct JitProgram : Program {
     CUfunction f = variant(2, tb, -1);
     if (!f) return cudaErrorInvalidDeviceFunction;
     const size_t smem = tile + (tb ? table_bytes : 0);
-    if (smem > 48 * 1024 && A.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem) != CUDA_SUCCESS) return cudaErrorInvalidValue;
+    if (!smem_opt_in(f, smem)) return cudaErrorInvalidValue;
     if (launch_carveout() >= 0) A.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_PREFERRED_SHARED_MEMORY_CARVEOUT, launch_carveout());
     BankArgs args = a; RtArgs r = rt;
     void* params[] = {&args, &r};
     const unsigned vpc = a.vpc ? a.vpc : (unsigned)threads, grid = (a.V + vpc - 1) / vpc;
-    CUresult rc = A.LaunchKernel(f, grid, 1, 1, (unsigned)threads, 1, 1, (unsigned)smem, (CUstream)st, params, nullptr);
-    return rc == CUDA_SUCCESS ? cudaSuccess : cudaErrorLaunchFailure;
+    return launch_result(A.LaunchKernel(f, grid, 1, 1, (unsigned)threads, 1, 1, (unsigned)smem, (CUstream)st, params, nullptr), "resident kernel");
   }
   cudaError_t launch_staged(const BankArgs& a, int mode, size_t table_bytes, cudaStream_t st) const override {
     const Api& A = api();
@@ -223,13 +243,12 @@ struct JitProgram : Program {
     if (smem > 227 * 1024) return cudaErrorInvalidValue;
     CUfunction f = variant(mode, tb, width);
     if (!f) return cudaErrorInvalidDeviceFunction;
-    if (smem > 48 * 1024 && A.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem) != CUDA_SUCCESS) return cudaErrorInvalidValue;
+    if (!smem_opt_in(f, smem)) return cudaErrorInvalidValue;
     if (launch_carveout() >= 0) A.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_PREFERRED_SHARED_MEMORY_CARVEOUT, launch_carveout());
     BankArgs args = a;
     void* params[] = {&args};
     const unsigned vpc = a.vpc ? a.vpc : (unsigned)width, grid = (a.V + vpc - 1) / vpc;
-    CUresult r = A.LaunchKernel(f, grid, 1, 1, (unsigned)(stages * width), 1, 1, (unsigned)smem, (CUstream)st, params, nullptr);
-    return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorLaunchFailure;
+    return launch_result(A.LaunchKernel(f, grid, 1, 1, (unsigned)(stages * width), 1, 1, (unsigned)smem, (CUstream)st, params, nullptr), "staged kernel");
   }
   cudaError_t launch(const BankArgs& a, int mode, size_t table_bytes, cudaStream_t st) const override {
     const Api& A = api();
@@ -240,13 +259,12 @@ struct JitProgram : Program {
     CUfunction f = variant(mode, tb);
     if (!f) return cudaErrorInvalidDeviceFunction;
     const size_t smem = tile + (tb ? table_bytes : 0);
-    if (smem > 48 * 1024 && A.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, (int)smem) != CUDA_SUCCESS) return cudaErrorInvalidValue;
+    if (!smem_opt_in(f, smem)) return cudaErrorInvalidValue;
     if (launch_carveout() >= 0) A.FuncSetAttribute(f, CU_FUNC_ATTRIBUTE_PREFERRED_SHARED_MEMORY_CARVEOUT, launch_carveout());
     BankArgs args = a;
     void* params[] = {&args};
     const unsigned vpc = a.vpc ? a.vpc : (unsigned)threads, grid = (a.V + vpc - 1) / vpc;
-    CUresult r = A.LaunchKernel(f, grid, 1, 1, (unsigned)threads, 1, 1, (unsigned)smem, (CUstream)st, params, nullptr);
-    return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorLaunchFailure;
+    return launch_result(A.LaunchKernel(f, grid, 1, 1, (unsigned)threads, 1, 1, (unsigned)smem, (CUstream)st, params, nullptr), "kernel");
   }
 };
 

@@ -52,8 +52,8 @@ def mock_env():
         srcs = [os.path.join(CSRC, "host", f) for f in ("graph.cpp", "wavetable.cpp", "bank.cpp", "group.cpp", "wavfile.cpp")] + [os.path.join(CSRC, "capi.cpp"), os.path.join(MOCK, "registry_mock.cpp")]
         san = ["-fsanitize=" + SAN, "-g", "-fno-omit-frame-pointer"] if SAN else []
         subprocess.check_call(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-w", "-shared", "-fPIC", "-DFDSP_HOST_EMUL=1", *san, "-I", MOCK, "-I", CSRC,
-                               "-x", "c++", *srcs, "-o", lib + ".tmp", "-ldl"])
-        os.replace(lib + ".tmp", lib)
+                               "-x", "c++", *srcs, "-o", lib + ".tmp%d" % os.getpid(), "-ldl"])
+        os.replace(lib + ".tmp%d" % os.getpid(), lib)   # per process: pytest-xdist workers may build the same library at once
     env = dict(os.environ, FDSP_B200_LIB=lib, FDSP_MOCK_ROOT=ROOT, FDSP_MOCK_CACHE=os.path.join(build, "classes"), FDSP_MOCK_SCHEDULE="late")
     if SAN:   # every "device" buffer is a host allocation here, so the sanitizer sees each out-of-bounds word the GPU would silently read or write
         rt = subprocess.check_output(["gcc", "-print-file-name=lib" + ("asan" if SAN == "address" else "ubsan") + ".so"], text=True).strip()

@@ -115,6 +115,17 @@ def jobs():
         s = sg(v)
         add(s, (1, 2, 3))
         out[(s, 2, (1 if has_table(s) else 0) | (255 << 8))] = True
+    # the f32 filters (tests/test_gpu_filters.py): every audio-rate family with live and held controls (rows, the resident process()
+    # kernel), at its control edges, and on both sides of a Moog stage cut (the stage-pipelined kernel at 32 and 128 voices per CTA)
+    import test_gpu_filters as FL
+    for fam in FL.FAM:
+        for mk in (FL.live_voice, FL.held_voice, FL.edge_voice):
+            s = sg(mk(fam, 0))
+            add(s, (1,))
+            out[(s, 2, (1 if has_table(s) else 0) | (255 << 8))] = True
+        s = sg(FL.cut_voice(fam, 0))
+        add(s, (1,))
+        out[(s, 1, 128 << 8)] = True
     return sorted(out)
 
 
