@@ -107,6 +107,55 @@ class GpuBank:
             e.entry = int(failed.value)
             raise
 
+    def set_voices_device(self, kind, values, voices=None, address=(), stream=None, nvalues=1):
+        """`set_voices` with the values in device memory, their coefficients computed on the device: `values` is a float32 CUDA tensor on
+        the bank's device, contiguous [n, nvalues] or [n] (any object with a `__cuda_array_interface__` will do), or a raw device pointer
+        to `len(voices)` rows of `nvalues` floats. `stream` (a torch.cuda.Stream or a cudaStream_t as an int) is the stream that writes the
+        values: by default the tensor's current stream, or the legacy default stream for a pointer. The call is asynchronous; the bank
+        waits for `stream` and `stream` for the bank, so the values may be overwritten in stream order once it returns. The nodes the
+        address reaches must be ones whose set the device computes (see fdsp_bank_set_voices_device). Unlike `set_voices`, a refusal
+        applies no entry; the FdspError's `entry` is the first refused one."""
+        if isinstance(values, int):
+            if voices is None:
+                raise ValueError("values: a raw pointer needs `voices` (one index per entry)")
+            ptr, n, nv = values, len(voices), int(nvalues)
+        elif hasattr(values, "data_ptr") and hasattr(values, "is_cuda"):   # a torch tensor, read directly (its __cuda_array_interface__ is slow)
+            import torch
+            if not values.is_cuda or values.dtype != torch.float32 or values.dim() not in (1, 2) or not values.is_contiguous():
+                raise ValueError("values: a contiguous float32 CUDA tensor, [n, nvalues] or [n]")
+            if values.device.index != self.device:
+                raise ValueError(f"values: on cuda:{values.device.index}, the bank is on cuda:{self.device}")
+            n, nv = (values.shape[0], 1) if values.dim() == 1 else tuple(values.shape)
+            ptr = values.data_ptr()
+            if stream is None:
+                stream = torch.cuda.current_stream(values.device)
+        else:
+            cai = getattr(values, "__cuda_array_interface__", None)
+            if cai is None:
+                raise TypeError("values: a float32 CUDA tensor or a raw device pointer")
+            shape = tuple(cai["shape"])
+            if cai["typestr"] != "<f4" or len(shape) not in (1, 2):
+                raise ValueError("values: float32, [n, nvalues] or [n]")
+            n, nv = (shape[0], 1) if len(shape) == 1 else shape
+            if cai.get("strides") not in (None, (4,) if len(shape) == 1 else (4 * nv, 4)):
+                raise ValueError("values: must be contiguous")
+            ptr = cai["data"][0]
+        st = getattr(stream, "cuda_stream", stream) or 0
+        vp = None
+        if voices is not None:
+            vs = np.ascontiguousarray(voices, np.uint32)
+            if vs.shape != (n,):
+                raise ValueError("voices: one voice index per entry")
+            vp = vs.ctypes.data_as(C.POINTER(C.c_uint32))
+        addr = [x for pair in address for x in pair]
+        failed = C.c_uint32(0)
+        try:
+            check(self.L.fdsp_bank_set_voices_device(self.h, kind, vp, n, C.cast(C.c_void_p(ptr), C.POINTER(C.c_float)), nv,
+                                                     (C.c_int64 * max(1, len(addr)))(*addr), len(address), C.c_void_p(st), C.byref(failed)))
+        except FdspError as e:
+            e.entry = int(failed.value)
+            raise
+
     # ---- sequencer banks (voices built with fundsp_b200.sequencer.event): the mix output is Sequencer::process
     @classmethod
     def from_sequencer(cls, seq, device=0, per_voice=False, mix=True, sample_rate=None):

@@ -74,7 +74,8 @@ _SIG = {
     "fdsp_bank_set_sample_rate": (I, [P, D]), "fdsp_bank_reset": (I, [P]), "fdsp_bank_add_voice": (I, [P, P, C.POINTER(U32)]), "fdsp_jit_precompile": (I, [C.c_char_p, I, I]), "fdsp_bank_class_stages": (I, [P, I]),
     "fdsp_group_unique_id": (I, [P, U64]), "fdsp_group_create": (I, [I, I, P, I, C.POINTER(P)]), "fdsp_group_destroy": (None, [P]), "fdsp_group_rank": (I, [P]), "fdsp_group_size": (I, [P]),
     "fdsp_bank_render_reduced": (I, [P, P, U64, FP, FP, I]), "fdsp_bank_reduce_device": (I, [P, P, U64, P, U64, I]), "fdsp_jit_cache_stats": (None, [C.POINTER(I), C.POINTER(I)]), "fdsp_wave_save": (I, [C.c_char_p, FP, U32, U64, U64, D, I]), "fdsp_wave_encode": (C.c_int64, [C.POINTER(C.c_uint8), U64, FP, U32, U64, U64, D, I]), "fdsp_wave_load": (I, [C.c_char_p, FP, U64, C.POINTER(U32), C.POINTER(U64), C.POINTER(D)]), "fdsp_bank_edit_event": (I, [P, U32, D, D]), "fdsp_bank_push_event": (I, [P, P, C.POINTER(U32)]), "fdsp_bank_replace_voice": (I, [P, U32, P]), "fdsp_bank_remove_voice": (I, [P, U32]), "fdsp_bank_time": (D, [P]), "fdsp_bank_set": (I, [P, U32, I, FP, I, U64, C.POINTER(I64), I]),
-    "fdsp_bank_set_voices": (I, [P, I, C.POINTER(U32), U32, FP, I, C.POINTER(U64), C.POINTER(I64), I, C.POINTER(U32)]), "fdsp_bank_allocate": (I, [P, U64]),
+    "fdsp_bank_set_voices": (I, [P, I, C.POINTER(U32), U32, FP, I, C.POINTER(U64), C.POINTER(I64), I, C.POINTER(U32)]),
+    "fdsp_bank_set_voices_device": (I, [P, I, C.POINTER(U32), U32, FP, I, C.POINTER(I64), I, P, C.POINTER(U32)]), "fdsp_bank_allocate": (I, [P, U64]),
     "fdsp_bank_process": (I, [P, U32, FP, FP]), "fdsp_bank_render": (I, [P, U64, FP, FP, FP]),
     "fdsp_bank_render_device": (I, [P, U64, P, U64, P, U64, P, U64]), "fdsp_bank_sync": (I, [P]), "fdsp_bank_stream": (P, [P]),
     "fdsp_bank_num_classes": (I, [P]), "fdsp_bank_class_info": (I, [P, I, C.c_char_p, I, C.POINTER(U32), C.POINTER(U32), C.POINTER(U32), C.POINTER(U64)]),

@@ -342,6 +342,17 @@ API int fdsp_bank_set_voices(fdsp_bank* b, int kind, const uint32_t* voices, uin
   if (failed_entry) *failed_entry = failed;
   return status(e, FDSP_ERR_ARG);
 }
+API int fdsp_bank_set_voices_device(fdsp_bank* b, int kind, const uint32_t* voices, uint32_t n, const float* values_dev, int nvalues,
+                                    const int64_t* addr, int naddr, void* stream, uint32_t* failed_entry) {
+  if (failed_entry) *failed_entry = n;
+  if (!b || nvalues < 0 || nvalues > 5 || naddr < 0 || naddr > 6 || (n > 0 && nvalues > 0 && !values_dev) || (naddr > 0 && !addr)) return fail(FDSP_ERR_ARG, "bad setting");
+  Setting s; s.kind = kind;
+  for (int i = 0; i < naddr; i++) s.address.push_back({(int)addr[2 * i], (uint64_t)addr[2 * i + 1]});
+  uint32_t failed = n;
+  std::string e = b->b.set_voices_device(s, n, voices, values_dev, nvalues, (cudaStream_t)stream, &failed);
+  if (failed_entry) *failed_entry = failed;
+  return status(e);
+}
 // ---- JIT cache (csrc/host/jit.cpp): compiled units are kept on disk next to the library; a machine without a GPU can fill it
 API int fdsp_jit_precompile(const char* signature, int mode, int table_variant) {
   if (!signature) return fail(FDSP_ERR_ARG, "null signature");

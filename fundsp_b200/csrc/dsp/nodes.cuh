@@ -1033,10 +1033,10 @@ template <int KIND, int NIN> struct OnePole {
   template <bool T, class C> static FDSP_DEV void step(R& r, const C& c, const Fr<NIN>& in, Fr<1>& o) {
     if (NIN > 1) {
       const float p = in.v[NIN > 1 ? 1 : 0];
-      if (KIND == 2) r.coeff = (1.0f - p) / (1.0f + p);
+      if (KIND == 2) r.coeff = onepole_coeff(2, c.sr, p);
       else {
-        if (r.ksr != c.sr) { r.ksr = c.sr; r.coeff = m::expf_(-TAU_F * r.param / c.sr); }
-        if (p != r.param) { r.param = p; r.coeff = m::expf_(-TAU_F * p / c.sr); }
+        if (r.ksr != c.sr) { r.ksr = c.sr; r.coeff = onepole_coeff(KIND, c.sr, r.param); }
+        if (p != r.param) { r.param = p; r.coeff = onepole_coeff(KIND, c.sr, p); }
       }
     }
     const float x = in.v[0];
@@ -2606,8 +2606,7 @@ template <int KIND, int MODE, int OFF, int A0, int A1, int A2, int A3, int A4, c
     if constexpr (KIND == 0) { const SvfCoefs k = svf_coefs<MODE>(sr, v[0], v[1], v[2]); r.a1 = k.a1; r.a2 = k.a2; r.a3 = k.a3; r.m0 = k.m0; r.m1 = k.m1; r.m2 = k.m2; }
     else if constexpr (KIND == 1) { const BqCoefs k = bq_butter_lowpass(sr, v[0]); r.a1 = k.a1; r.a2 = k.a2; r.b0 = k.b0; r.b1 = k.b1; r.b2 = k.b2; }
     else if constexpr (KIND == 3) { r.a1 = v[0]; r.a2 = v[1]; r.b0 = v[2]; r.b1 = v[3]; r.b2 = v[4]; }
-    else if constexpr (KIND == 4 || KIND == 5) r.coeff = m::expf_(-TAU_F * v[0] / sr);
-    else if constexpr (KIND == 6) r.coeff = 1.0f - TAU_F / sr * v[0];
+    else if constexpr (KIND >= 4 && KIND <= 6) r.coeff = onepole_coeff(KIND == 6 ? 3 : KIND - 4, sr, v[0]);
     else if constexpr (KIND == 7) { for (int c = 0; c < T::OUT; c++) r.v[c] = v[0]; }
     else pan_weights(v[0], r.lw, r.rw);
   }

@@ -1,6 +1,7 @@
 // fundsp_b200 bank runtime implementation — see bank.h.
 #include "bank.h"
 #include "../dsp/fdn_args.h"
+#include "../dsp/libm.cuh"
 
 #include <algorithm>
 #include <mutex>
@@ -130,6 +131,7 @@ std::string VoiceClass::clear_history(cudaStream_t st) {
 std::string Bank::lower_and_upload(bool upload_state) {
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   // a looping sequencer (ReplayMode::Loop): every event of the bank carries the sequencer's loop period
   {
     double la = 0.0; bool any = false; size_t events = 0;
@@ -200,6 +202,7 @@ std::string Bank::lower_and_upload(bool upload_state) {
                             return a.sig == b.sig && a.voices == b.voices && a.uniform == b.uniform; });
   if (!same_shape) {
     classes = std::move(fresh);   // (releases the old classes' buffers)
+    voice_cls.clear(); voice_col.clear();
     upload_state = true;
   }
   for (auto& c : classes) {
@@ -276,6 +279,7 @@ std::string Bank::lower_and_upload(bool upload_state) {
 }
 
 std::string Bank::set_sample_rate(double s) {  // AudioUnit::set_sample_rate
+  TRY(ctl_sync());
   sr = s;
   for (auto& n : nodes) {   // the bank of a sequencer is re-rated like the sequencer: its events' units are reset (a unit pushed later is not)
     const bool reset = event_rerate_resets(n.get(), unit_rate());
@@ -291,6 +295,7 @@ std::string Bank::set(uint32_t voice, const Setting& st) {  // AudioUnit::set (s
   if (voice >= V()) return "#A set: voice index out of range";
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   // the setting is tried on a COPY of the voice's host graph: a refused setting (one that would change a class-uniform word) leaves
   // both the host graph and the device untouched; the copy replaces the original only after the upload
   std::unique_ptr<HNode> trial(nodes[voice]->clone());
@@ -352,6 +357,7 @@ std::string Bank::set_voices(const Setting& st, uint32_t n, const uint32_t* voic
   if (n == 0) return "";
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   std::vector<uint64_t> key;
   for (const Address& a : st.address) { key.push_back((uint64_t)a.type); key.push_back(a.value); }
   std::vector<SvClass> staged;
@@ -492,6 +498,245 @@ std::string Bank::sv_flush(const std::vector<SvClass>& staged) {
   return "";
 }
 
+// ---- Bank::set_voices_device
+
+// One entry: the controls of the node at column `col` of its class's [CTL_ROWS][V] table (kind | mode << 8, sample rate, v[0..5)), with the
+// first take[kind] values replaced by the entry's x[0..nx) (0 past nx, as a host Setting holds them) as the node's set() does; its parameter
+// words from the function its host lowering calls, at rows p0.. of the class's [NP][V] block; and the controls written back.
+struct CtlLaunch {
+  uint32_t *params, *ctl; const uint32_t *cols, *entries; const float* values;
+  uint32_t V, p0, m; int nch, nvalues; int take[9];   // take: the values a setting of this call's kind writes, per node kind (controls_taken)
+};
+FDSP_HD void set_controls_entry(const CtlLaunch& a, uint32_t e) {
+  const uint32_t col = a.cols[e], V = a.V;
+  const float* x = a.values + (size_t)a.entries[e] * (size_t)a.nvalues;
+  const uint32_t kind = a.ctl[col] & 0xffu, mode = a.ctl[col] >> 8;
+  const int take = a.take[kind < 9u ? kind : 8u];
+  float v[5];
+  for (int k = 0; k < 5; k++) v[k] = k < take ? (k < a.nvalues ? x[k] : 0.0f) : m::fromb(a.ctl[(size_t)(2 + k) * V + col]);
+  const float sr = m::fromb(a.ctl[(size_t)V + col]);
+  float w[6];
+  int nw = 0;
+  switch (kind) {
+    case 0: {
+      const SvfCoefs c = svf_coefs_mode((int)mode, sr, v[0], v[1], v[2]);
+      w[0] = c.a1; w[1] = c.a2; w[2] = c.a3; w[3] = c.m0; w[4] = c.m1; w[5] = c.m2; nw = 6;
+      break;
+    }
+    case 1: { const BqCoefs c = bq_butter_lowpass(sr, v[0]); w[0] = c.a1; w[1] = c.a2; w[2] = c.b0; w[3] = c.b1; w[4] = c.b2; nw = 5; break; }
+    case 3: for (int k = 0; k < 5; k++) w[k] = v[k]; nw = 5; break;
+    case 4: case 5: case 6: w[0] = onepole_coeff(kind == 6 ? 3 : (int)kind - 4, sr, v[0]); nw = 1; break;
+    case 7: for (int k = 0; k < a.nch; k++) a.params[(size_t)(a.p0 + k) * V + col] = m::fbits(v[0]); break;
+    default: pan_weights(v[0], w[0], w[1]); nw = 2; break;
+  }
+  for (int k = 0; k < nw; k++) a.params[(size_t)(a.p0 + k) * V + col] = m::fbits(w[k]);
+  for (int k = 0; k < take; k++) a.ctl[(size_t)(2 + k) * V + col] = m::fbits(v[k]);
+}
+#ifdef FDSP_HOST_EMUL
+// the CPU mock device: the same writes, queued on the stream as a launch is
+static cudaError_t launch_set_controls(const CtlLaunch& a, cudaStream_t st) {
+  return mock_launch(st, [=] {
+    for (uint32_t e = 0; e < a.m; e++) set_controls_entry(a, e);
+    return (cudaError_t)cudaSuccess;
+  });
+}
+#else
+__global__ void __launch_bounds__(256) set_controls_kernel(const CtlLaunch a) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < a.m) set_controls_entry(a, e);
+}
+static cudaError_t launch_set_controls(const CtlLaunch& a, cudaStream_t st) {
+  set_controls_kernel<<<(a.m + 255) / 256, 256, 0, st>>>(a);
+  return cudaGetLastError();
+}
+#endif
+
+// the parameter words a target of controls `kind` lowers (nch: a Constant's channels)
+static uint32_t ctl_words(uint32_t kind, uint32_t nch) {
+  return kind == 0 ? 6u : (kind == 1 || kind == 3) ? 5u : kind == 7 ? nch : kind == 8 ? 2u : 1u;
+}
+
+std::string Bank::set_voices_device(const Setting& st, uint32_t n, const uint32_t* voices, const float* values, int nvalues, cudaStream_t caller,
+                                    uint32_t* failed) {
+  *failed = n;
+  if (n == 0) return "";
+  CU(cudaSetDevice(device));
+  std::vector<uint64_t> key;
+  bool by_index = true;
+  for (const Address& a : st.address) { key.push_back((uint64_t)a.type); key.push_back(a.value); by_index = by_index && a.type == 1; }
+  CtlLaunch args{};
+  for (int k = 0; k < 9; k++) args.take[k] = controls_taken(k, st.kind);
+  if (voice_cls.size() != V()) {
+    voice_cls.assign(V(), UINT32_MAX); voice_col.assign(V(), 0);
+    for (size_t ci = 0; ci < classes.size(); ci++)
+      for (uint32_t i = 0; i < classes[ci].V(); i++) { voice_cls[classes[ci].voices[i]] = (uint32_t)ci; voice_col[classes[ci].voices[i]] = i; }
+  }
+  // per class an entry touches: the node the address reaches (the path is one for every voice of a class; the node there may differ) and
+  // its table, built from the host graphs when it is not current (that changes nothing the bank computes)
+  struct Touch { VoiceClass* c = nullptr; std::string refused; bool nowhere = false; VoiceClass::CtlTable* t = nullptr; uint32_t p0 = 0, np = 0;
+                 std::vector<int32_t> last; uint32_t m = 0; };
+  std::vector<int> touch_of(classes.size(), -1);
+  std::vector<Touch> touch;
+  auto resolve = [&](VoiceClass& c, Touch& u) -> std::string {
+    u.c = &c;
+    Setting ls = st;
+    HNode* leaf = by_index ? setting_leaf(nodes[c.voices[0]].get(), &ls, &u.nowhere) : nullptr;
+    if (u.nowhere) return "";   // the address leads nowhere
+    if (!leaf) {
+      u.refused = by_index ? "#U set_voices_device: the address ends at a System, a Net, a Slot or a crossfading vertex, whose set the device does not compute"
+                           : "#U set_voices_device: .node(id) addresses are not resolved on the device";
+      return "";
+    }
+    auto it = c.leaf_at.find(key);
+    if (it == c.leaf_at.end()) it = c.leaf_at.emplace(key, leaf_at_of(c, nodes[c.voices[0]].get(), st)).first;
+    u.last.assign(c.V(), -1);
+    if (!it->second.ok || !it->second.np) return "";   // no column range of parameter words: every voice's node is checked on its own below
+    u.p0 = it->second.p0; u.np = it->second.np;
+    for (uint32_t r : c.sh_rows)   // Bank::sh_pull rewrites such a row whole from its host image, which the device's words never reach
+      if (r >= u.p0 && r < u.p0 + u.np) {
+        u.refused = "#U set_voices_device: the node's parameter words share a row with other voices' Shared readers (var(&shared) in the same class)";
+        return "";
+      }
+    u.t = &c.ctl[u.p0];
+    if (!u.t->fresh) {
+      TRY(rt_end_streak());
+      TRY(ctl_build(c, *u.t, st.address, it->second.np));
+    }
+    return "";
+  };
+  // every entry is checked before anything is applied; per column the last entry wins
+  for (uint32_t j = 0; j < n; j++) {
+    const uint32_t v = voices ? voices[j] : j;
+    if (v >= V() || voice_cls[v] == UINT32_MAX) { *failed = j; return "#A set_voices_device: voice index out of range"; }
+    const size_t ci = voice_cls[v];
+    const uint32_t i = voice_col[v];
+    if (touch_of[ci] < 0) { touch_of[ci] = (int)touch.size(); touch.emplace_back(); TRY(resolve(classes[ci], touch.back())); }
+    Touch& u = touch[(size_t)touch_of[ci]];
+    if (!u.refused.empty()) { *failed = j; return u.refused; }
+    if (u.nowhere) continue;
+    const uint32_t kw = u.t ? u.t->kind[i] : VoiceClass::CTL_NONE;
+    if (kw == VoiceClass::CTL_NONE) {   // none of the device's targets: the entry changes nothing only where the node ignores the setting
+      Setting ls = st;
+      bool nowhere = false;
+      HNode* leaf = setting_leaf(nodes[v].get(), &ls, &nowhere);
+      if (leaf && setting_ignored(leaf, ls)) continue;
+      std::string g;
+      if (leaf) leaf->sig(g);
+      *failed = j;
+      return "#U set_voices_device: voice " + std::to_string(v) + ": the setting reaches " + g.substr(0, 80) + (leaf ? " (ID " + std::to_string(leaf->id()) + ")" : "") +
+             ", whose set the device does not compute (FixedSvf, the fixed ButterLowpass / Biquad, the fixed one-poles, Constant and Panner<U1>)";
+    }
+    if (!args.take[kw & 0xffu]) continue;   // the node ignores this kind of setting
+    if (u.last[i] < 0) u.m++;
+    u.last[i] = (int32_t)j;
+  }
+  size_t total = 0;
+  for (const Touch& u : touch) total += 2 * (size_t)u.m;
+  if (!total) return "";
+  TRY(rt_end_streak());
+  // per class: the columns [m], then the entries whose values they take [m]
+  if (sv_pending) { CU(cudaEventSynchronize(sv_copied)); sv_pending = false; }
+  TRY(sv_stage.grow(total));
+  TRY(d_sv.grow(total));
+  size_t at = 0;
+  for (Touch& u : touch) {
+    if (!u.m) continue;
+    uint32_t e = 0;
+    for (uint32_t i = 0; i < u.c->V(); i++) {
+      if (u.last[i] < 0) continue;
+      sv_stage[at + e] = i; sv_stage[at + u.m + e] = (uint32_t)u.last[i];
+      u.t->touched[i] = 1;
+      e++;
+    }
+    at += 2 * (size_t)u.m;
+  }
+  if (!dv_in) { CU(cudaEventCreateWithFlags(dv_in.put(), cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(dv_out.put(), cudaEventDisableTiming)); }
+  if (!sv_copied) CU(cudaEventCreateWithFlags(sv_copied.put(), cudaEventDisableTiming));
+  CU(cudaEventRecord(dv_in, caller));   // the values are written on the caller's stream
+  CU(cudaStreamWaitEvent(stream, dv_in, 0));
+  CU(cudaMemcpyAsync(d_sv, sv_stage, total * 4, cudaMemcpyHostToDevice, stream));
+  CU(cudaEventRecord(sv_copied, stream));
+  sv_pending = true;
+  at = 0;
+  for (Touch& u : touch) {
+    if (!u.m) continue;
+    CtlLaunch a = args;
+    a.params = u.c->d_params; a.ctl = u.t->d; a.cols = d_sv + at; a.entries = d_sv + at + u.m; a.values = values;
+    a.V = u.c->V(); a.p0 = u.p0; a.m = u.m; a.nvalues = nvalues;
+    a.nch = (int)u.np;   // (a Constant's parameter words are its channels)
+    CU(launch_set_controls(a, stream));
+    launches++;
+    u.t->ahead = true;
+    at += 2 * (size_t)u.m;
+  }
+  CU(cudaEventRecord(dv_out, stream));   // the caller may overwrite the values once its stream is past the kernels
+  CU(cudaStreamWaitEvent(caller, dv_out, 0));
+  return "";
+}
+
+// Class c's table of the node at address `at`, whose parameter words are np rows, from the host graphs of its voices.
+std::string Bank::ctl_build(VoiceClass& c, VoiceClass::CtlTable& t, const std::vector<Address>& at, uint32_t np) {
+  const uint32_t Vc = c.V();
+  std::vector<uint32_t> h((size_t)VoiceClass::CTL_ROWS * Vc, 0u);
+  t.at = at;
+  t.kind.assign(Vc, VoiceClass::CTL_NONE);
+  for (uint32_t i = 0; i < Vc; i++) {
+    Setting ls; ls.address = at;
+    bool nowhere = false;
+    HNode* leaf = setting_leaf(nodes[c.voices[i]].get(), &ls, &nowhere);
+    Controls k;
+    if (!leaf || !read_controls(leaf, &k) || ctl_words((uint32_t)k.kind, (uint32_t)k.nch) != np) continue;
+    t.kind[i] = h[i] = (uint32_t)k.kind | (uint32_t)k.mode << 8;
+    h[(size_t)Vc + i] = f2u(k.sr);
+    for (int q = 0; q < 5; q++) h[(size_t)(2 + q) * Vc + i] = f2u(k.v[q]);
+  }
+  TRY(t.d.grow(h.size()));
+  CU(cudaMemcpyAsync(t.d, h.data(), h.size() * 4, cudaMemcpyHostToDevice, stream));
+  CU(cudaStreamSynchronize(stream));   // (h is pageable)
+  t.touched.assign(Vc, 0);
+  t.fresh = true; t.ahead = false;
+  return "";
+}
+
+std::string Bank::ctl_sync() {
+  size_t words = 0;
+  for (const VoiceClass& c : classes) for (auto& kv : c.ctl) if (kv.second.ahead) words += (size_t)VoiceClass::CTL_ROWS * c.V();
+  if (words) {
+    CU(cudaSetDevice(device));
+    TRY(rt_stop());
+    TRY(ctl_stage.grow(words));
+    size_t at = 0;
+    for (const VoiceClass& c : classes)
+      for (auto& kv : c.ctl) {
+        if (!kv.second.ahead) continue;
+        CU(cudaMemcpyAsync(ctl_stage + at, kv.second.d, (size_t)VoiceClass::CTL_ROWS * c.V() * 4, cudaMemcpyDeviceToHost, stream));
+        at += (size_t)VoiceClass::CTL_ROWS * c.V();
+      }
+    CU(cudaStreamSynchronize(stream));
+    at = 0;
+    for (VoiceClass& c : classes)
+      for (auto& kv : c.ctl) {
+        const VoiceClass::CtlTable& t = kv.second;
+        if (!t.ahead) continue;
+        const uint32_t Vc = c.V();
+        for (uint32_t i = 0; i < Vc; i++) {
+          if (!t.touched[i]) continue;
+          Setting ls; ls.address = t.at;
+          bool nowhere = false;
+          HNode* leaf = setting_leaf(nodes[c.voices[i]].get(), &ls, &nowhere);
+          if (!leaf) return "internal: set_voices_device: a set voice no longer reaches its node";
+          Controls k;
+          k.kind = (int)(t.kind[i] & 0xffu);
+          for (int q = 0; q < 5; q++) k.v[q] = m::fromb(ctl_stage[at + (size_t)(2 + q) * Vc + i]);
+          leaf->set(controls_setting(k));   // (the node's own set: its coefficients follow, with its own sample rate)
+        }
+        at += (size_t)VoiceClass::CTL_ROWS * Vc;
+      }
+  }
+  for (VoiceClass& c : classes) for (auto& kv : c.ctl) kv.second.fresh = kv.second.ahead = false;
+  return "";
+}
+
 double Bank::loop_point() const {
   if (!(loop_arg > 0.0)) return std::numeric_limits<double>::infinity();
   const double ur = unit_rate();
@@ -524,6 +769,7 @@ std::string Bank::state0_to_device(VoiceClass& c, const uint32_t** out) {
 // `l`: the words to run with. `reset_state`: the construction-time state that reset() restores (defaults to l.S).
 std::string Bank::upload_voice(uint32_t voice, const Lowering& l, bool with_state, const std::vector<uint32_t>* reset_state) {
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   uint32_t i = 0;
   if (VoiceClass* cp = locate(classes, voice, &i)) {
     VoiceClass& c = *cp;
@@ -551,6 +797,7 @@ std::string Bank::edit_event(uint32_t voice, double end_time, double fade_out) {
   if (voice >= V()) return "#A edit: voice index out of range";
   CU(cudaSetDevice(device));
   if (loop_arg > 0.0) return "#U edit: events of a looping sequencer are not edited on the device (their current times live in the state words)";
+  TRY(ctl_sync());
   if (!event_edit(nodes[voice].get(), end_time, fade_out)) return "#A edit: the voice is not a sequencer event";
   Lowering l;
   nodes[voice]->lower(l);
@@ -574,6 +821,7 @@ std::string Bank::replace_voice(uint32_t voice, HNode* node) {
   if (voice >= V()) return "#A replace: voice index out of range";
   if (n->inputs() != nin || n->outputs() != nout) return "#U replace: the unit's arity differs from the bank's";
   CU(cudaSetDevice(device));
+  TRY(ctl_sync());
   std::string a, b;
   n->sig(a); nodes[voice]->sig(b);
   // another graph class (Net::replace takes any unit of the same arity, src/net.rs:460-470): the voice moves to the class of its new graph —
@@ -615,6 +863,7 @@ std::string Bank::regroup(HNode* node, int at, uint32_t* voice, const Carry* car
   for (auto& c : classes) if (c.form != Form::plain) return std::string("#U ") + what + ": banks with a two-stage class (FDN reverb, tensor-core convolver) cannot be regrouped in place; rebuild the bank";
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   Lowering l0, l;
   lower_entering(n.get(), &l0, &l, true);
   if (!l.ok) return "#U " + l.why;
@@ -690,6 +939,7 @@ std::string Bank::crossfade_voice(uint32_t voice, int ease, float fade_time, HNo
   if (n->inputs() != nin || n->outputs() != nout) return "#U crossfade: the unit's arity differs from the bank's";
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   const HNode* cur = nodes[voice].get();
   Carry carry{0, 0, 0, 0, 0, 0};
   auto count = [](const HNode* h, uint32_t* ns, uint64_t* nd) { Lowering q; h->lower(q); *ns = (uint32_t)q.S.size(); *nd = 0; for (uint32_t d : q.dlen) *nd += d; return q.ok; };
@@ -744,6 +994,7 @@ std::string Bank::slot_arm_now(uint32_t voice, int ease, double fade_time, HNode
   std::unique_ptr<HNode> n(unit);
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   uint32_t i = 0;
   if (VoiceClass* cp = locate(classes, voice, &i)) {
     VoiceClass& c = *cp;
@@ -872,6 +1123,7 @@ std::string Bank::push_event(HNode* node, uint32_t* voice) {   // Sequencer::pus
   if (loop_arg > 0.0) return "#U push: a looping sequencer bank takes its events before the first render";
   if (n->inputs() != nin || n->outputs() != nout) return "#U push: the event's arity differs from the bank's";
   CU(cudaSetDevice(device));
+  TRY(ctl_sync());
   const double sd = 1.0 / unit_rate();
   Lowering l0, l;
   lower_entering(n.get(), &l0, &l, false);   // (a start time in the past makes the event sound from the next block on)
@@ -895,6 +1147,7 @@ std::string Bank::push_event(HNode* node, uint32_t* voice) {   // Sequencer::pus
 std::string Bank::reset() {  // AudioUnit::reset: back to the construction-time state
   CU(cudaSetDevice(device));
   TRY(rt_end_streak());
+  TRY(ctl_sync());
   while (!slot_latest.empty()) {   // SlotBackend::reset adopts the LATEST configuration (src/slot.rs:156-172): arm it (its words become the voice's reset image)
     auto it = slot_latest.begin();
     const uint32_t voice = it->first;
@@ -1382,6 +1635,7 @@ std::string Bank::process(uint32_t size, const float* in, float* out) {  // Audi
 
 std::string Bank::clone_into(Bank& dst) const {
   TRY(const_cast<Bank*>(this)->rt_stop());
+  TRY(const_cast<Bank*>(this)->ctl_sync());   // the clone is built from the host graphs
   std::vector<HNode*> copies;
   for (auto& n : nodes) copies.push_back(n->clone());
   dst.sr = sr; dst.tree_mix = tree_mix; dst.net_rate = net_rate; dst.vertex_of_voice = vertex_of_voice;
@@ -1421,6 +1675,7 @@ std::string Bank::sh_check(uint32_t voice, const std::vector<SharedUse>& uses) c
 }
 
 std::string Bank::sh_rebuild() {
+  TRY(ctl_sync());
   std::map<const SharedCell*, int> index;
   sh_cells.clear(); sh_last.clear(); sh_last_writer.clear();
   size_t stage = 0;

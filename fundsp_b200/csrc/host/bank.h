@@ -60,6 +60,15 @@ struct VoiceClass {
   // found once on one voice (every voice of a class has one structure); !ok: its voices take Bank::set
   struct LeafAt { bool ok = false; uint32_t p0 = 0, np = 0, s0 = 0, ns = 0; };
   std::map<std::vector<uint64_t>, LeafAt> leaf_at;
+  // Bank::set_voices_device: per node an address reaches, keyed by the node's first parameter row (two addresses that reach one node share
+  // its table), that node's controls (graph.h Controls) on every voice as the device's sets leave them: [CTL_ROWS][V] words (kind | mode << 8,
+  // sample rate, v[0..5)). `kind` is the host's copy of row 0, CTL_NONE where the voice's node is none of the device's targets: one class
+  // signature can hold different nodes (dc and var both lower as Constant<1>; biquad, butterpass and resonator as Biquad). `at`: an address
+  // that reaches the node. Built from the host graphs on first use and again after any call that reconciles them (Bank::ctl_sync); `ahead`:
+  // the device has set columns `touched` since, which the host graphs do not know yet.
+  static constexpr uint32_t CTL_ROWS = 7, CTL_NONE = 0xFFFFFFFFu;
+  struct CtlTable { bool fresh = false, ahead = false; std::vector<Address> at; std::vector<uint32_t> kind; Array<uint32_t> d; std::vector<uint8_t> touched; };
+  std::map<uint32_t, CtlTable> ctl;
   uint32_t V() const { return (uint32_t)voices.size(); }
   bool fdn_with_dry() const { return form == Form::fdn && k; }   // two stages, software-pipelined by render_device_run
   std::string clear_history(cudaStream_t st);   // zeroes what the form's own buffers carry from call to call (on upload and reset)
@@ -148,8 +157,21 @@ struct Bank {
   std::string set_voices(const Setting& s, uint32_t n, const uint32_t* voices, const float* values, int nvalues, const uint64_t* seeds, uint32_t* failed);
   struct SvClass { VoiceClass* c; VoiceClass::LeafAt at; std::vector<uint32_t> cols, words; };   // one class's staged entries ([entry][word])
   std::string sv_flush(const std::vector<SvClass>& staged);
-  PinnedArray<uint32_t> sv_stage; Array<uint32_t> d_sv;   // set_voices' parameter words: host staging and its device copy
+  PinnedArray<uint32_t> sv_stage; Array<uint32_t> d_sv;   // set_voices' parameter words (set_voices_device's entry indices): host staging and its device copy
   Event sv_copied; bool sv_pending = false;               // recorded behind the copy of sv_stage: it is rewritten only after that copy has landed
+  // set() on n entries whose values are [n][nvalues] f32 in device memory, written by the caller's stream `st`: entry j sets voice voices[j]
+  // (j when voices is null). Every entry is checked on the host first; on a refusal *failed = j and nothing is applied. The node the address
+  // reaches must be one whose set the device computes (graph.h Controls): one kernel per class touched turns the values into parameter words
+  // and controls (VoiceClass::ctl). Asynchronous: `stream` waits for the values on `st`, and `st` for the kernels. The host graphs learn the
+  // new controls in ctl_sync, before any call that reads them.
+  std::string set_voices_device(const Setting& s, uint32_t n, const uint32_t* voices, const float* values, int nvalues, cudaStream_t st, uint32_t* failed);
+  std::string ctl_build(VoiceClass& c, VoiceClass::CtlTable& t, const std::vector<Address>& at, uint32_t np);
+  // Before a call that reads or lowers the host graphs: the controls the device has set go into the host graphs (one download per table
+  // that is ahead, one synchronise), and every table is rebuilt from the host graphs on its next use, since the call may change them.
+  // process() and the renders reach it only through slot_service, when a parked Slot / crossfade update falls due and is armed.
+  std::string ctl_sync();
+  PinnedArray<uint32_t> ctl_stage; Event dv_in, dv_out;   // the tables' download; the caller's stream -> `stream` -> the caller's stream
+  std::vector<uint32_t> voice_cls, voice_col;             // per voice: its class and column (set_voices_device; cleared when the classes are rebuilt)
   std::string ensure_staging(uint32_t chunk);
   std::string render_device(uint64_t n, const float* in_dev, uint64_t in_stride, float* out_dev, uint64_t out_stride, float* mix_dev,
                             uint64_t mix_stride);

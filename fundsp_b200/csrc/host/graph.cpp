@@ -207,13 +207,7 @@ struct TapN : HNode {  // src/delay.rs:141-286 Tap / :379-505 TapLinear
 // ---------------------------------------------------------------- SVF (src/svf.rs)
 typedef fdsp::SvfCoefs Coefs6;
 Coefs6 svf_coefs(int mode, float sr, float cutoff, float q, float gain) {  // src/svf.rs:26-221 (shared host/device code)
-  switch (mode) {
-    case 0: return fdsp::svf_coefs<0>(sr, cutoff, q, gain); case 1: return fdsp::svf_coefs<1>(sr, cutoff, q, gain);
-    case 2: return fdsp::svf_coefs<2>(sr, cutoff, q, gain); case 3: return fdsp::svf_coefs<3>(sr, cutoff, q, gain);
-    case 4: return fdsp::svf_coefs<4>(sr, cutoff, q, gain); case 5: return fdsp::svf_coefs<5>(sr, cutoff, q, gain);
-    case 6: return fdsp::svf_coefs<6>(sr, cutoff, q, gain); case 7: return fdsp::svf_coefs<7>(sr, cutoff, q, gain);
-    default: return fdsp::svf_coefs<8>(sr, cutoff, q, gain);
-  }
+  return fdsp::svf_coefs_mode(mode, sr, cutoff, q, gain);
 }
 struct Svf : HNode {  // FixedSvf (ID 43, :857-1031) and Svf (ID 36, :744-855)
   int mode; bool fixed; float sr, cutoff, q, gain;
@@ -550,11 +544,8 @@ struct OnePoleN : HNode {  // src/filter.rs: kind 0 Lowpole, 1 Highpole, 2 Allpo
   int kind, nin; float param, coeff = 0, sr = (float)DEFAULT_SR;
   OnePoleN(int k, float p, int n) : kind(k), nin(n), param(p) { set_param(p); }
   void set_param(float p) {
-    const float TAU = 6.28318548202514648f;
     param = p;
-    if (kind == 0 || kind == 1) coeff = m::expf_(-TAU * p / sr);
-    else if (kind == 2) coeff = (1.0f - p) / (1.0f + p);
-    else if (kind == 3) coeff = 1.0f - TAU / sr * p;
+    if (kind != 4) coeff = fdsp::onepole_coeff(kind, sr, p);
   }
   int inputs() const override { return nin; } int outputs() const override { return 1; }
   uint64_t id() const override { static const uint64_t ids[5] = {18, 47, 46, 22, 26}; return ids[kind]; }
@@ -1184,18 +1175,18 @@ struct SystemN : HNode {
     }
     return n;
   }
-  // the target's current set values, as its host node holds them
-  void values(const Target& t, float* v) const {
-    HNode* n = at(t.hops);
-    switch (t.kind) {
-      case 0: { Svf* f = static_cast<Svf*>(n); v[0] = f->cutoff; v[1] = f->q; v[2] = f->gain; break; }
-      case 1: v[0] = static_cast<Biquad*>(n)->f; break;
-      case 3: { const BqCoefs& c = static_cast<Biquad*>(n)->c; v[0] = c.a1; v[1] = c.a2; v[2] = c.b0; v[3] = c.b1; v[4] = c.b2; break; }
-      case 4: case 5: case 6: v[0] = static_cast<OnePoleN*>(n)->param; break;
-      case 7: v[0] = static_cast<Constant*>(n)->v[0]; break;
-      default: v[0] = static_cast<Panner*>(n)->value; break;
+  // the current set values of a target of `kind`, as its host node holds them
+  static void values(const HNode* n, int kind, float* v) {
+    switch (kind) {
+      case 0: { const Svf* f = static_cast<const Svf*>(n); v[0] = f->cutoff; v[1] = f->q; v[2] = f->gain; break; }
+      case 1: v[0] = static_cast<const Biquad*>(n)->f; break;
+      case 3: { const BqCoefs& c = static_cast<const Biquad*>(n)->c; v[0] = c.a1; v[1] = c.a2; v[2] = c.b0; v[3] = c.b1; v[4] = c.b2; break; }
+      case 4: case 5: case 6: v[0] = static_cast<const OnePoleN*>(n)->param; break;
+      case 7: v[0] = static_cast<const Constant*>(n)->v[0]; break;
+      default: v[0] = static_cast<const Panner*>(n)->value; break;
     }
   }
+  void values(const Target& t, float* v) const { values(at(t.hops), t.kind, v); }
   int inputs() const override { return x->inputs(); } int outputs() const override { return x->outputs(); }
   uint64_t id() const override { return 67; }
   void reset() override { x->reset(); }
@@ -1504,6 +1495,30 @@ HNode* setting_leaf(HNode* voice, Setting* s, bool* ignored) {
   if (!n || dynamic_cast<SystemN*>(n) || dynamic_cast<HNet*>(n) || dynamic_cast<SlotN*>(n) || dynamic_cast<XfadeN*>(n)) return nullptr;
   return n;
 }
+bool read_controls(HNode* n, Controls* c) {
+  int n_sv = 0;
+  *c = Controls();
+  if (!SystemN::classify(n, &c->kind, &c->mode, &n_sv) || c->kind == 2) { c->kind = -1; return false; }
+  SystemN::values(n, c->kind, c->v);
+  if (const Svf* f = dynamic_cast<const Svf*>(n)) c->sr = f->sr;
+  else if (const Biquad* b = dynamic_cast<const Biquad*>(n)) c->sr = b->sr;
+  else if (const OnePoleN* o = dynamic_cast<const OnePoleN*>(n)) c->sr = o->sr;
+  if (const Constant* k = dynamic_cast<const Constant*>(n)) c->nch = (int)k->v.size();
+  return true;
+}
+int controls_taken(int kind, int setting) {
+  int slots[5], n = 0;
+  if (SystemN::accepts(kind, setting, slots)) for (int k = 0; k < 5; k++) n += slots[k] >= 0;
+  return n;
+}
+Setting controls_setting(const Controls& c) {
+  static const int full[9] = {P_CENTER_Q_GAIN, P_CENTER, P_NULL, P_BIQUAD, P_CENTER, P_CENTER, P_CENTER, P_VALUE, P_PAN};
+  Setting s;
+  s.kind = c.kind >= 0 && c.kind < 9 ? full[c.kind] : P_NULL;
+  for (int k = 0; k < 5; k++) s.v[k] = c.v[k];
+  return s;
+}
+bool setting_ignored(const HNode* n, const Setting& s) { return SystemN::ignores(n, s); }
 bool event_edit(HNode* n, double end_time, double fade_out) {   // Sequencer::edit on an event (:441-483, no loop: start == original start)
   EventN* e = dynamic_cast<EventN*>(n);
   if (!e) return false;

@@ -147,6 +147,16 @@ HNode* reach_setting(HNode* n, Setting* s, std::vector<int>* hops);
 // a crossfading vertex.
 HNode* setting_leaf(HNode* voice, Setting* s, bool* ignored);
 
+// The nodes whose set() the device computes (the targets of update(), nodes.cuh UpdTarget, and of Bank::set_voices_device), with what
+// their set() reads and writes. kind: 0 FixedSvf (mode 0-8), 1 the fixed ButterLowpass, 3 the fixed Biquad, 4 Lowpole, 5 Highpole,
+// 6 DCBlock (the fixed one-poles), 7 Constant (nch channels), 8 Panner<U1>. v: (cutoff, q, gain), (cutoff), (a1, a2, b0, b1, b2),
+// (cutoff), (cutoff), (cutoff), (value), (pan). sr: the node's own sample rate.
+struct Controls { int kind = -1, mode = 0, nch = 0; float sr = 0.0f; float v[5] = {0, 0, 0, 0, 0}; };
+bool read_controls(HNode* n, Controls* c);                 // false: n is none of those nodes
+int controls_taken(int kind, int setting);                 // the leading values of v a setting of that kind writes (0: the node ignores it)
+Setting controls_setting(const Controls& c);               // the setting that gives such a node the values c.v (with its own sample rate)
+bool setting_ignored(const HNode* n, const Setting& s);    // n.set(s) leaves every word n lowers as it was
+
 // ---- builders (one per primitive; composites consume their children)
 HNode* mk_constant(int n, const float* v);
 HNode* mk_pass();

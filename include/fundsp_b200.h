@@ -288,6 +288,22 @@ int fdsp_bank_set(fdsp_bank* b, uint32_t voice, int kind, const float* values, i
    and one launch per class the entries touch. */
 int fdsp_bank_set_voices(fdsp_bank* b, int kind, const uint32_t* voices, uint32_t n, const float* values, int nvalues, const uint64_t* seeds,
                          const int64_t* address_pairs, int naddress, uint32_t* failed_entry);
+/* fdsp_bank_set_voices with the values in device memory: values_dev is [n][nvalues] f32 on the bank's device, and the coefficients are
+   computed there, one kernel per class the entries touch. voices (NULL: entry j is voice j) is host memory. `stream` is the cudaStream_t
+   that writes the values (NULL: the legacy default stream): the bank waits for the work queued on it, and it waits for the bank's kernels,
+   so the caller may overwrite the values in stream order once this returns. Asynchronous: the sets take effect from the next process or
+   render call, and leave the bank exactly as fdsp_bank_set_voices with the same values would (entries of one voice: the last one wins).
+   The node an address reaches must be a FixedSvf (center, center_q, center_q_gain), the fixed ButterLowpass (center), the fixed Biquad
+   (biquad), a fixed Lowpole / Highpole / DCBlock (center), a Constant (value) or a Panner<U1> (pan); an address that leads nowhere, or a
+   setting the node ignores, changes nothing. Values are not checked.
+   Unlike fdsp_bank_set_voices, a refusal applies NO entry (the host never sees the values, so every entry is checked first):
+   *failed_entry = the first refused entry (n on success), FDSP_ERR_ARG for a voice out of range, FDSP_ERR_UNSUPPORTED for a voice whose
+   address reaches any other node that does not ignore the setting (checked voice by voice: voices of one class can hold different nodes,
+   e.g. dc and var), a Slot, a crossfading vertex, a System or a Net, or uses .node(id), or whose node's parameter words share a row with
+   other voices' Shared readers (var(&shared) in the same class). The host graphs take the device's sets before any call that reads
+   them; process and the renders never wait for that, except when a parked Slot / crossfade update falls due in them. */
+int fdsp_bank_set_voices_device(fdsp_bank* b, int kind, const uint32_t* voices, uint32_t n, const float* values_dev, int nvalues,
+                                const int64_t* address_pairs, int naddress, void* stream, uint32_t* failed_entry);
 int fdsp_bank_allocate(fdsp_bank* b, uint64_t max_render_samples);          /* AudioUnit::allocate: later calls do not allocate */
 /* AudioUnit::process: size <= 64; host buffers in [inputs][64], out [outputs][64]; size 0 is a no-op */
 int fdsp_bank_process(fdsp_bank* b, uint32_t size, const float* in, float* out);

@@ -393,6 +393,16 @@ class Bank {
     check(fdsp_bank_set_voices(b_, kind, voices.empty() ? nullptr : voices.data(), n, values.data(), nvalues, seeds.empty() ? nullptr : seeds.data(),
                                a.empty() ? nullptr : a.data(), (int)address.size(), failed_entry));
   }
+  // set_voices with the values in device memory (fdsp_bank_set_voices_device): `n` entries of [n][nvalues] floats at values_dev, written on
+  // `stream` (a cudaStream_t; nullptr: the legacy default stream). Asynchronous; a refusal applies no entry and throws, with the first
+  // refused entry's index in *failed_entry.
+  void set_voices_device(int kind, const float* values_dev, uint32_t n, int nvalues, const std::vector<uint32_t>& voices = {},
+                         std::initializer_list<std::pair<int, int64_t>> address = {}, void* stream = nullptr, uint32_t* failed_entry = nullptr) {
+    std::vector<int64_t> a;
+    for (auto& p : address) { a.push_back(p.first); a.push_back(p.second); }
+    check(fdsp_bank_set_voices_device(b_, kind, voices.empty() ? nullptr : voices.data(), n, values_dev, nvalues, a.empty() ? nullptr : a.data(),
+                                      (int)address.size(), stream, failed_entry));
+  }
   void allocate(uint64_t max_samples = 64) { check(fdsp_bank_allocate(b_, max_samples)); }
   // sequencer banks: Sequencer::time / edit / push on a running bank (a pushed event reuses the slot of a finished event of its class)
   double time() const { return fdsp_bank_time(b_); }

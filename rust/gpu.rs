@@ -143,6 +143,8 @@ extern "C" {
     fn fdsp_bank_set(b: *mut FdspBank, voice: u32, kind: c_int, v: *const f32, nv: c_int, seed: u64, addr: *const i64, naddr: c_int) -> c_int;
     fn fdsp_bank_set_voices(b: *mut FdspBank, kind: c_int, voices: *const u32, n: u32, v: *const f32, nv: c_int, seeds: *const u64, addr: *const i64,
                             naddr: c_int, failed_entry: *mut u32) -> c_int;
+    fn fdsp_bank_set_voices_device(b: *mut FdspBank, kind: c_int, voices: *const u32, n: u32, values_dev: *const f32, nv: c_int, addr: *const i64,
+                                   naddr: c_int, stream: *mut c_void, failed_entry: *mut u32) -> c_int;
     fn fdsp_bank_process(b: *mut FdspBank, size: u32, input: *const f32, output: *mut f32) -> c_int;
     fn fdsp_bank_render(b: *mut FdspBank, n: u64, input: *const f32, out_voices: *mut f32, out_mix: *mut f32) -> c_int;
     // multi-GPU mix-down (csrc/host/group.h)
@@ -581,6 +583,22 @@ impl GpuBank {
             fdsp_bank_set_voices(self.h, kind as c_int, voices.map_or(core::ptr::null(), |v| v.as_ptr()), n as u32, values.as_ptr(), nvalues as c_int,
                                  core::ptr::null(), addr.as_ptr(), address.len() as c_int, &mut failed)
         };
+        check(rc).map_err(|e| (failed, e))
+    }
+    /// `set_voices` with the values in device memory, their coefficients computed on the device (`fdsp_bank_set_voices_device`): `n` rows
+    /// of `nvalues` f32 at `values_dev` on the bank's device, written on the CUDA stream `stream` (null: the legacy default stream). The
+    /// call is asynchronous and orders itself after `stream`, and `stream` after it. On a refusal no entry is applied; Err holds the first
+    /// refused entry's index.
+    ///
+    /// # Safety
+    /// `values_dev` must point to `n * nvalues` floats of device memory that stay valid until `stream` has passed this call.
+    pub unsafe fn set_voices_device(&mut self, kind: i32, values_dev: *const f32, n: u32, nvalues: usize, voices: Option<&[u32]>, address: &[(i32, i64)],
+                                    stream: *mut c_void) -> Result<(), (u32, String)> {
+        if nvalues > 5 || voices.map_or(false, |v| v.len() != n as usize) { return Err((0, String::from("set_voices_device: nvalues <= 5 and one voice per entry"))); }
+        let addr: Vec<i64> = address.iter().flat_map(|&(t, v)| [t as i64, v]).collect();
+        let mut failed = 0u32;
+        let rc = fdsp_bank_set_voices_device(self.h, kind as c_int, voices.map_or(core::ptr::null(), |v| v.as_ptr()), n, values_dev, nvalues as c_int,
+                                             addr.as_ptr(), address.len() as c_int, stream, &mut failed);
         check(rc).map_err(|e| (failed, e))
     }
     pub fn voice_of_vertex(&self, vertex: usize) -> Option<u32> { let v = unsafe { fdsp_bank_voice_of_vertex(self.h, vertex as c_int) }; if v < 0 { None } else { Some(v as u32) } }
